@@ -8,8 +8,8 @@
 A "step" = one pass of the hot path over one batch of 32 synthetic images: FAIDetr.forward (normalise -> ResNet50-vd ->
 hybrid encoder -> 6-layer deformable decoder) + the fused DETR post-process kernel.
   value : whole-job images/s with inputs resident in HBM (CUDA-graph replay of the forward + post-process launch), in the PARITY-GREEN
-          mode `fp32_tc` (fp32 storage, three fp16 tcgen05 products per conv/linear: meets north_star's 1e-3 / identical keep-set bars,
-          tests/test_gpu_e2e.py, profiles/r02_error_budget.md).  The fp16 mode (one product; the reference's own CUDA numerics class, but
+          mode `fp32_tc` (fp32 storage, three fp16 wgmma products per conv/linear: meets north_star's 1e-3 / identical keep-set bars,
+          tests/test_gpu_e2e.py).  The fp16 mode (one product; the reference's own CUDA numerics class, but
           outside the bars) is reported beside it as `fast_mode`.
   e2e   : same metric through the public API (FocoosModel.stream / infer_async) from PINNED HOST uint8 images, H2D and D2H inside
           the timed region, two batches in flight
@@ -34,22 +34,6 @@ import torch  # noqa: E402
 
 METRIC = "images/sec fai-detr-l bs=32 640x640 inference"
 GFLOP_PER_IMG_USEFUL = 139.05  # SURVEY.md §8(d): excludes the dead mask_features conv
-IDEAL_US_PER_IMG_16BIT = 129.0  # SURVEY.md §8(d) sum-of-max roofline at 16-bit activations
-IDEAL_US_PER_IMG_FP32 = 259.0   # SURVEY.md §8(d): fp32 activations + half-rate (tf32-class) MMA
-
-
-def ncu_traffic(kernel_substr: str):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, read from the committed ncu capture of THIS round
-    (profiles/r02_ncu_dominant.csv, written by tools/ncu_extract.py from an `ncu --set full` report); None when no capture matches."""
-    import csv
-    path = os.path.join(ROOT, "profiles", "r02_ncu_dominant.csv")
-    if not os.path.exists(path):
-        return None, None
-    with open(path) as f:
-        for row in csv.DictReader(f):
-            if kernel_substr in row.get("kernel", ""):
-                return float(row["dram_bytes_read"]) + float(row["dram_bytes_write"]), os.path.relpath(path, ROOT)
-    return None, None
 
 
 def measured_peaks():
@@ -58,7 +42,7 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d["bf16_tflops_sustained"], "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "source": "fallback"}
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "source": "H100 SXM data sheet (dense fp16/bf16, 700 W), not measured"}
 
 
 def seeded_weights():
@@ -70,7 +54,7 @@ def seeded_weights():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -194,6 +178,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--quick", action="store_true", help="skip the bs=1 latency, parity-mode and other-config legs")
     ap.add_argument("--no-other-configs", action="store_true", help="skip the MaskFormer / BisenetFormer / fine-tune legs (separate processes)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (model logits / boxes, post-processed detections) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
@@ -201,7 +187,7 @@ def main():
     cores = os.cpu_count() or 1
     cpu_threads = min(cores, 32)  # torch CPU conv kernels stop scaling (and regress) beyond ~32 threads on this path
     config = {"workload": "fai-detr-l-obj365 bs=32/GPU 640x640 inference (BASELINE configs[1])", "per_gpu_batch": args.batch, "global_batch": args.batch * world,
-              "weights": "seeded random (focoos_b200.utils.seeded_weights, seed 0)", "parallelism": f"replicas x{world}", "l2_policy": "inputs_larger_than_L2 (each step streams >2 GB of activations + 88 MB of weights through the 126 MB L2; 39 MB uint8 input batch)"}
+              "weights": "seeded random (focoos_b200.utils.seeded_weights, seed 0)", "parallelism": f"replicas x{world}", "l2_policy": "inputs_larger_than_L2 (each step streams >2 GB of activations + 88 MB of weights through the 50 MB L2; 39 MB uint8 input batch)"}
     sd = seeded_weights()
 
     if args.impl == "reference":
@@ -240,7 +226,7 @@ def main():
 
     def step_device():
         out = fm.model(x_dev)
-        return ops.detr_postprocess(out.logits, out.boxes, sizes_dev, 300, 0.5)
+        return out, ops.detr_postprocess(out.logits, out.boxes, sizes_dev, 300, 0.5)
 
     # ---- warm-up (also builds the engine), then capture forward+post-process in a CUDA graph
     l0 = ops.launch_count()
@@ -263,8 +249,8 @@ def main():
     def run_step():
         if graph is not None:
             graph.replay()
-        else:
-            step_device()
+            return g_out
+        return step_device()
 
     for _ in range(max(args.warmup, 3)):
         run_step()
@@ -276,9 +262,16 @@ def main():
     with ClockSampler(local_rank) as clk:
         e0.record()
         for _ in range(args.steps):
-            run_step()
+            last = run_step()
         e1.record()
         torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        # the arrays the last timed step handed back (a graph replay writes them in place): the model logits / boxes (about 14 MB) in float32, the integer detections in float64
+        out, (d_scores, d_labels, d_boxes, d_query, d_count) = last
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        dumps = {"logits": out.logits, "boxes": out.boxes, "det_scores": d_scores, "det_labels": d_labels, "det_boxes": d_boxes, "det_query": d_query, "det_count": d_count}
+        for name, t in dumps.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.detach().cpu().numpy().astype(np.float32 if t.is_floating_point() else np.float64))
     ms_total = D.max_over_ranks(e0.elapsed_time(e1), dev)  # device time, max over ranks
     D.synchronize()
     ms_step = ms_total / args.steps
@@ -340,7 +333,7 @@ def main():
             return ops.detr_postprocess(o.logits, o.boxes, s1, 300, 0.5)
 
         lat = _latency(step1, not args.no_graph)
-        # ---- the fp16 mode (one tcgen05 product per conv/linear) on the same workload: faster, outside the parity bars
+        # ---- the fp16 mode (one wgmma product per conv/linear) on the same workload: faster, outside the parity bars
         if args.precision == "fp32_tc":
             m2 = FAIDetr(DETRConfig(), precision="fp16")
             m2.load_state_dict(sd, strict=True)
@@ -352,9 +345,8 @@ def main():
 
             ms2 = _throughput_ms(step2, not args.no_graph, max(5, args.steps // 2))
             fast = {"precision": "fp16", "value": B / (ms2 / 1e3), "unit": "images/s", "ms_per_step": ms2, "n_gpus": 1,
-                    "frac_of_ideal_16bit": (IDEAL_US_PER_IMG_16BIT * B / 1e3) / ms2,
                     "note": "fp16 storage, one product: the reference's own CUDA numerics class (fp16 autocast, focoos_model.py:604-609) but OUTSIDE north_star's bars (boxes 1.5e-3, "
-                            "298-299/300 queries, ~70% identical integer boxes: profiles/r02_error_budget.md); not the headline"}
+                            "not all queries or integer boxes identical); not the headline"}
             del m2
             torch.cuda.empty_cache()
 
@@ -389,17 +381,13 @@ def main():
         k_ms = r0.elapsed_time(r1) / nrep
         flops = 2.0 * B * 80 * 80 * 256 * 256 * 9
         ach = flops / (k_ms * 1e-3) / 1e12
-        traffic, traffic_src = ncu_traffic("conv_tc_kernel")
-        ideal_ms = (IDEAL_US_PER_IMG_FP32 if split else IDEAL_US_PER_IMG_16BIT) * B / 1e3
         roof = {"bound": "tensor", "kernel": "conv_tc_kernel on the 3x3 256->256 @80x80 conv (re-parameterised RepVGG block of the FPN CSPRepLayer; 3 launches/step at this shape, 16% of model FLOPs; "
-                                             "conv_tc_kernel as a family = 97% of FLOPs)" + (", fp32-accurate as THREE fp16 tcgen05 products" if split else ""),
+                                             "conv_tc_kernel as a family = 97% of FLOPs)" + (", fp32-accurate as THREE fp16 wgmma products" if split else ""),
                 "achieved": ach, "peak": peaks["tf_burst"], "unit": "TFLOP/s", "frac": ach / peaks["tf_burst"], "peak_source": peaks["source"] + " burst bf16 (kernel timed alone)",
-                "launch_ms": k_ms, "flops_per_launch": flops, "traffic": traffic, "traffic_source": traffic_src,
+                "launch_ms": k_ms, "flops_per_launch": flops,
                 "issued": {"tflops": ach * (3 if split else 1), "frac": ach * (3 if split else 1) / peaks["tf_burst"],
                            "note": "tensor-pipe work actually issued (3 products per algorithmic product in fp32_tc); `achieved`/`frac` count ALGORITHMIC flops only"},
-                "model": {"useful_gflop_per_img": GFLOP_PER_IMG_USEFUL, "achieved_tflops_whole_step": GFLOP_PER_IMG_USEFUL * B / ms_step,
-                          "ideal_ms_per_step": ideal_ms, "ideal_basis": "SURVEY 8(d) sum-of-max: " + ("fp32 activations + half-rate MMA (259 us/img)" if split else "16-bit activations (129 us/img)"),
-                          "frac_of_ideal": ideal_ms / ms_step}}
+                "model": {"useful_gflop_per_img": GFLOP_PER_IMG_USEFUL, "achieved_tflops_whole_step": GFLOP_PER_IMG_USEFUL * B / ms_step}}
         del xr, wr, yr
         torch.cuda.empty_cache()
 
@@ -456,9 +444,9 @@ def main():
             cpu = {"value": cv, "unit": "images/s", "cores": cpu_threads, "host_cores": cores, "kind": "port", "sample": "6 timed passes of batch 2 after 1 warm-up (oracle port of the reference's torch fp32 CPU forward + post-process)"}
         line = {"metric": METRIC, "value": value, "unit": "images/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_step,
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": {"fp16": "f16", "fp32": "f32", "fp32_tc": "f32 (storage and accumulation; every conv/linear product = 3 f16 tcgen05 products, error ~2^-21)"}[args.precision], "data": "synthetic",
-                "parity": {"fp32_tc": "meets north_star: identical query sets and (class, int box) keep-sets, boxes/scores < 1e-3 (tests/test_gpu_e2e.py::test_fp32_tc_meets_the_parity_bars, profiles/r02_error_budget.md)",
-                           "fp32": "meets north_star (CUDA-core fp32 mode)", "fp16": "outside north_star's bars (profiles/r02_error_budget.md)"}[args.precision],
+                "dtype": {"fp16": "f16", "fp32": "f32", "fp32_tc": "f32 (storage and accumulation; every conv/linear product = 3 f16 wgmma products, error ~2^-21)"}[args.precision], "data": "synthetic",
+                "parity": {"fp32_tc": "meets north_star: identical query sets and (class, int box) keep-sets, boxes/scores < 1e-3 (tests/test_gpu_e2e.py::test_fp32_tc_meets_the_parity_bars)",
+                           "fp32": "meets north_star (CUDA-core fp32 mode)", "fp16": "outside north_star's bars"}[args.precision],
                 "config": config, "clocks": clk.summary(), "e2e": e2e, "gpu_launches": launches_per_step * args.steps, "launches_per_step": launches_per_step,
                 "cuda_graph": graph is not None, "latency_bs1": lat, "fast_mode": fast, "other_configs": other, "train_config5": train, "roofline": roof, "cpu_baseline": cpu, "detections_img0": len(dets[0])}
         print(json.dumps(line))

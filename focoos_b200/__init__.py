@@ -1,4 +1,4 @@
-"""focoos_b200 — B200-native (sm_100a) implementation of the FocoosAI/focoos detection hot path."""
+"""focoos_b200 — H100-native (sm_90a) implementation of the FocoosAI/focoos detection hot path."""
 from .bisenetformer import BisenetFormer, BisenetFormerConfig  # noqa: F401
 from .fai_detr import FAIDetr  # noqa: F401
 from .fai_mf import FAIMaskFormer, MaskFormerConfig  # noqa: F401

@@ -14,8 +14,8 @@ H=1); weights stay in the reference's state_dict layout (OIHW / [N,K]) and are r
     AttentionFn       nn.MultiheadAttention core   softmax(QK^T s)V per head
     MSDAFn            ms_deform_attn_core_pytorch  (+ softmax over levels*points, sampling-location arithmetic)
 
-`conv_precision`: "fp32" = SIMT fp32 kernels; "fp32_tc" = tcgen05 split-precision products (fp32 storage) where the shape allows;
-"amp" = ONE tcgen05 product on fp16-rounded operands with fp32 accumulation and fp32 storage - the arithmetic class of the reference's own
+`conv_precision`: "fp32" = SIMT fp32 kernels; "fp32_tc" = wgmma split-precision products (fp32 storage) where the shape allows;
+"amp" = ONE wgmma product on fp16-rounded operands with fp32 accumulation and fp32 storage - the arithmetic class of the reference's own
 training (torch.autocast(fp16) + GradScaler, trainer/trainer.py:645,735-771), a third of the tensor work of "fp32_tc".
 """
 from __future__ import annotations
@@ -205,7 +205,7 @@ def _to_half_contiguous(t):
 
 
 def conv_any(x, w_khwc, bias, stride: int, pad: int, precision: str, act=ops.ACT_NONE, x_pair=None, return_pair=False):
-    """x NHWC fp32, w [Cout,KH,KW,Cin] fp32 -> NHWC fp32 through the SIMT fp32 or the split-precision tcgen05 kernel.
+    """x NHWC fp32, w [Cout,KH,KW,Cin] fp32 -> NHWC fp32 through the SIMT fp32 or the split-precision tensor-core kernel.
     x_pair: the [hi|lo] fp16 pair of x if the caller already has it; return_pair: also return the pair used (None on the SIMT path)."""
     B, H, W, C = x.shape
     Cout, KH, KW, _ = w_khwc.shape

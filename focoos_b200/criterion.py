@@ -1,4 +1,4 @@
-"""DETR training criterion on the B200 (SURVEY §8 a20), mirroring the reference classes:
+"""DETR training criterion on the GPU (SURVEY §8 a20), mirroring the reference classes:
 
   BoxHungarianMatcher   focoos/models/fai_detr/modelling.py:643-758  (cost on the GPU, assignment on the GPU instead of scipy on the CPU)
   SetCriterion          focoos/models/fai_detr/modelling.py:408-612  (losses "vfl" + "boxes", deep supervision over the aux outputs)

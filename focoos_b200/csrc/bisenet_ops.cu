@@ -8,7 +8,7 @@ namespace fb200 {
 
 static inline unsigned grid_cap2(int64_t total, int threads) {
   int64_t g = cdiv(total, threads);
-  const int64_t cap = 148LL * 32;
+  const int64_t cap = (int64_t)kNumSMs * 32;
   return (unsigned)(g < cap ? (g > 0 ? g : 1) : cap);
 }
 
@@ -263,7 +263,7 @@ extern "C" int fb200_channel_scale(const void* x, const void* gate, const void* 
 
 extern "C" int fb200_mask_argmax(const float* masks, const float* scores, int B, int Q, int64_t HW, uint8_t* labels, int* counts, void* stream) {
   FB_CHECK_ARG(masks && scores && labels && counts && Q >= 1 && Q <= 255, "mask_argmax: bad arguments (Q <= 255)");
-  dim3 grid((unsigned)std::min<int64_t>(cdiv((HW & 3) ? HW : HW / 4, 256), 148 * 4), (unsigned)B);
+  dim3 grid((unsigned)std::min<int64_t>(cdiv((HW & 3) ? HW : HW / 4, 256), kNumSMs * 4), (unsigned)B);
   mask_argmax_kernel<<<grid, 256, Q * 8, (cudaStream_t)stream>>>(masks, scores, Q, HW, labels, counts);
   FB_CHECK_LAUNCH("mask_argmax");
   return FB200_OK;

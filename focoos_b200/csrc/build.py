@@ -1,4 +1,4 @@
-"""Build libfocoos_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libfocoos_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m focoos_b200.csrc.build [--force]
 """
@@ -12,11 +12,12 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 SOURCES = ["conv_simt.cu", "conv_tc.cu", "pool_resize.cu", "norm_attn.cu", "msda.cu", "select.cu", "head_fused.cu", "mf_ops.cu", "bisenet_ops.cu", "criterion.cu", "optim.cu", "bwd_conv_norm.cu", "bwd_attn.cu", "wgrad_tc.cu"]
-HEADERS = ["common.cuh", os.path.join(ROOT, "include", "focoos_b200.h")]
+HEADERS = ["common.cuh", "wgmma.cuh", os.path.join(ROOT, "include", "focoos_b200.h")]
 LIB_DIR = os.path.join(os.path.dirname(HERE), "lib")
 LIB = os.path.join(LIB_DIR, "libfocoos_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-I", os.path.join(ROOT, "include"), "-I", HERE]
 
 
@@ -52,7 +53,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed for {src}:\n{out}")
         if verbose and out:
             print(out)
-    link = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    link = [NVCC, "-shared", "-o", LIB, *objs, *ARCH, "-lcudart"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout)

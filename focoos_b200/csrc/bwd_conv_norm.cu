@@ -148,7 +148,7 @@ __global__ void dilate2_kernel(const float* __restrict__ dy, int B, int Ho, int 
 // ------------------------------------------------------------------------------------------------------------------
 // column reductions over [R, C] (row pitch).  MODE 0: sum x   1: sum (x-mean)^2   2: BN backward (sum g, sum g*xhat)
 // partial[blockIdx.y][c] per row-slice; 32 channels x 8 row lanes per block.
-constexpr int CR_ROWS = 296;  // row slices (2 x 148 SMs)
+constexpr int CR_ROWS = 2 * kNumSMs;  // row slices (two per SM)
 
 __device__ __forceinline__ float act_grad(int act, float z, float y) {  // y = forward output where one exists, else pass z twice
   if (act == FB200_ACT_RELU) return y > 0.f ? 1.f : 0.f;
@@ -717,7 +717,7 @@ __global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float* __restr
   for (int i = threadIdx.x; i < C; i += blockDim.x) { pg[(int64_t)blockIdx.x * C + i] = ln_sm[i]; pb[(int64_t)blockIdx.x * C + i] = ln_sm[C + i]; }
 }
 
-inline unsigned grid_for(int64_t n, int threads = 256) { return (unsigned)std::min<int64_t>(cdiv(n, threads), 148 * 16); }
+inline unsigned grid_for(int64_t n, int threads = 256) { return (unsigned)std::min<int64_t>(cdiv(n, threads), kNumSMs * 16); }
 
 }  // namespace
 }  // namespace fb200
@@ -727,8 +727,8 @@ using namespace fb200;
 extern "C" int64_t fb200_conv_wgrad_workspace_bytes(int B, int Ho, int Wo, int Cin, int Cout, int KH, int KW) {
   const int64_t tiles = (int64_t)cdiv(Cout, WG_TM) * cdiv(Cin, WG_TN) * KH * KW;
   const int64_t P = (int64_t)B * Ho * Wo;
-  int64_t splits = std::max<int64_t>(1, std::min<int64_t>(cdiv(148 * 4, tiles), cdiv(P, 512)));
-  splits = std::max<int64_t>(splits, 296);  // the stem kernel writes one partial per block (<= 296 blocks)
+  int64_t splits = std::max<int64_t>(1, std::min<int64_t>(cdiv(kNumSMs * 4, tiles), cdiv(P, 512)));
+  splits = std::max<int64_t>(splits, 2 * kNumSMs);  // the stem kernel writes one partial per block (<= 2 per SM)
   return splits * Cout * KH * KW * Cin * 4 + 16;
 }
 
@@ -737,9 +737,9 @@ extern "C" int fb200_conv_wgrad(const float* x, int B, int H, int W, int Cin, in
   FB_CHECK_ARG(x && dy && dw && workspace, "conv_wgrad: null pointer");
   FB_CHECK_ARG(B > 0 && Cin > 0 && Cout > 0 && KH > 0 && KW > 0 && stride >= 1, "conv_wgrad: bad sizes");
   FB_CHECK_ARG(Ho == (H + 2 * pad - KH) / stride + 1 && Wo == (W + 2 * pad - KW) / stride + 1, "conv_wgrad: output size does not match");
-  if (KH == 3 && KW == 3 && stride == 2 && pad == 1 && Cin <= 4 && Cout == 32 && 296LL * 32 * 9 * Cin * 4 + 16 <= fb200_conv_wgrad_workspace_bytes(B, Ho, Wo, Cin, Cout, KH, KW)) {
+  if (KH == 3 && KW == 3 && stride == 2 && pad == 1 && Cin <= 4 && Cout == 32 && 2LL * kNumSMs * 32 * 9 * Cin * 4 + 16 <= fb200_conv_wgrad_workspace_bytes(B, Ho, Wo, Cin, Cout, KH, KW)) {
     const int tiles_w = (int)cdiv(Wo, SW_TW), tiles_h = (int)cdiv(Ho, SW_TH);
-    const int nblk = (int)std::min<int64_t>(296, (int64_t)B * tiles_w * tiles_h);
+    const int nblk = (int)std::min<int64_t>(2 * kNumSMs, (int64_t)B * tiles_w * tiles_h);
     cudaStream_t st0 = (cudaStream_t)stream;
     conv_wgrad_stem_kernel<<<nblk, 256, 0, st0>>>(x, x_pitch, dy, dy_pitch, B, H, W, Cin, Ho, Wo, tiles_w, tiles_h, reinterpret_cast<float*>(workspace));
     FB_CHECK_LAUNCH("conv_wgrad(stem)");
@@ -750,7 +750,7 @@ extern "C" int fb200_conv_wgrad(const float* x, int B, int H, int W, int Cin, in
   }
   const int64_t tiles = (int64_t)cdiv(Cout, WG_TM) * cdiv(Cin, WG_TN);
   const int64_t P = (int64_t)B * Ho * Wo;
-  const int64_t splits = std::max<int64_t>(1, std::min<int64_t>(cdiv(148 * 4, tiles * KH * KW), cdiv(P, 512)));
+  const int64_t splits = std::max<int64_t>(1, std::min<int64_t>(cdiv(kNumSMs * 4, tiles * KH * KW), cdiv(P, 512)));
   const int64_t per = cdiv(cdiv(P, splits), WG_TK) * WG_TK;
   float* part = reinterpret_cast<float*>(workspace);
   cudaStream_t st = (cudaStream_t)stream;
@@ -786,7 +786,7 @@ static inline unsigned cf_grid(int64_t R, int C) {
   if (on < 0) { const char* e = getenv("FB200_BN_CF"); on = e ? atoi(e) : 1; }
   const int cv = C / 4;
   if (!on || C % 4 || cv <= 0) return 0;
-  int64_t blocks = std::min<int64_t>(cdiv(R * cv, 256), 148 * 16);
+  int64_t blocks = std::min<int64_t>(cdiv(R * cv, 256), kNumSMs * 16);
   if (cv <= 256) { if (256 % cv) return 0; }           // every block holds whole rows' worth of column groups
   else { if (cv % 256) return 0; const int64_t m = cv / 256; blocks = blocks / m * m; }
   return (unsigned)std::max<int64_t>(blocks, cv > 256 ? cv / 256 : 1);

@@ -1,4 +1,4 @@
-// Shared helpers for the focoos_b200 CUDA kernels (sm_100a only).
+// Shared helpers for the focoos_b200 CUDA kernels (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -81,7 +81,7 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
-// shared by conv_simt.cu (SIMT path) and conv_tc.cu (tcgen05 path)
+// shared by conv_simt.cu (SIMT path) and conv_tc.cu (tensor-core path)
 struct ConvParams {
   const void* x; const void* w; const float* scale; const float* bias; const void* res; void* out;
   int B, H, W, Cin, x_pitch, KH, KW, stride, pad, Ho, Wo, Cout, res_pitch, out_pitch, act;
@@ -93,6 +93,9 @@ struct ConvParams {
 };
 
 static inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// SMs of the target GPU (H100 SXM): sizes grid-stride caps and split counts; kernels stay correct on any SM count
+constexpr int kNumSMs = 132;
 
 // dispatch helper on activation dtype
 #define FB_DISPATCH_DTYPE(dt, T, ...)                         \

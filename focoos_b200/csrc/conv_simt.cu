@@ -2,7 +2,7 @@
 //   * fb200_stem_conv3x3s2 — normalise + 3x3/s2 conv + BN + act straight from the NCHW fp32 image.
 //   * conv_igemm_simt      — generic implicit-GEMM conv / linear with fused scale/bias/residual/act
 //                            epilogue.  This is the fp32 parity path and the fall-back for shapes the
-//                            tcgen05 kernel (conv_tc.cu) does not take (Cin % 64 != 0, fp32 activations).
+//                            tensor-core kernel (conv_tc.cu) does not take (Cin % 64 != 0, fp32 activations).
 #include <stdarg.h>
 
 #include "common.cuh"
@@ -481,21 +481,11 @@ using namespace fb200;
 
 extern "C" const char* fb200_last_error(void) { return fb200::g_err; }
 extern "C" int fb200_version(void) { return 100; }
-namespace fb200 { int conv_tc_set_pair_mode(int v); void conv_tc_set_trace(void* buf); }  // conv_tc.cu
-extern "C" int fb200_set_conv_trace(void* device_buf) {
-  conv_tc_set_trace(device_buf);
-  return FB200_OK;
-}
-extern "C" int fb200_set_option(int option, int value) {
-  if (option == FB200_OPT_CONV_CTA_PAIR && value >= 0 && value <= 2) return conv_tc_set_pair_mode(value);
-  set_error("set_option: unknown option %d / value %d", option, value);
-  return FB200_ERR_INVALID;
-}
 extern "C" int fb200_device_supports_tcgen05(void) {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return FB200_ERR_CUDA;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return FB200_ERR_CUDA;
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }
 
 static int stem_launch(const void* img, bool u8, int B, int H, int W, const float* w, const float* scale, const float* bias, const float* mean3,
@@ -554,7 +544,7 @@ extern "C" int fb200_linear_rowmax_pair(const void* x, int64_t M, int K, int x_p
   p.x_lo_off = x_lo_off;
   p.rowmax = rowmax;
   if (!conv2d_tc_supported(p, FB200_F16, FB200_F32)) {
-    set_error("linear_rowmax_pair: shape not supported by the tcgen05 split path (K=%d)", K);
+    set_error("linear_rowmax_pair: shape not supported by the tensor-core split path (K=%d)", K);
     return FB200_ERR_UNSUPPORTED;
   }
   return conv2d_tc(p, (cudaStream_t)stream);
@@ -599,7 +589,7 @@ extern "C" int fb200_conv2d_pair(const void* x, int B, int H, int W, int C, int 
   p.out_bs = out_batch_stride > 0 ? out_batch_stride : (int64_t)p.Ho * p.Wo * out_pitch;
   p.x_lo_off = x_lo_off; p.out_lo_off = out_lo_off; p.res_lo_off = res_lo_off;
   if (!conv2d_tc_supported(p, FB200_F16, out_dtype)) {
-    set_error("conv2d_pair: shape / alignment not supported by the tcgen05 split path (C=%d Cout=%d k=%dx%d s=%d out_dtype=%d)", C, Cout, KH, KW, stride, out_dtype);
+    set_error("conv2d_pair: shape / alignment not supported by the tensor-core split path (C=%d Cout=%d k=%dx%d s=%d out_dtype=%d)", C, Cout, KH, KW, stride, out_dtype);
     return FB200_ERR_UNSUPPORTED;
   }
   return conv2d_tc(p, (cudaStream_t)stream);
@@ -617,7 +607,7 @@ extern "C" int fb200_linear_rowmax(const void* x, int64_t M, int K, int x_pitch,
   p.out_bs = (int64_t)M * p.out_pitch;
   p.rowmax = rowmax;
   if (!conv2d_tc_supported(p, FB200_F16, FB200_F32)) {
-    set_error("linear_rowmax: shape not supported by the tcgen05 path (K=%d must be a multiple of 32, fp16 operands, 16-byte aligned)", K);
+    set_error("linear_rowmax: shape not supported by the tensor-core path (K=%d must be a multiple of 32, fp16 operands, 16-byte aligned)", K);
     return FB200_ERR_UNSUPPORTED;
   }
   return conv2d_tc(p, (cudaStream_t)stream);
@@ -651,7 +641,7 @@ static int conv2d_impl(const void* x, int x_dtype, int B, int H, int W, int Cin,
   p.w_bs = w_bs;
   const bool tc_ok = conv2d_tc_supported(p, x_dtype, out_dtype);
   if (algo == FB200_ALGO_TCGEN05 && !tc_ok) {
-    set_error("conv2d: tcgen05 path does not support this shape/dtype (Cin=%d Cout=%d k=%dx%d s=%d dtype=%d/%d)", Cin, Cout, KH, KW, stride, x_dtype, out_dtype);
+    set_error("conv2d: tensor-core path does not support this shape/dtype (Cin=%d Cout=%d k=%dx%d s=%d dtype=%d/%d)", Cin, Cout, KH, KW, stride, x_dtype, out_dtype);
     return FB200_ERR_UNSUPPORTED;
   }
   if ((algo == FB200_ALGO_AUTO && tc_ok) || algo == FB200_ALGO_TCGEN05) return conv2d_tc(p, st);

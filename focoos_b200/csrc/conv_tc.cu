@@ -1,24 +1,23 @@
-// tcgen05 implicit-GEMM convolution / linear for sm_100a  (fp16 operands, fp32 accumulate in TMEM).
+// wgmma implicit-GEMM convolution / linear for sm_90a  (fp16 operands, fp32 accumulate in registers).
 //
 //   D[m, n] = act( (sum_k A[m,k] * W[n,k]) * scale[n] + bias[n] + residual[m,n] )
 //   m = output pixel (b, ho, wo), n = output channel, k = (kh, kw, c).
 //
-// Design: PERSISTENT, warp-specialised CTAs (grid = #SMs x CTAs/SM); each CTA walks 128 x BLOCK_N output tiles
+// Design: PERSISTENT, warp-specialised CTAs (grid = #SMs); each CTA walks 128 x BLOCK_N output tiles
 // (N tiles fastest so CTAs that share an A tile run together and A comes from L2).
-//   warp 0   TMA producer.  A is never materialised as im2col: an M-tile is a BW x BH rectangle of output
-//            pixels of one image, and the A block for filter tap (kh,kw), channel chunk c0 is the SAME
-//            rectangle of the NHWC input shifted by (kh-pad, kw-pad) — one 4-D tiled TMA load whose
-//            out-of-bounds rows/columns (the conv zero padding, and ragged tile edges) are zero-filled by the
-//            TMA unit.  Stride-2 3x3 convs use a 5-D view (c', w/2, h&1, h/2, b) of the same tensor so that
-//            every tap is again a dense box.  1x1 convs and linears are the degenerate W = M, H = 1 case.
-//            Smem tiles land in the canonical K-major SWIZZLE_128B (or _64B for Cin = 32) layout tcgen05 wants.
-//   warp 1   MMA issuer: one elected lane issues BLOCK_K/16 x tcgen05.mma (128 x BLOCK_N x 16) per k-block into
-//            one of TWO TMEM accumulator stages; tcgen05.commit releases the smem stage / signals the epilogue.
-//   warp 2   TMEM allocator (2 x BLOCK_N columns).
-//   warps 4-7 epilogue, overlapped with the next tile's main loop: tcgen05.ld 32 columns at a time -> folded-BN
-//            scale/bias, residual (before or after the activation), ReLU/SiLU/GELU (switch hoisted out of the
-//            element loops — a per-element switch made the first version I-cache bound, profiles/r01_trip3) ->
-//            fp16/fp32 -> swizzled smem staging (double buffered) -> TMA store (clips ragged tiles / Cout tails).
+//   warp-group 0   TMA producer (one thread).  A is never materialised as im2col: an M-tile is a BW x BH rectangle of output
+//                  pixels of one image, and the A block for filter tap (kh,kw), channel chunk c0 is the SAME rectangle of the
+//                  NHWC input shifted by (kh-pad, kw-pad) — one 4-D tiled TMA load whose out-of-bounds rows/columns (the conv zero
+//                  padding, and ragged tile edges) are zero-filled by the TMA unit.  Stride-2 convs use a 5-D view
+//                  (c', w/2, h&1, h/2, b) of the same tensor so that every tap is again a dense box.  1x1 convs and linears are the
+//                  degenerate W = M, H = 1 case.  Smem tiles land in the canonical K-major SWIZZLE_128B (or _64B for 32-channel
+//                  chunks) layout wgmma reads through its shared-memory descriptors.
+//   warp-groups 1-2  consumers: group g owns tile rows 64g..64g+63.  Per k-block it issues BLOCK_K/16 x wgmma.m64nBLOCK_Nk16
+//                  (three per step in the fp32-accurate fused-split mode) into its register accumulator and releases the ring stage
+//                  one k-block later (wgmma.wait_group 1).  The epilogue of its rows follows: folded-BN scale/bias, residual (before
+//                  or after the activation), ReLU/SiLU/GELU -> fp16/fp32/pair -> swizzled smem staging (double buffered, shared by
+//                  both groups) -> TMA store (clips ragged tiles / Cout tails).  The producer keeps filling the ring with the next
+//                  tile's operands meanwhile.
 //
 // Algorithmic bytes: A (M x Cin, each input pixel counted once), W, D (+ residual) once each.
 #include <cuda.h>
@@ -27,30 +26,16 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace fb200 {
 
 namespace tc {
 
-// The debug timeline (fb200_set_conv_trace) and the experiment knobs (FB200_TC_DBG) are compiled in by default; -DFB200_TC_NO_TRACE / -DFB200_TC_NO_DBG strip them
-// (A/B builds: tools/ab_lib.py)
-#ifdef FB200_TC_NO_TRACE
-constexpr bool kTrace = false;
-#else
-constexpr bool kTrace = true;
-#endif
-#ifdef FB200_TC_NO_DBG
-constexpr bool kDbg = false;
-#else
-constexpr bool kDbg = true;
-#endif
-
 constexpr int BLOCK_M = 128;
 constexpr int STAGING_BYTES = BLOCK_M * 128;  // one staging tile: 128 rows x 128 B
-constexpr int PRODUCER_THREADS = 128;  // warps 0-3: TMA, MMA, TMEM alloc, spare
-// epilogue warp-groups (128 threads each): BLOCK_N >= 128 -> two groups, each owning half of the tile's columns
-template <int BLOCK_N> __host__ __device__ constexpr int epi_groups() { return BLOCK_N >= 128 ? 2 : 1; }
-template <int BLOCK_N> __host__ __device__ constexpr int num_threads() { return PRODUCER_THREADS + 128 * epi_groups<BLOCK_N>(); }
+constexpr int NUM_THREADS = 384;              // producer warp-group + two consumer warp-groups
+constexpr int CONSUMER_WARPS = 8;
 
 // Output / residual stored as the fp16 [hi | lo] PAIR of the fp32 value (hi = fp16(v), lo = fp16(v - hi)): the operand format of the fp32-accurate convs,
 // written straight from the epilogue so that no separate split pass runs between two convs.  sizeof == 4: a staging chunk is 32 columns like fp32, laid out as
@@ -61,24 +46,18 @@ template <> struct is_pair<PairOut> { static constexpr bool value = true; };
 
 struct KParams {
   const float* scale; const float* bias; const void* res;
-  int res_pitch, act, Cout;
-  int KH, KW, pad, cchunks;        // cchunks = Cin / BLOCK_K (3C/BLOCK_K in split-precision mode)
-  int seg_chunks, lo_off;          // split-precision: chunks per K segment (C/BLOCK_K) and channel offset of the A operand's lo half (C unless the input is a channel slice of a wider pair buffer); 0 = off
+  int act, Cout;
+  int KH, KW, pad, cchunks;        // cchunks = Cin / BLOCK_K (segmented split-precision: 3C / BLOCK_K; fused split: C / BLOCK_K)
+  int seg_chunks, lo_off;          // split-precision: chunks per K segment (C/BLOCK_K, 0 = off) and channel offset of the A operand's lo half (C unless the input is a channel slice of a wider pair buffer)
   int w_seg;                       // split-precision: channels per weight segment ([W_hi | W_lo | W_hi] per tap)
   int BW, BH, tiles_w, tiles_h;    // output tile rectangle and tile counts per image
-  int Ho, Wo;                      // output spatial size (residual addressing / validity)
+  int Ho, Wo;                      // output spatial size (validity of rows)
   int x_pitch;                     // stride-2 view only (c' = wp * pitch + c)
   int stride2;                     // 0: 4-D stride-1 view, 1: 5-D stride-2 view
   int num_k_blocks;
   int n_tiles, total_tiles;        // N tiles per M tile; total = m_tiles * n_tiles
-  int res_tma;                     // 1: the residual tile is TMA-loaded into the staging buffer (coalesced, one chunk ahead) instead of per-thread LDG
-  int halo_boff;                   // halo mode: also set the descriptor base-offset field (A/B experiment knob FB200_TC_HALO=2)
   float* rowmax;                   // not null: row-max-only epilogue (query selection scores), nothing is stored
   int w_batched;                   // 1: weights differ per image (3-D weight map, third coordinate = image)
-  int dbg;                         // tuning aid (env FB200_TC_DBG): 1 = skip TMA store, 2 = skip residual, 4 = skip TMEM load
-  unsigned long long* trace;       // debug timeline (fb200_set_conv_trace): 128 clock64 slots per CTA, see tools/conv_trace.py
-  int nimg;                        // images in the (possibly flattened) view: M tiles beyond it are phantoms of an odd CTA-pair count
-  int ncat;                        // fused split with BLOCK_N <= 128: A_hi x [W_hi | W_lo] as ONE MMA of N = 2 * BLOCK_N (see NCAT in conv_tc_kernel)
 };
 
 // ---------------------------------------------------------------------------------------------- PTX
@@ -110,9 +89,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void epi_bar(int grp) { asm volatile("bar.sync %0, 128;" ::"r"(grp + 1) : "memory"); }
+__device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -145,105 +122,24 @@ __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk
 template <int N> __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- CTA-pair (cta_group::2) variants: the two CTAs of a cluster compute ONE 256 x BLOCK_N tile; each loads its own 128 A rows and HALF of the B tile,
-// the leader (cluster rank 0) issues the MMAs for both, commits are multicast to both CTAs' barriers
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t mapa_rank0(uint32_t addr) {  // the same shared-memory offset in the leader CTA (shared::cluster window)
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(0));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads of a CTA pair: data lands in the EXECUTING CTA's shared memory, the transaction bytes are counted on the LEADER's barrier
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* map, uint32_t bar_cluster, void* dst, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(const CUtensorMap* map, uint32_t bar_cluster, void* dst, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(const CUtensorMap* map, uint32_t bar_cluster, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_2sm(const CUtensorMap* map, uint32_t bar_cluster, void* dst, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-
-// K-major swizzled shared-memory matrix descriptor (sm_100 format: version 1 at bit 46, layout type at bits 61-63)
+// K-major swizzled shared-memory matrix descriptor (sm_90 format: layout type at bits 62-63, 1 = SWIZZLE_128B, 2 = SWIZZLE_64B)
 template <int BLOCK_K>
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address, 16-byte units
   d |= (uint64_t)1 << 16;                         // leading byte offset (unused for swizzled K-major) = 1
   d |= (uint64_t)((8 * BLOCK_K * 2) >> 4) << 32;  // stride byte offset: 8 rows x (BLOCK_K*2) B
-  d |= (uint64_t)1 << 46;                         // descriptor version (Blackwell)
-  d |= (uint64_t)(BLOCK_K == 64 ? 2 : 4) << 61;   // SWIZZLE_128B (2) / SWIZZLE_64B (4)
+  d |= (uint64_t)(BLOCK_K == 64 ? 1 : 2) << 62;
   return d;
 }
-// instruction descriptor: D=F32, A=B=F16, both K-major, M=128, N=BLOCK_N
-__host__ __device__ constexpr uint32_t make_idesc(int n, int m = 128) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {  // arrives on the barrier at this offset in BOTH CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
-// activation on 32 values with the switch OUTSIDE the element loop (uniform branch, lean straight-line bodies)
 template <bool GELU>
-__device__ __forceinline__ void act32(float (&v)[32], int act) {
-  if constexpr (GELU) {  // exact-erf GELU (AIFI FFN only) lives in its own kernel instantiation: ~50 instructions / element
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = 0.5f * v[j] * (1.f + erff(v[j] * 0.70710678118654752440f));
-    return;
-  }
+__device__ __forceinline__ float act1(float v, int act) {
+  if constexpr (GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f));  // exact-erf GELU (AIFI FFN only): its own instantiation
   switch (act & 15) {
-    case FB200_ACT_RELU:
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-      break;
-    case FB200_ACT_SILU:
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __fdividef(v[j], 1.f + __expf(-v[j]));
-      break;
-    default: break;
+    case FB200_ACT_RELU: return fmaxf(v, 0.f);
+    case FB200_ACT_SILU: return __fdividef(v, 1.f + __expf(-v));
+    default: return v;
   }
 }
 
@@ -253,644 +149,272 @@ __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
   else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
-// BLOCK_K == 96 selects the HALO mode for 32-channel 3x3 stride-1 convs (the ResNet-vd stem): an M tile is 128 consecutive pixels of ONE image row, a
-// k-block is one filter ROW (kh): the (128 + 2) x 32-channel input strip is loaded ONCE and the three kw taps are three UMMA descriptors whose start
-// address is shifted by one 64-byte pixel row each - the tap boxes are no longer re-read from L2 three times (these layers run at the L2 bandwidth).
-template <int BLOCK_K> __host__ __device__ constexpr bool is_halo() { return BLOCK_K == 96; }
-template <int BLOCK_K> __host__ __device__ constexpr int phys_k() { return BLOCK_K == 96 ? 32 : BLOCK_K; }  // channels per shared-memory row
-// FS ("fused split", fp32-accurate mode): one ring stage holds the hi AND lo halves of both operands of a 64-channel chunk - A_hi, A_lo, B_hi, B_lo are loaded ONCE
-// and feed the three products hi x W_hi, hi x W_lo, lo x W_hi (the segmented layout streams every operand tile through the TMA engine / L2 three times)
-template <int BLOCK_N, int BLOCK_K, bool FS = false> __host__ __device__ constexpr int a_stage_bytes() { return BLOCK_K == 96 ? (FS ? 2 : 1) * 9216 : (FS ? 2 : 1) * BLOCK_M * BLOCK_K * 2; }  // halo: 130 rows x 64 B, 1 KiB aligned
-template <int BLOCK_N, int BLOCK_K, bool CTA2 = false, bool FS = false> __host__ __device__ constexpr int b_stage_bytes() { return BLOCK_K == 96 ? 0 : (FS ? 2 : 1) * (CTA2 ? BLOCK_N / 2 : BLOCK_N) * BLOCK_K * 2; }
-// halo mode keeps ALL NINE weight taps resident in shared memory for the life of the persistent CTA (9 x BLOCK_N x 64 B <= 36 KiB): per tile only the
-// three input strips travel from L2
-template <int BLOCK_N, int BLOCK_K, bool FS = false> __host__ __device__ constexpr int b_resident_bytes() { return BLOCK_K == 96 ? (FS ? 18 : 9) * BLOCK_N * 64 : 0; }  // FS: W_hi and W_lo of every tap
-template <int BLOCK_N, int BLOCK_K, bool CTA2 = false, bool FS = false> constexpr int stage_bytes() { return a_stage_bytes<BLOCK_N, BLOCK_K, FS>() + b_stage_bytes<BLOCK_N, BLOCK_K, CTA2, FS>(); }
-template <int BLOCK_N, int STAGES, int BLOCK_K, int NSTG, bool CTA2 = false, bool FS = false> constexpr int smem_bytes() {
-  return STAGES * stage_bytes<BLOCK_N, BLOCK_K, CTA2, FS>() + b_resident_bytes<BLOCK_N, BLOCK_K, FS>() + NSTG * epi_groups<BLOCK_N>() * STAGING_BYTES + 2 * BLOCK_N * 4 +
-         (2 * STAGES + 5 + NSTG * epi_groups<BLOCK_N>()) * 8 + 16 + (FS ? 0 : 1024) /*align slack; the FS configurations need every byte and rely on the 1024-byte alignment of dynamic shared memory (checked in the kernel)*/;
+// FS ("fused split", fp32-accurate mode): one ring stage holds the hi AND lo halves of both operands of a channel chunk - A_hi, A_lo, B_hi, B_lo are loaded ONCE
+// and feed the three products hi x W_hi, hi x W_lo, lo x W_hi
+template <int BLOCK_K, bool FS> __host__ __device__ constexpr int a_stage_bytes() { return (FS ? 2 : 1) * BLOCK_M * BLOCK_K * 2; }
+template <int BLOCK_N, int BLOCK_K, bool FS> __host__ __device__ constexpr int b_stage_bytes() { return (FS ? 2 : 1) * BLOCK_N * BLOCK_K * 2; }
+template <int BLOCK_N, int STAGES, int BLOCK_K, int NSTG, bool FS> constexpr int smem_bytes() {
+  return STAGES * (a_stage_bytes<BLOCK_K, FS>() + b_stage_bytes<BLOCK_N, BLOCK_K, FS>()) + NSTG * STAGING_BYTES + (2 * STAGES + 1) * 8 + 1024 /*align slack*/;
 }
 
 // ---------------------------------------------------------------------------------------------- kernel
-template <int BLOCK_N, int STAGES, typename TOut, int MIN_BLOCKS, int BLOCK_K, int NSTG, bool GELU, bool CTA2, bool FS>
-__global__ void __launch_bounds__(num_threads<BLOCK_N>(), MIN_BLOCKS)
+template <int BLOCK_N, int STAGES, typename TOut, int BLOCK_K, int NSTG, bool GELU, bool FS>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_r,
                const __grid_constant__ CUtensorMap tmap_d2, const __grid_constant__ CUtensorMap tmap_r2, const KParams p) {
   constexpr bool PAIR = is_pair<TOut>::value;  // tmap_d2 / tmap_r2: the lo planes of the output / residual (pair format only)
+  static_assert(BLOCK_K == 32 || BLOCK_K == 64, "one swizzle row per channel chunk");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  if constexpr (FS) { if (smem != smem_raw) __trap(); }  // no alignment slack in the FS configurations
-  constexpr bool HALO = is_halo<BLOCK_K>();
-  constexpr int BKP = phys_k<BLOCK_K>();
-  constexpr int A_STAGE_BYTES = a_stage_bytes<BLOCK_N, BLOCK_K, FS>();
-  constexpr int B_STAGE_BYTES = b_stage_bytes<BLOCK_N, BLOCK_K, CTA2, FS>();
-  static_assert(!(CTA2 && HALO), "the halo mode is single-CTA");
-  static_assert(!(FS && !HALO && BLOCK_K != 64), "the fused-split mode works on 64-channel chunks (or on the 32-channel halo strips)");
-  constexpr int A_HALF = BLOCK_M * 64 * 2;                                  // FS: bytes of one A half (hi or lo) inside a stage
-  constexpr int B_HALF = (CTA2 ? BLOCK_N / 2 : BLOCK_N) * 64 * 2;           // FS: bytes of one B half
-  uint32_t cta_rank = 0;  // CTA pair: 0 = leader (issues the MMAs), 1 = peer
-  if constexpr (CTA2) cta_rank = cluster_ctarank();
-  // persistent tile walk: a CTA pair shares one tile index (two adjacent M tiles x one N tile)
-  const int t_first = CTA2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int t_stride = CTA2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  constexpr int A_STAGE_BYTES = a_stage_bytes<BLOCK_K, FS>();
+  constexpr int B_STAGE_BYTES = b_stage_bytes<BLOCK_N, BLOCK_K, FS>();
+  constexpr int A_HALF = BLOCK_M * BLOCK_K * 2;   // FS: bytes of one A half (hi or lo) inside a stage
+  constexpr int B_HALF = BLOCK_N * BLOCK_K * 2;   // FS: bytes of one B half
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  constexpr int EPI_GROUPS = epi_groups<BLOCK_N>();
-  uint8_t* smem_w = smem_b + STAGES * B_STAGE_BYTES;   // halo mode: the nine resident weight taps
-  uint8_t* staging = smem_w + b_resident_bytes<BLOCK_N, BLOCK_K, FS>();  // EPI_GROUPS x NSTG x 16 KiB
-  float* s_scale = reinterpret_cast<float*>(staging + EPI_GROUPS * NSTG * STAGING_BYTES);
-  float* s_bias = s_scale + BLOCK_N;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_bias + BLOCK_N);
+  uint8_t* staging = smem_b + STAGES * B_STAGE_BYTES;  // NSTG x 16 KiB
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + NSTG * STAGING_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;   // [2]
-  uint64_t* res_bar = tmem_empty_bar + 2;         // [EPI_GROUPS * NSTG] residual tile landed in staging buffer
-  uint64_t* w_bar = res_bar + EPI_GROUPS * NSTG;  // halo mode: resident weights landed
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(w_bar + 1);
+  uint64_t* res_bar = empty_bar + STAGES;  // residual chunk landed in the staging buffer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // N-concatenated split products: a tcgen05.mma with both operands in shared memory costs ~128 cycles for its 128 x 16 A slice whatever N is
-  // (profiles/r02_conv_timeline.md), so with BLOCK_N <= 128 the products A_hi x W_hi and A_hi x W_lo are issued as ONE MMA against the adjacent [W_hi | W_lo] rows
-  // (N = 2 * BLOCK_N, accumulator columns [0, 2 * BLOCK_N)); A_lo x W_hi accumulates into columns [0, BLOCK_N) and the epilogue adds the two halves: two MMAs per
-  // 16-channel step instead of three.  Enabled per launch by p.ncat.
-  constexpr bool NCAT_OK = FS && !CTA2 && BLOCK_N <= 128;
-  constexpr int ACC_COLS = NCAT_OK ? 2 * BLOCK_N : BLOCK_N;  // TMEM columns of one accumulator stage
-  constexpr uint32_t TMEM_COLS = (2 * ACC_COLS) < 32 ? 32 : (2 * ACC_COLS);  // two accumulator stages
-  const bool ncat = NCAT_OK && p.ncat;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_d) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full_bar[i], 1); mbar_init(&tmem_empty_bar[i], (CTA2 ? 8 : 4) * EPI_GROUPS); }  // pair: both CTAs' epilogue warps release the leader's accumulator stage
-    for (int i = 0; i < EPI_GROUPS * NSTG; ++i) mbar_init(&res_bar[i], 1);
-    mbar_init(w_bar, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], CONSUMER_WARPS); }
+    mbar_init(res_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (CTA2) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  if constexpr (CTA2) cluster_sync_all();  // the peer's barriers are initialised before any remote arrive / complete_tx can reach them
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  // Programmatic dependent launch (host side: launch(), FB200_TC_PDL): this grid may have been started while the previous kernel of the stream was still draining its
-  // last tiles - everything above (tensor-map prefetch, barrier init, TMEM allocation, cluster handshake) touched no global data.  Let OUR dependents start the same
-  // way, then wait until the prerequisite grid has completed and its writes are visible before any role reads activations / residuals or writes outputs.
-  // Both instructions are no-ops for a launch without the attribute.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
   const int tiles_per_img = p.tiles_w * p.tiles_h;
-  // debug timeline: slot 0 = kernel entry of this CTA (globaltimer ns), 1 = setup done (clock64); per tile k < 20: 2+6k = accumulator stage free,
-  // 3+6k = first operands landed, 4+6k = last MMA issued (MMA thread); 5+6k = accumulator complete seen, 6+6k = tile stored (epilogue group 0); 7+6k = producer tile start
-  unsigned long long* const trc = (kTrace && p.trace) ? p.trace + (size_t)blockIdx.x * 128 : nullptr;
-  const int dbgv = kDbg ? p.dbg : 0;
-  auto stamp = [&](int slot) { if (trc && slot < 128) trc[slot] = (unsigned long long)clock64(); };
-  if (trc && threadIdx.x == 0) { unsigned long long g; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g)); trc[0] = g; trc[1] = (unsigned long long)clock64(); }
-  struct TileXY { int n0, mt, img, h0, w0; };
+  struct TileXY { int n0, img, h0, w0; };
   auto tile_of = [&](int t) {
     TileXY r;
     r.n0 = (t % p.n_tiles) * BLOCK_N;
-    r.mt = t / p.n_tiles;
-    if constexpr (CTA2) r.mt = r.mt * 2 + (int)cta_rank;
-    r.img = r.mt / tiles_per_img;
-    const int rem = r.mt - r.img * tiles_per_img;
+    const int mt = t / p.n_tiles;
+    r.img = mt / tiles_per_img;
+    const int rem = mt - r.img * tiles_per_img;
     r.h0 = (rem / p.tiles_w) * p.BH;
     r.w0 = (rem % p.tiles_w) * p.BW;
     return r;
   };
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================================================================== TMA producer
-    if (lane == 0) {
-      const uint32_t tx_bytes = HALO ? (uint32_t)((FS ? 2 : 1) * (p.BW + 2) * 64) : (uint32_t)(p.BW * p.BH * BKP * 2) + (uint32_t)B_STAGE_BYTES;
-      if constexpr (HALO) {  // the nine weight taps, once (fused split: W_hi and W_lo of each tap; the packed row of a tap is [W_hi | W_lo | W_hi] = 96 halves)
-        mbar_arrive_expect_tx(w_bar, (uint32_t)b_resident_bytes<BLOCK_N, BLOCK_K, FS>());
-        if constexpr (FS) {
-          for (int tap = 0; tap < 9; ++tap) {
-            tma_load_2d(&tmap_b, w_bar, smem_w + (tap * 2) * (BLOCK_N * 64), tap * 96, 0);
-            tma_load_2d(&tmap_b, w_bar, smem_w + (tap * 2 + 1) * (BLOCK_N * 64), tap * 96 + 32, 0);
-          }
-        } else {
-          for (int tap = 0; tap < 9; ++tap) tma_load_2d(&tmap_b, w_bar, smem_w + tap * (BLOCK_N * 64), tap * 32, 0);
-        }
-      }
-      // channel coordinate of K-chunk cc.  Split-precision mode (fp32-accurate products from fp16 tensor cores): the stored tensor is
-      // [hi(C) | lo(C)] and K runs over three segments  hi x W_hi,  hi x W_lo,  lo x W_hi  (weights packed [W_hi | W_lo | W_hi]).
-      auto a_chan = [&](int cc) -> int {
-        if (p.seg_chunks == 0) return cc * BLOCK_K;
-        const int seg = cc / p.seg_chunks, within = cc - seg * p.seg_chunks;
-        return (seg == 2 ? p.lo_off : 0) + within * BLOCK_K;
-      };
-      int stage = 0;
-      uint32_t phase = 0;
-      int fills = 0;
-      long long wait_empty = 0;  // debug timeline slot 124: cycles the producer waited for a free ring stage
-      for (int t = t_first; t < p.total_tiles; t += t_stride) {
-        const TileXY tc = tile_of(t);
-        const int n0 = tc.n0, mt = tc.mt, img = tc.img, h0 = tc.h0, w0 = tc.w0;
-        stamp(7 + 6 * ((t - t_first) / t_stride));
-        if constexpr (HALO) {
-          for (int kh = 0; kh < 3; ++kh) {  // one k-block per filter row: the input strip once, the three kw weight slices
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-            tma_load_4d(&tmap_a, &full_bar[stage], smem_a + stage * A_STAGE_BYTES, 0, w0 - 1, h0 + kh - 1, img);
-            if constexpr (FS) tma_load_4d(&tmap_a, &full_bar[stage], smem_a + stage * A_STAGE_BYTES + 9216, p.lo_off, w0 - 1, h0 + kh - 1, img);  // the lo strip
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          continue;
-        }
-        {  // L2 prefetch for the tile this CTA will process next (one box per channel chunk; taps overlap)
-          const int tn = t + t_stride;
-          if (tn < p.total_tiles && (tn / p.n_tiles) != (t / p.n_tiles)) {
-            const TileXY tnx = tile_of(tn);
-            const int imgn = tnx.img, h0n = tnx.h0, w0n = tnx.w0;
-            for (int cc = 0; cc < p.cchunks; ++cc) {
-              const int a_c0 = a_chan(cc);
-              if (!p.stride2) tma_prefetch_4d(&tmap_a, a_c0, w0n, h0n, imgn);
-              else {
-                for (int par = 0; par < 4; ++par)  // the four (h, w) parities of the 2x2 input cell
-                  tma_prefetch_5d(&tmap_a, (par & 1) * p.x_pitch + a_c0, w0n, par >> 1, h0n, imgn);
-              }
-            }
-          }
-        }
-        if constexpr (FS) {
-          for (int kb = 0; kb < p.num_k_blocks; ++kb) {  // k-block = (tap, 64-channel chunk): A_hi, A_lo, W_hi, W_lo once each
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
-            const int kh = tap / p.KW, kw = tap - kh * p.KW;
-            uint8_t* dst_a = smem_a + stage * A_STAGE_BYTES;
-            uint8_t* dst_b = smem_b + stage * B_STAGE_BYTES;
-            const int c_hi = cc * 64, c_lo = p.lo_off + cc * 64;
-            const int k_hi = tap * 3 * p.w_seg + cc * 64, k_lo = k_hi + p.w_seg;  // weights packed [W_hi | W_lo | W_hi] per tap
-            const uint32_t fs_bytes = 2u * (uint32_t)(p.BW * p.BH * 128) + (uint32_t)B_STAGE_BYTES;
-            if constexpr (CTA2) {
-              if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * fs_bytes);
-              const uint32_t lbar = mapa_rank0(smem_u32(&full_bar[stage]));
-              if (!p.stride2) {
-                tma_load_4d_2sm(&tmap_a, lbar, dst_a, c_hi, w0 + kw - p.pad, h0 + kh - p.pad, img);
-                tma_load_4d_2sm(&tmap_a, lbar, dst_a + A_HALF, c_lo, w0 + kw - p.pad, h0 + kh - p.pad, img);
-              } else {
-                const int th = kh - p.pad, tw = kw - p.pad;
-                tma_load_5d_2sm(&tmap_a, lbar, dst_a, (tw & 1) * p.x_pitch + c_hi, w0 + (tw >> 1), th & 1, h0 + (th >> 1), img);
-                tma_load_5d_2sm(&tmap_a, lbar, dst_a + A_HALF, (tw & 1) * p.x_pitch + c_lo, w0 + (tw >> 1), th & 1, h0 + (th >> 1), img);
-              }
-              const int nb = n0 + (int)cta_rank * (BLOCK_N / 2);
-              tma_load_2d_2sm(&tmap_b, lbar, dst_b, k_hi, nb);
-              tma_load_2d_2sm(&tmap_b, lbar, dst_b + B_HALF, k_lo, nb);
-            } else {
-              mbar_arrive_expect_tx(&full_bar[stage], fs_bytes);
-              if (!p.stride2) {
-                tma_load_4d(&tmap_a, &full_bar[stage], dst_a, c_hi, w0 + kw - p.pad, h0 + kh - p.pad, img);
-                tma_load_4d(&tmap_a, &full_bar[stage], dst_a + A_HALF, c_lo, w0 + kw - p.pad, h0 + kh - p.pad, img);
-              } else {
-                const int th = kh - p.pad, tw = kw - p.pad;
-                tma_load_5d(&tmap_a, &full_bar[stage], dst_a, (tw & 1) * p.x_pitch + c_hi, w0 + (tw >> 1), th & 1, h0 + (th >> 1), img);
-                tma_load_5d(&tmap_a, &full_bar[stage], dst_a + A_HALF, (tw & 1) * p.x_pitch + c_lo, w0 + (tw >> 1), th & 1, h0 + (th >> 1), img);
-              }
-              if (p.w_batched) {  // per-image weights (the mask product of the MaskFormer-family heads): third coordinate = image
-                tma_load_3d(&tmap_b, &full_bar[stage], dst_b, k_hi, n0, img);
-                tma_load_3d(&tmap_b, &full_bar[stage], dst_b + B_HALF, k_lo, n0, img);
-              } else {
-                tma_load_2d(&tmap_b, &full_bar[stage], dst_b, k_hi, n0);
-                tma_load_2d(&tmap_b, &full_bar[stage], dst_b + B_HALF, k_lo, n0);
-              }
-            }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          continue;
-        }
-        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-          const long long e0_ = trc ? clock64() : 0;
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (trc) wait_empty += clock64() - e0_;
-          if ((dbgv & 8) && fills >= STAGES) {  // experiment: operands stay whatever the first ring fill loaded - no TMA traffic, the MMAs run at their own pace
-            if (cta_rank == 0) mbar_arrive(&full_bar[stage]);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            continue;
-          }
-          ++fills;
-          const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
-          const int a_c0 = a_chan(cc);
-          const int kh = tap / p.KW, kw = tap - kh * p.KW;
-          void* dst_a = smem_a + stage * A_STAGE_BYTES;
-          if constexpr (CTA2) {  // both CTAs load their A rows and their half of B; all bytes are counted on the leader's barrier
-            if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * tx_bytes);
-            const uint32_t lbar = mapa_rank0(smem_u32(&full_bar[stage]));
-            if (!p.stride2) {
-              tma_load_4d_2sm(&tmap_a, lbar, dst_a, a_c0, w0 + kw - p.pad, h0 + kh - p.pad, img);
-            } else {
-              const int th = kh - p.pad, tw = kw - p.pad;
-              tma_load_5d_2sm(&tmap_a, lbar, dst_a, (tw & 1) * p.x_pitch + a_c0, w0 + (tw >> 1), th & 1, h0 + (th >> 1), img);
-            }
-            const int nb = n0 + (int)cta_rank * (BLOCK_N / 2);
-            if (p.w_batched) tma_load_3d_2sm(&tmap_b, lbar, smem_b + stage * B_STAGE_BYTES, kb * BKP, nb, img);
-            else tma_load_2d_2sm(&tmap_b, lbar, smem_b + stage * B_STAGE_BYTES, kb * BKP, nb);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            continue;
-          }
-          mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-          if (!p.stride2) {
-            tma_load_4d(&tmap_a, &full_bar[stage], dst_a, a_c0, w0 + kw - p.pad, h0 + kh - p.pad, img);
-          } else {
-            // input h = 2*ho + kh - pad -> (h>>1, h&1).  3x3/pad 1: kh=0 -> (ho-1,1); 1 -> (ho,0); 2 -> (ho,1).  2x2/pad 0: kh -> (ho,kh)
-            const int th = kh - p.pad, tw = kw - p.pad;
-            const int dh = th >> 1, hp = th & 1;   // arithmetic shift: -1 -> (-1, 1)
-            const int dw = tw >> 1, wp = tw & 1;
-            tma_load_5d(&tmap_a, &full_bar[stage], dst_a, wp * p.x_pitch + a_c0, w0 + dw, hp, h0 + dh, img);
-          }
-          if (p.w_batched) tma_load_3d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES, kb * BKP, n0, img);
-          else if ((dbgv & 64) && BLOCK_N >= 128) {  // experiment: same bytes, more TMA instructions
-            const int parts = (dbgv & 128) ? 4 : 2;
-            for (int q = 0; q < parts; ++q)
-              tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES + q * (B_STAGE_BYTES / parts), kb * BKP, n0 + q * (BLOCK_N / parts));
-          } else tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES, kb * BKP, n0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-      if (trc) trc[124] = (unsigned long long)wait_empty;
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (CTA pair: the leader only)
-    if (lane == 0 && cta_rank == 0) {
-      constexpr uint32_t idesc = make_idesc(BLOCK_N, CTA2 ? 256 : 128);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      long long wait_full = 0, wait_acc = 0;  // debug timeline: cycles the issuer spent waiting for operands / for a free accumulator stage (slots 122, 123)
-      if constexpr (HALO) mbar_wait(w_bar, 0);
-      for (int t = t_first; t < p.total_tiles; t += t_stride) {
-        const long long a0_ = trc ? clock64() : 0;
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);  // epilogue has drained this accumulator stage
-        tcgen05_fence_after();
-        if (trc) wait_acc += clock64() - a0_;
-        const int tk = (t - t_first) / t_stride;
-        stamp(2 + 6 * tk);
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * ACC_COLS);
-        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-          const long long w0_ = trc ? clock64() : 0;
-          if (!(dbgv & 32)) mbar_wait(&full_bar[stage], phase);  // dbg 32: the MMAs never wait for operands (timing experiment: loads still run)
-          tcgen05_fence_after();
-          if (trc) wait_full += clock64() - w0_;
-          if (kb == 0) stamp(3 + 6 * tk);
-          const uint64_t da = make_smem_desc<BKP>(smem_u32(smem_a + stage * A_STAGE_BYTES));
-          const uint64_t db = make_smem_desc<BKP>(smem_u32(smem_b + stage * B_STAGE_BYTES));
-          if constexpr (FS && HALO) {
-            const uint64_t da_lo = make_smem_desc<BKP>(smem_u32(smem_a + stage * A_STAGE_BYTES + 9216));
-#pragma unroll
-            for (int kw = 0; kw < 3; ++kw) {  // the strip shifted by kw pixels; three products per 16-channel step
-              const uint64_t ah = da + (uint64_t)(kw * 4), al = da_lo + (uint64_t)(kw * 4);
-              const uint64_t bh = make_smem_desc<BKP>(smem_u32(smem_w + ((kb * 3 + kw) * 2) * (BLOCK_N * 64)));
-              const uint64_t bl = make_smem_desc<BKP>(smem_u32(smem_w + ((kb * 3 + kw) * 2 + 1) * (BLOCK_N * 64)));
-              if constexpr (NCAT_OK) {
-                if (ncat) {  // W_lo of a tap follows its W_hi in the resident weights: one N = 2 * BLOCK_N MMA for both
-                  constexpr uint32_t idesc2 = make_idesc(2 * BLOCK_N, 128);
-#pragma unroll
-                  for (int k = 0; k < 2; ++k) {
-                    const uint64_t ko = (uint64_t)(k * 2);
-                    umma_f16(tmem_d, ah + ko, bh + ko, idesc2, (kb > 0 || kw > 0 || k > 0) ? 1u : 0u);
-                    umma_f16(tmem_d, al + ko, bh + ko, idesc, 1u);
-                  }
-                  continue;
-                }
-              }
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {
-                const uint64_t ko = (uint64_t)(k * 2);
-                umma_f16(tmem_d, ah + ko, bh + ko, idesc, (kb > 0 || kw > 0 || k > 0) ? 1u : 0u);
-                umma_f16(tmem_d, ah + ko, bl + ko, idesc, 1u);
-                umma_f16(tmem_d, al + ko, bh + ko, idesc, 1u);
-              }
-            }
-          } else if constexpr (FS) {
-            const uint64_t da_lo = make_smem_desc<BKP>(smem_u32(smem_a + stage * A_STAGE_BYTES + A_HALF));
-            const uint64_t db_lo = make_smem_desc<BKP>(smem_u32(smem_b + stage * B_STAGE_BYTES + B_HALF));
-            auto issue = [&](uint64_t a, uint64_t b, uint32_t acc_flag) {
-              if constexpr (CTA2) umma_f16_2sm(tmem_d, a, b, idesc, acc_flag);
-              else umma_f16(tmem_d, a, b, idesc, acc_flag);
-            };
-            bool done = false;
-            if constexpr (NCAT_OK) {
-              if (ncat) {  // the W_lo half of the stage follows the W_hi half (B_HALF = BLOCK_N rows of 128 B): one N = 2 * BLOCK_N MMA for both
-                constexpr uint32_t idesc2 = make_idesc(2 * BLOCK_N, 128);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  const uint64_t ko = (uint64_t)(k * 2);
-                  umma_f16(tmem_d, da + ko, db + ko, idesc2, (kb > 0 || k > 0) ? 1u : 0u);
-                  umma_f16(tmem_d, da_lo + ko, db + ko, idesc, 1u);
-                }
-                done = true;
-              }
-            }
-            if (!done) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {  // hi x W_hi, hi x W_lo, lo x W_hi per 16-channel step, all into the same fp32 accumulator
-                const uint64_t ko = (uint64_t)(k * 2);
-                issue(da + ko, db + ko, (kb > 0 || k > 0) ? 1u : 0u);
-                issue(da + ko, db_lo + ko, 1u);
-                issue(da_lo + ko, db + ko, 1u);
-              }
-            }
-          } else if constexpr (HALO) {
-#pragma unroll
-            for (int kw = 0; kw < 3; ++kw) {
-              // tap kw reads the strip shifted by kw pixels = kw * 64 B (+4 per pixel in 16-byte units); p.halo_boff: also patch the descriptor's
-              // base-offset field (bits 49-51) with the 128-byte phase of the shifted start
-              uint64_t dak = da + (uint64_t)(kw * 4);
-              if (p.halo_boff) dak |= (uint64_t)(((smem_u32(smem_a + stage * A_STAGE_BYTES) + kw * 64) >> 7) & 7) << 49;
-              const uint64_t dbk = make_smem_desc<BKP>(smem_u32(smem_w + (kb * 3 + kw) * (BLOCK_N * 64)));
-#pragma unroll
-              for (int k = 0; k < 2; ++k) umma_f16(tmem_d, dak + (uint64_t)(k * 2), dbk + (uint64_t)(k * 2), idesc, (kb > 0 || kw > 0 || k > 0) ? 1u : 0u);
-            }
-          } else {
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / 16; ++k) {
-              // advance 16 halves = 32 B inside the swizzle row: +2 in 16-byte units
-              const uint32_t td = ((dbgv & 16) && (k & 1)) ? tmem_base + (uint32_t)((acc ^ 1) * BLOCK_N) : tmem_d;  // dbg 16: two independent accumulation chains
-              if constexpr (CTA2) umma_f16_2sm(td, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-              else umma_f16(td, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-            }
-          }
-          if constexpr (CTA2) umma_commit_2sm(&empty_bar[stage]);
-          else umma_commit(&empty_bar[stage]);  // smem stage may be refilled once these MMAs have read it
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if constexpr (CTA2) umma_commit_2sm(&tmem_full_bar[acc]);
-        else umma_commit(&tmem_full_bar[acc]);
-        stamp(4 + 6 * tk);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      if (trc) { trc[122] = (unsigned long long)wait_full; trc[123] = (unsigned long long)wait_acc; trc[125] = (unsigned long long)clock64(); }
-    }
-  } else if (warp >= 4) {
-    // ===================================================================== epilogue (128 threads)
-    const int grp = (warp - 4) >> 2;     // column group
-    const int ew = warp & 3;             // TMEM lane quarter (a warp may only touch lanes 32*(warp%4)..+31)
-    const int row = ew * 32 + lane;      // tile row == TMEM lane
-    const int bh = row / p.BW, bw = row - bh * p.BW;
-    const int et = threadIdx.x - PRODUCER_THREADS - grp * 128;
-    constexpr int GROUP_COLS = BLOCK_N / EPI_GROUPS;
-    const int c_begin = grp * GROUP_COLS, c_end = c_begin + GROUP_COLS;
-    uint8_t* const my_staging = staging + grp * NSTG * STAGING_BYTES;
-    constexpr int CHUNK_COLS = 128 / (int)sizeof(TOut);  // output columns per 128-byte staging row
-    const bool post = (p.act & FB200_ACT_RESIDUAL_AFTER) != 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    uint32_t chunk_ctr = 0;
-    // Residual: this thread's 128-byte row chunk is fetched (8 x LDG.128, L2-prefetched a tile ahead by TMA) at the top of
-    // each chunk, before the staging-buffer wait / TMEM load, and consumed after them.  (A one-chunk-ahead register
-    // pipeline was measured slower — profiles/r01_trip11 vs trip12; deeper prefetch needs an smem ring: next round.)
-    constexpr int RES_VECS = 8;  // 16-byte vectors per 128-byte row chunk
-    const bool has_res = p.res != nullptr && !(dbgv & 2);
-    uint4 rcur[RES_VECS];
-    auto res_fetch = [&](int tt, int cc0, uint4 (&dst)[RES_VECS]) -> bool {
-      if (PAIR || !has_res || tt >= p.total_tiles) return false;  // pair residuals always come through TMA
-      const TileXY tx = tile_of(tt);
-      const int n0_ = tx.n0, img_ = tx.img;
-      if (n0_ + cc0 + CHUNK_COLS > p.Cout || cc0 + CHUNK_COLS > c_end) return false;
-      const int ho_ = tx.h0 + bh, wo_ = tx.w0 + bw;
-      if (!(row < p.BW * p.BH && ho_ < p.Ho && wo_ < p.Wo && img_ < p.nimg)) return false;
-      const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const TOut*>(p.res) + (((int64_t)img_ * p.Ho + ho_) * p.Wo + wo_) * p.res_pitch + n0_ + cc0);
-#pragma unroll
-      for (int q = 0; q < RES_VECS; ++q) dst[q] = __ldg(src + q);
-      return true;
+    if (threadIdx.x != 0) return;
+    const uint32_t a_bytes = (uint32_t)(p.BW * p.BH * BLOCK_K * 2);
+    // channel coordinate of K-chunk cc.  Segmented split-precision mode (fp32-accurate products from fp16 tensor cores, fp16 output): the stored tensor is
+    // [hi(C) | lo(C)] and K runs over three segments  hi x W_hi,  hi x W_lo,  lo x W_hi  (weights packed [W_hi | W_lo | W_hi]).
+    auto a_chan = [&](int cc) -> int {
+      if (p.seg_chunks == 0) return cc * BLOCK_K;
+      const int seg = cc / p.seg_chunks, within = cc - seg * p.seg_chunks;
+      return (seg == 2 ? p.lo_off : 0) + within * BLOCK_K;
     };
-    // ---- residual through TMA (res_tma): the [BW x BH x CHUNK_COLS] residual box of chunk k+1 is loaded into the staging buffer that chunk will
-    // use, one chunk ahead of its consumption; each thread then reads ITS row from shared memory (same swizzle as the output staging), adds the
-    // accumulator and writes the result back in place before the TMA store.  Coalescing is the TMA unit's job (the per-thread LDG.128 pattern touches
-    // 32 different 128-byte lines per instruction), nothing is held in registers across the wait, and no extra shared memory is needed.
-    const bool res_tma = has_res && p.res_tma && NSTG >= 2;
-    uint64_t* const my_res_bar = res_bar + grp * NSTG;
-    const uint32_t res_box_bytes = (uint32_t)(p.BW * p.BH * 128);
-    auto chunk_valid = [&](int tt, int cc0) { return tt < p.total_tiles && cc0 < c_end && (tt % p.n_tiles) * BLOCK_N + cc0 < p.Cout; };
-    auto issue_res = [&](int tt, int cc0, uint32_t k) {  // elected thread only
-      const TileXY tx = tile_of(tt);
-      const int n0_ = tx.n0, img_ = tx.img, h0_ = tx.h0, w0_ = tx.w0;
-      uint64_t* bar = &my_res_bar[k % NSTG];
-      mbar_arrive_expect_tx(bar, res_box_bytes);
-      tma_load_4d(&tmap_r, bar, my_staging + (k % NSTG) * STAGING_BYTES, n0_ + cc0, w0_, h0_, img_);
-      if constexpr (PAIR) tma_load_4d(&tmap_r2, bar, my_staging + (k % NSTG) * STAGING_BYTES + STAGING_BYTES / 2, n0_ + cc0, w0_, h0_, img_);
+    auto load_a = [&](uint64_t* bar, void* dst, int c, int kh, int kw, int h0, int w0, int img) {
+      if (!p.stride2) {
+        tma_load_4d(&tmap_a, bar, dst, c, w0 + kw - p.pad, h0 + kh - p.pad, img);
+      } else {
+        // input h = 2*ho + kh - pad -> (h>>1, h&1).  3x3/pad 1: kh=0 -> (ho-1,1); 1 -> (ho,0); 2 -> (ho,1).  2x2/pad 0: kh -> (ho,kh)
+        const int th = kh - p.pad, tw = kw - p.pad;  // arithmetic shift: -1 -> (-1, 1)
+        tma_load_5d(&tmap_a, bar, dst, (tw & 1) * p.x_pitch + c, w0 + (tw >> 1), th & 1, h0 + (th >> 1), img);
+      }
     };
-    if (res_tma && et == 0 && chunk_valid(t_first, c_begin)) issue_res(t_first, c_begin, 0);
-    for (int t = t_first; t < p.total_tiles; t += t_stride) {
+    auto load_b = [&](uint64_t* bar, void* dst, int k, int n0, int img) {
+      if (p.w_batched) tma_load_3d(&tmap_b, bar, dst, k, n0, img);  // per-image weights (the mask product of the MaskFormer-family heads)
+      else tma_load_2d(&tmap_b, bar, dst, k, n0);
+    };
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
       const TileXY tc = tile_of(t);
-      const int n0 = tc.n0, img = tc.img, h0 = tc.h0, w0 = tc.w0;
-      const int ho = h0 + bh, wo = w0 + bw;
-      const bool row_valid = (row < p.BW * p.BH) && ho < p.Ho && wo < p.Wo && img < p.nimg;
-      if (has_res && !res_tma && et == 0) {  // L2 prefetch of the NEXT tile's residual columns owned by this group
-        const int tn = t + t_stride;
-        if (tn < p.total_tiles) {
+      {  // L2 prefetch for the tile this CTA will process next (one box per channel chunk; taps overlap)
+        const int tn = t + gridDim.x;
+        if (tn < p.total_tiles && (tn / p.n_tiles) != (t / p.n_tiles)) {
           const TileXY tnx = tile_of(tn);
-          const int n0n = tnx.n0, imgn = tnx.img, h0n = tnx.h0, w0n = tnx.w0;
-          for (int c = c_begin; c < c_end; c += 128 / (int)sizeof(TOut))
-            if (n0n + c < p.Cout) tma_prefetch_4d(&tmap_r, n0n + c, w0n, h0n, imgn);
-        }
-      }
-      // per-tile scale / bias (n0 changes with the N tile)
-      epi_bar(grp);  // the group is done with the previous tile's scale/bias
-      for (int i = c_begin + et; i < c_end; i += 128) {
-        const int n = n0 + i;
-        s_scale[i] = (p.scale && n < p.Cout) ? p.scale[n] : 1.f;
-        s_bias[i] = (p.bias && n < p.Cout) ? p.bias[n] : 0.f;
-      }
-      epi_bar(grp);
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tcgen05_fence_after();
-      if (grp == 0 && et == 0) stamp(5 + 6 * ((t - t_first) / t_stride));
-      const uint32_t tmem_acc = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc * ACC_COLS);
-      float row_max = -INFINITY;
-      if (p.rowmax) {  // row-max-only epilogue: enc_outputs_class.max(-1) (modelling.py:1210) without materialising the [B*S, num_classes] logits
-#pragma unroll 1
-        for (int c0 = c_begin; c0 < c_end && n0 + c0 < p.Cout; c0 += 32) {
-          uint32_t r[32];
-          tmem_ld32(tmem_acc + (uint32_t)c0, r);
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (n0 + c0 + j < p.Cout) row_max = fmaxf(row_max, fmaf(__uint_as_float(r[j]), s_scale[c0 + j], s_bias[c0 + j]));
-        }
-        if (row_valid) atomic_max_float(p.rowmax + ((int64_t)img * p.Ho + ho) * p.Wo + wo, row_max);
-      }
-#pragma unroll 1
-      for (int c0 = c_begin; c0 < c_end && !p.rowmax; c0 += CHUNK_COLS) {
-        if (n0 + c0 >= p.Cout) break;  // uniform across the group
-        if (dbgv & 4) break;          // experiment: no epilogue work at all
-        uint8_t* stg = my_staging + (chunk_ctr % NSTG) * STAGING_BYTES;
-        uint8_t* srow = stg + row * 128;
-        bool res_vec = false;
-        if (res_tma) {
-          if (et == 0) {  // prefetch the NEXT chunk's residual into the buffer it will use: that buffer's last store must have finished reading it
-            int tn = t, cn = c0 + CHUNK_COLS;
-            if (!chunk_valid(tn, cn)) { tn = t + t_stride; cn = c_begin; }
-            if (chunk_valid(tn, cn)) {
-              tma_store_wait_read<(NSTG >= 2 ? NSTG - 2 : 0)>();
-              issue_res(tn, cn, chunk_ctr + 1);
+          const int nchunks = FS ? 2 * p.cchunks : p.cchunks;
+          for (int cc = 0; cc < nchunks; ++cc) {
+            const int a_c0 = FS ? (cc < p.cchunks ? cc * BLOCK_K : p.lo_off + (cc - p.cchunks) * BLOCK_K) : a_chan(cc);
+            if (!p.stride2) tma_prefetch_4d(&tmap_a, a_c0, tnx.w0, tnx.h0, tnx.img);
+            else {
+              for (int par = 0; par < 4; ++par)  // the four (h, w) parities of the 2x2 input cell
+                tma_prefetch_5d(&tmap_a, (par & 1) * p.x_pitch + a_c0, tnx.w0, par >> 1, tnx.h0, tnx.img);
             }
           }
-          mbar_wait(&my_res_bar[chunk_ctr % NSTG], (chunk_ctr / NSTG) & 1);  // this chunk's residual has landed in `stg`
+        }
+      }
+      for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
+        const int kh = tap / p.KW, kw = tap - kh * p.KW;
+        uint8_t* dst_a = smem_a + stage * A_STAGE_BYTES;
+        uint8_t* dst_b = smem_b + stage * B_STAGE_BYTES;
+        if constexpr (FS) {  // k-block = (tap, channel chunk): A_hi, A_lo, W_hi, W_lo once each
+          const int k_hi = tap * 3 * p.w_seg + cc * BLOCK_K, k_lo = k_hi + p.w_seg;  // weights packed [W_hi | W_lo | W_hi] per tap
+          mbar_arrive_expect_tx(&full_bar[stage], 2u * a_bytes + (uint32_t)B_STAGE_BYTES);
+          load_a(&full_bar[stage], dst_a, cc * BLOCK_K, kh, kw, tc.h0, tc.w0, tc.img);
+          load_a(&full_bar[stage], dst_a + A_HALF, p.lo_off + cc * BLOCK_K, kh, kw, tc.h0, tc.w0, tc.img);
+          load_b(&full_bar[stage], dst_b, k_hi, tc.n0, tc.img);
+          load_b(&full_bar[stage], dst_b + B_HALF, k_lo, tc.n0, tc.img);
         } else {
-          res_vec = res_fetch(t, c0, rcur);
-          // the TMA store that last used this staging buffer must have finished READING it
-          if (et == 0) tma_store_wait_read<NSTG - 1>();
-          epi_bar(grp);
+          mbar_arrive_expect_tx(&full_bar[stage], a_bytes + (uint32_t)B_STAGE_BYTES);
+          load_a(&full_bar[stage], dst_a, a_chan(cc), kh, kw, tc.h0, tc.w0, tc.img);
+          load_b(&full_bar[stage], dst_b, kb * BLOCK_K, tc.n0, tc.img);
         }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+    return;
+  }
+
+  // ===================================================================== consumers: wgmma main loop + epilogue
+  const int ct = threadIdx.x - 128;           // 0..255
+  const int g = ct >> 7;                      // warp-group: tile rows 64g .. 64g + 63
+  const int r0 = g * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2);  // accumulator rows r0 and r0 + 8 of this thread
+  const int cq = 2 * (lane & 3);              // first of the two adjacent accumulator columns
+  constexpr int NACC = BLOCK_N / 2;
+  constexpr int CHUNK_COLS = 128 / (int)sizeof(TOut);  // output columns per 128-byte staging row
+  const bool post = (p.act & FB200_ACT_RESIDUAL_AFTER) != 0;
+  const bool has_res = p.res != nullptr;
+  float acc[NACC];
+  int stage = 0;
+  uint32_t phase = 0, res_phase = 0, chunk_ctr = 0;
+  for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+    const TileXY tc = tile_of(t);
+    int prev = -1;
+    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES) + (uint32_t)(g * 64 * BLOCK_K * 2);
+      const uint32_t sb = smem_u32(smem_b + stage * B_STAGE_BYTES);
+      const uint64_t da = make_smem_desc<BLOCK_K>(sa), db = make_smem_desc<BLOCK_K>(sb);
+      wgmma_fence();
 #pragma unroll
-        for (int sub = 0; sub < CHUNK_COLS / 32; ++sub) {
-          if (c0 + sub * 32 >= c_end) break;  // BLOCK_N = 32 with fp16 output: half a staging row
-          uint32_t r[32];
-          tmem_ld32(tmem_acc + (uint32_t)(c0 + sub * 32), r);
-          if constexpr (NCAT_OK) {
-            if (ncat) {  // second half of the accumulator: the A_hi x W_lo product
-              uint32_t r2[32];
-              tmem_ld32(tmem_acc + (uint32_t)(BLOCK_N + c0 + sub * 32), r2);
+      for (int k = 0; k < BLOCK_K / 16; ++k) {
+        // advance 16 halves = 32 B inside the swizzle row: +2 in 16-byte units
+        const uint64_t ko = (uint64_t)(k * 2);
+        Wgmma<BLOCK_N, 0>::mma(acc, da + ko, db + ko, (kb > 0 || k > 0) ? 1u : 0u);
+        if constexpr (FS) {  // hi x W_lo, lo x W_hi into the same fp32 accumulator
+          const uint64_t da_lo = make_smem_desc<BLOCK_K>(sa + A_HALF), db_lo = make_smem_desc<BLOCK_K>(sb + B_HALF);
+          Wgmma<BLOCK_N, 0>::mma(acc, da + ko, db_lo + ko, 1u);
+          Wgmma<BLOCK_N, 0>::mma(acc, da_lo + ko, db + ko, 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's products are done: its stage may be refilled
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+
+    auto scale_of = [&](int n) { return (p.scale && n < p.Cout) ? __ldg(p.scale + n) : 1.f; };
+    auto bias_of = [&](int n) { return (p.bias && n < p.Cout) ? __ldg(p.bias + n) : 0.f; };
+    auto row_valid = [&](int row, int64_t& pix) {
+      const int bh = row / p.BW, bw = row - bh * p.BW;
+      const int ho = tc.h0 + bh, wo = tc.w0 + bw;
+      pix = ((int64_t)tc.img * p.Ho + ho) * p.Wo + wo;
+      return row < p.BW * p.BH && ho < p.Ho && wo < p.Wo;
+    };
+    if (p.rowmax) {  // row-max-only epilogue: enc_outputs_class.max(-1) without materialising the [B*S, num_classes] logits
+      float m[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-              for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-            }
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int n = tc.n0 + 8 * j + cq + e;
+          if (n < p.Cout) {
+            const float s = scale_of(n), b = bias_of(n);
+            m[0] = fmaxf(m[0], fmaf(acc[4 * j + e], s, b));
+            m[1] = fmaxf(m[1], fmaf(acc[4 * j + 2 + e], s, b));
           }
-          float v[32];
+        }
+      }
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 sc = *reinterpret_cast<const float4*>(&s_scale[c0 + sub * 32 + j]);
-            const float4 bi = *reinterpret_cast<const float4*>(&s_bias[c0 + sub * 32 + j]);
-            v[j + 0] = fmaf(__uint_as_float(r[j + 0]), sc.x, bi.x);
-            v[j + 1] = fmaf(__uint_as_float(r[j + 1]), sc.y, bi.y);
-            v[j + 2] = fmaf(__uint_as_float(r[j + 2]), sc.z, bi.z);
-            v[j + 3] = fmaf(__uint_as_float(r[j + 3]), sc.w, bi.w);
-          }
+      for (int h = 0; h < 2; ++h) {
+        m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
+        m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
+        int64_t pix;
+        if ((lane & 3) == 0 && row_valid(r0 + 8 * h, pix)) atomic_max_float(p.rowmax + pix, m[h]);
+      }
+      continue;
+    }
+#pragma unroll
+    for (int ch = 0; ch < (BLOCK_N + CHUNK_COLS - 1) / CHUNK_COLS; ++ch) {
+      const int c0 = ch * CHUNK_COLS;
+      if (tc.n0 + c0 >= p.Cout) break;  // uniform across the consumers
+      uint8_t* stg = staging + (chunk_ctr % NSTG) * STAGING_BYTES;
+      if (ct == 0) {
+        tma_store_wait_read<NSTG - 1>();  // the TMA store that last used this staging buffer has finished READING it
+        if (has_res) {  // the [BW x BH x CHUNK_COLS] residual box lands in the staging buffer; each thread adds and overwrites its own elements
+          mbar_arrive_expect_tx(res_bar, (uint32_t)(p.BW * p.BH * 128));
+          tma_load_4d(&tmap_r, res_bar, stg, tc.n0 + c0, tc.w0, tc.h0, tc.img);
+          if constexpr (PAIR) tma_load_4d(&tmap_r2, res_bar, stg + STAGING_BYTES / 2, tc.n0 + c0, tc.w0, tc.h0, tc.img);
+        }
+      }
+      consumer_bar();
+      if (has_res) { mbar_wait(res_bar, res_phase); res_phase ^= 1; }
+#pragma unroll
+      for (int jj = 0; jj < CHUNK_COLS / 8; ++jj) {
+        const int j = c0 / 8 + jj;
+        if (j >= BLOCK_N / 8) break;
+        const int lc = 8 * jj + cq;  // column inside the chunk
+        const int n = tc.n0 + c0 + lc;
+        const float s0 = scale_of(n), s1 = scale_of(n + 1), b0 = bias_of(n), b1 = bias_of(n + 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          float v0 = fmaf(acc[4 * j + 2 * h], s0, b0), v1 = fmaf(acc[4 * j + 2 * h + 1], s1, b1);
+          // byte offset of (row, lc) in the swizzled staging tile: 16-byte piece index XOR the row phase
+          int off;
+          if constexpr (PAIR) off = row * 64 + ((((lc >> 3) ^ ((row >> 1) & 3)) << 4) | ((lc & 7) * 2));  // two 64-byte-row planes, 64-byte swizzle
+          else if constexpr (sizeof(TOut) == 2) off = row * 128 + ((((lc >> 3) ^ (row & 7)) << 4) | ((lc & 7) * 2));
+          else off = row * 128 + ((((lc >> 2) ^ (row & 7)) << 4) | ((lc & 3) * 4));
           auto add_residual = [&]() {
-            if (res_tma) {  // this thread's row of the TMA-loaded residual box, 16-byte pieces at the swizzled positions it will overwrite below
-              if constexpr (PAIR) {
-                const uint8_t* hrow = stg + row * 64;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const int ph = (q ^ ((row >> 1) & 3)) << 4;
-                  const uint4 th = *reinterpret_cast<const uint4*>(hrow + ph), tl = *reinterpret_cast<const uint4*>(hrow + STAGING_BYTES / 2 + ph);
-                  const uint32_t hw[4] = {th.x, th.y, th.z, th.w}, lw[4] = {tl.x, tl.y, tl.z, tl.w};
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hw[e])), fl = __half22float2(*reinterpret_cast<const __half2*>(&lw[e]));
-                    v[q * 8 + 2 * e] += fh.x + fl.x;
-                    v[q * 8 + 2 * e + 1] += fh.y + fl.y;
-                  }
-                }
-              } else if constexpr (sizeof(TOut) == 2) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const uint4 t4 = *reinterpret_cast<const uint4*>(srow + (((sub * 4 + q) ^ (row & 7)) << 4));
-                  const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&t4.x)), f1 = __half22float2(*reinterpret_cast<const __half2*>(&t4.y));
-                  const float2 f2 = __half22float2(*reinterpret_cast<const __half2*>(&t4.z)), f3 = __half22float2(*reinterpret_cast<const __half2*>(&t4.w));
-                  v[q * 8 + 0] += f0.x; v[q * 8 + 1] += f0.y; v[q * 8 + 2] += f1.x; v[q * 8 + 3] += f1.y;
-                  v[q * 8 + 4] += f2.x; v[q * 8 + 5] += f2.y; v[q * 8 + 6] += f3.x; v[q * 8 + 7] += f3.y;
-                }
-              } else {
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                  const uint4 t4 = *reinterpret_cast<const uint4*>(srow + ((q ^ (row & 7)) << 4));
-                  v[q * 4 + 0] += __uint_as_float(t4.x); v[q * 4 + 1] += __uint_as_float(t4.y);
-                  v[q * 4 + 2] += __uint_as_float(t4.z); v[q * 4 + 3] += __uint_as_float(t4.w);
-                }
-              }
-            } else if (res_vec) {
-              if constexpr (sizeof(TOut) == 2) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {  // 4 x 16 B = 32 halves of this sub-chunk
-                  const uint4 t4 = rcur[sub * 4 + q];
-                  const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&t4.x)), f1 = __half22float2(*reinterpret_cast<const __half2*>(&t4.y));
-                  const float2 f2 = __half22float2(*reinterpret_cast<const __half2*>(&t4.z)), f3 = __half22float2(*reinterpret_cast<const __half2*>(&t4.w));
-                  v[q * 8 + 0] += f0.x; v[q * 8 + 1] += f0.y; v[q * 8 + 2] += f1.x; v[q * 8 + 3] += f1.y;
-                  v[q * 8 + 4] += f2.x; v[q * 8 + 5] += f2.y; v[q * 8 + 6] += f3.x; v[q * 8 + 7] += f3.y;
-                }
-              } else {
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {  // 8 x 16 B = 32 floats
-                  const uint4 t4 = rcur[q];
-                  v[q * 4 + 0] += __uint_as_float(t4.x); v[q * 4 + 1] += __uint_as_float(t4.y);
-                  v[q * 4 + 2] += __uint_as_float(t4.z); v[q * 4 + 3] += __uint_as_float(t4.w);
-                }
-              }
+            if (!has_res) return;
+            if constexpr (PAIR) {
+              const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(stg + off));
+              const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(stg + STAGING_BYTES / 2 + off));
+              v0 += fh.x + fl.x;
+              v1 += fh.y + fl.y;
+            } else if constexpr (sizeof(TOut) == 2) {
+              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(stg + off));
+              v0 += f.x;
+              v1 += f.y;
+            } else {
+              const float2 f = *reinterpret_cast<const float2*>(stg + off);
+              v0 += f.x;
+              v1 += f.y;
             }
           };
           if (!post) add_residual();
-          act32<GELU>(v, p.act);
+          v0 = act1<GELU>(v0, p.act);
+          v1 = act1<GELU>(v1, p.act);
           if (post) add_residual();
-          // 16-byte pieces into the 128B-swizzled staging row: physical chunk = logical chunk ^ (row & 7)
-          if constexpr (PAIR) {  // two dense 64-byte-row tiles (hi, lo), 64-byte swizzle: physical chunk = logical chunk ^ ((row >> 1) & 3)
-            uint8_t* hrow = stg + row * 64;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              uint32_t hw[4], lw[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float a = v[q * 8 + 2 * e], b = v[q * 8 + 2 * e + 1];
-                const __half2 h = __floats2half2_rn(a, b);
-                const float2 hf = __half22float2(h);
-                const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-                hw[e] = *reinterpret_cast<const uint32_t*>(&h);
-                lw[e] = *reinterpret_cast<const uint32_t*>(&l);
-              }
-              const int ph = (q ^ ((row >> 1) & 3)) << 4;
-              *reinterpret_cast<uint4*>(hrow + ph) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-              *reinterpret_cast<uint4*>(hrow + STAGING_BYTES / 2 + ph) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-            }
+          if constexpr (PAIR) {
+            const __half2 hi = __floats2half2_rn(v0, v1);
+            const float2 hf = __half22float2(hi);
+            *reinterpret_cast<__half2*>(stg + off) = hi;
+            *reinterpret_cast<__half2*>(stg + STAGING_BYTES / 2 + off) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
           } else if constexpr (sizeof(TOut) == 2) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {  // 8 halves per 16 B
-              __half2 h0_ = __floats2half2_rn(v[q * 8 + 0], v[q * 8 + 1]), h1_ = __floats2half2_rn(v[q * 8 + 2], v[q * 8 + 3]);
-              __half2 h2_ = __floats2half2_rn(v[q * 8 + 4], v[q * 8 + 5]), h3_ = __floats2half2_rn(v[q * 8 + 6], v[q * 8 + 7]);
-              const uint4 pk = make_uint4(*reinterpret_cast<uint32_t*>(&h0_), *reinterpret_cast<uint32_t*>(&h1_),
-                                          *reinterpret_cast<uint32_t*>(&h2_), *reinterpret_cast<uint32_t*>(&h3_));
-              *reinterpret_cast<uint4*>(srow + (((sub * 4 + q) ^ (row & 7)) << 4)) = pk;
-            }
+            *reinterpret_cast<__half2*>(stg + off) = __floats2half2_rn(v0, v1);
           } else {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {  // 4 floats per 16 B
-              const uint4 pk = make_uint4(__float_as_uint(v[q * 4 + 0]), __float_as_uint(v[q * 4 + 1]),
-                                          __float_as_uint(v[q * 4 + 2]), __float_as_uint(v[q * 4 + 3]));
-              *reinterpret_cast<uint4*>(srow + ((q ^ (row & 7)) << 4)) = pk;
-            }
+            *reinterpret_cast<float2*>(stg + off) = make_float2(v0, v1);
           }
         }
-        fence_proxy_async();
-        epi_bar(grp);
-        if (et == 0) {
-          if (!(dbgv & 1)) {
-            tma_store_4d(&tmap_d, stg, n0 + c0, w0, h0, img);
-            if constexpr (PAIR) tma_store_4d(&tmap_d2, stg + STAGING_BYTES / 2, n0 + c0, w0, h0, img);
-          }
-          tma_store_commit();
-        }
-        ++chunk_ctr;
       }
-      // all tcgen05.ld of this accumulator stage have completed (wait::ld): hand it back to the MMA warp
-      tcgen05_fence_before();
-      __syncwarp();
-      if (grp == 0 && et == 0) stamp(6 + 6 * ((t - t_first) / t_stride));
-      if (lane == 0) {
-        if constexpr (CTA2) mbar_arrive_cluster(mapa_rank0(smem_u32(&tmem_empty_bar[acc])));
-        else mbar_arrive(&tmem_empty_bar[acc]);
+      fence_proxy_async();
+      consumer_bar();
+      if (ct == 0) {
+        tma_store_4d(&tmap_d, stg, tc.n0 + c0, tc.w0, tc.h0, tc.img);
+        if constexpr (PAIR) tma_store_4d(&tmap_d2, stg + STAGING_BYTES / 2, tc.n0 + c0, tc.w0, tc.h0, tc.img);
+        tma_store_commit();
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      ++chunk_ctr;
     }
-    if (et == 0) tma_store_wait_all();
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if constexpr (CTA2) cluster_sync_all();  // neither CTA may retire (or free TMEM) while its partner can still touch its barriers / shared memory
-  if (warp == 2) {
-    tcgen05_fence_after();
-    if constexpr (CTA2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
+  if (ct == 0) tma_store_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------- host
@@ -928,6 +452,7 @@ static int encode(CUtensorMap* m, CUtensorMapDataType dt, int elt, int rank, voi
 }
 
 // best output rectangle (BW x BH <= 128 pixels) for an Ho x Wo map
+// best output rectangle (BW x BH <= 128 pixels) for an Ho x Wo map
 static void choose_tile(int Ho, int Wo, int* BW, int* BH) {
   double best = -1.0;
   for (int bw = 1; bw <= (Wo < 128 ? Wo : 128); ++bw) {
@@ -946,72 +471,25 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
-// programmatic dependent launch of consecutive conv_tc kernels (the prologue of launch n+1 overlaps the tail of launch n, see conv_tc_kernel).  Measured on the B200
-// (trip r02-20, graph replay of the whole step): 18.41 ms with, 18.40 ms without - the ~2 us prologue is already hidden behind the persistent CTAs' first TMA
-// round trip - so it is OFF by default; FB200_TC_PDL=1 turns it on.
-static bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("FB200_TC_PDL"); on = e ? atoi(e) : 0; }
-  return on != 0;
-}
-
-template <int BLOCK_N, int STAGES, typename TOut, int MIN_BLOCKS, int BLOCK_K, int NSTG, bool GELU, bool CTA2 = false, bool FS = false>
+template <int BLOCK_N, int STAGES, typename TOut, int BLOCK_K, int NSTG, bool GELU, bool FS = false>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& tr, const CUtensorMap& td2, const CUtensorMap& tr2,
                   const KParams& kp, cudaStream_t st) {
-  auto kern = conv_tc_kernel<BLOCK_N, STAGES, TOut, MIN_BLOCKS, BLOCK_K, NSTG, GELU, CTA2, FS>;
-  constexpr int smem = smem_bytes<BLOCK_N, STAGES, BLOCK_K, NSTG, CTA2, FS>();
-  constexpr int NUM_THREADS = num_threads<BLOCK_N>();
+  auto kern = conv_tc_kernel<BLOCK_N, STAGES, TOut, BLOCK_K, NSTG, GELU, FS>;
+  constexpr int smem = smem_bytes<BLOCK_N, STAGES, BLOCK_K, NSTG, FS>();
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  static_assert(MIN_BLOCKS * 2 * ((FS && !CTA2 && BLOCK_N <= 128) ? 2 * BLOCK_N : BLOCK_N) <= 512, "TMEM budget exceeded (a blocked tcgen05.alloc would deadlock)");
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { set_error("conv_tc: cudaFuncSetAttribute(%d B) failed: %s", smem, cudaGetErrorString(e)); return FB200_ERR_CUDA; }
     configured = true;
   }
-  if constexpr (CTA2) {  // one cluster of two CTAs per tile (SM pair of a TPC), persistent over the pair tiles
-    static_assert(MIN_BLOCKS == 1, "CTA pairs own the whole TMEM of both SMs");
-    const int64_t pairs = num_sms() / 2;
-    const unsigned grid = 2u * (unsigned)(kp.total_tiles < pairs ? kp.total_tiles : pairs);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid, 1, 1);
-    cfg.blockDim = dim3(NUM_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, td, tr, td2, tr2, kp);
-    if (e != cudaSuccess) { set_error("conv_tc(cta pair): launch failed: %s", cudaGetErrorString(e)); return FB200_ERR_CUDA; }
-    return FB200_OK;
-  }
-  int64_t cap = (int64_t)num_sms() * MIN_BLOCKS;
-  { static int gc = -1; if (gc < 0) { const char* e = getenv("FB200_GRID_CAP"); gc = e ? atoi(e) : 0; } if (gc > 0 && gc < cap) cap = gc; }  // experiment: fewer SMs
+  const int64_t cap = num_sms();
   const unsigned grid = (unsigned)(kp.total_tiles < cap ? kp.total_tiles : cap);
-  if (pdl_enabled()) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid, 1, 1);
-    cfg.blockDim = dim3(NUM_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, td, tr, td2, tr2, kp);
-    if (e != cudaSuccess) { set_error("conv_tc: launch failed: %s", cudaGetErrorString(e)); return FB200_ERR_CUDA; }
-    return FB200_OK;
-  }
   kern<<<grid, NUM_THREADS, smem, st>>>(ta, tb, td, tr, td2, tr2, kp);
   FB_CHECK_LAUNCH("conv_tc_kernel");
   return FB200_OK;
@@ -1019,23 +497,12 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
 
 }  // namespace tc
 
-static int g_cta_pair_mode = -1;  // FB200_OPT_CONV_CTA_PAIR
-static unsigned long long* g_trace = nullptr;  // fb200_set_conv_trace
-
-void conv_tc_set_trace(void* buf) { g_trace = static_cast<unsigned long long*>(buf); }
-
-int conv_tc_set_pair_mode(int v) {
-  const int old = g_cta_pair_mode < 0 ? 1 : g_cta_pair_mode;
-  g_cta_pair_mode = v;
-  return old;
-}
-
 bool conv2d_tc_supported(const ConvParams& p, int x_dtype, int out_dtype) {
   if (x_dtype != FB200_F16) return false;
   if (out_dtype != FB200_F16 && out_dtype != FB200_F32 && out_dtype != FB200_F16PAIR) return false;
   const int Clog = p.split3 ? p.Cin / 3 : p.Cin;  // channels of one K segment
-  if (out_dtype == FB200_F16PAIR) {  // pair output: fused-split layers (64-channel chunks or the 32-channel halo strips), planes 16-byte aligned
-    if (!p.split3 || (Clog % 64 != 0 && Clog != 32) || p.rowmax || p.w_bs != 0 || p.Cout % 8 != 0) return false;
+  if (out_dtype == FB200_F16PAIR) {  // pair output: fused-split layers, planes 16-byte aligned
+    if (!p.split3 || p.rowmax || p.w_bs != 0 || p.Cout % 8 != 0) return false;
     if ((p.out_lo_off * 2) % 16 != 0 || (p.out_pitch * 2) % 16 != 0 || (p.out_bs * 2) % 16 != 0) return false;
     if (p.res && ((p.res_lo_off * 2) % 16 != 0 || (p.res_pitch * 2) % 16 != 0 || p.Cout % 32 != 0)) return false;
   }
@@ -1060,7 +527,7 @@ bool conv2d_tc_supported(const ConvParams& p, int x_dtype, int out_dtype) {
 int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   using namespace tc;
   KParams kp;
-  kp.scale = p.scale; kp.bias = p.bias; kp.res = p.res; kp.res_pitch = p.res_pitch; kp.act = p.act; kp.Cout = p.Cout;
+  kp.scale = p.scale; kp.bias = p.bias; kp.res = p.res; kp.act = p.act; kp.Cout = p.Cout;
   kp.KH = p.KH; kp.KW = p.KW; kp.pad = p.pad;
   const int Clog = p.split3 ? p.Cin / 3 : p.Cin;
   const int BK = (Clog % 64 == 0) ? 64 : 32;
@@ -1080,16 +547,8 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
     if (p.M > 0x7fffffffLL) { set_error("conv_tc: M too large"); return FB200_ERR_UNSUPPORTED; }
     W = Wo = (int)p.M; H = Ho = 1; B = 1;
   }
-  // halo mode (see is_halo): 32-channel 3x3 stride-1 convs, fp16 in, no residual.  FB200_TC_HALO=0 disables, =2 also sets the descriptor base offset
-  static int halo_env = -1;
-  if (halo_env < 0) { const char* e = getenv("FB200_TC_HALO"); halo_env = e ? atoi(e) : 1; }
-  const bool halo_shape = halo_env != 0 && BK == 32 && Clog == 32 && p.KH == 3 && p.KW == 3 && p.stride == 1 && p.pad == 1 && !p.res && p.w_bs == 0 &&
-                          !p.rowmax && (p.act & 15) != FB200_ACT_GELU && Wo >= 64 && p.Cout <= 64;
-  const bool halo = halo_shape && (!p.split3 || p.out_dtype == FB200_F32 || p.out_dtype == FB200_F16PAIR);
-  kp.halo_boff = halo_env == 2 ? 1 : 0;
   int BW = 1, BH = 1;
-  if (halo) { BW = 128; BH = 1; kp.num_k_blocks = 3; }
-  else choose_tile(Ho, Wo, &BW, &BH);
+  choose_tile(Ho, Wo, &BW, &BH);
   kp.BW = BW; kp.BH = BH; kp.tiles_w = (Wo + BW - 1) / BW; kp.tiles_h = (Ho + BH - 1) / BH; kp.Ho = Ho; kp.Wo = Wo;
   const int64_t m_tiles = (int64_t)B * kp.tiles_w * kp.tiles_h;
 
@@ -1099,7 +558,7 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   if (!kp.stride2) {
     const uint64_t dims[4] = {(uint64_t)(p.split3 ? kp.lo_off + Clog : p.Cin), (uint64_t)W, (uint64_t)H, (uint64_t)B};
     const uint64_t str[4] = {1, P, P * W, P * W * H};
-    const uint32_t box[4] = {(uint32_t)BK, (uint32_t)(halo ? BW + 2 : BW), (uint32_t)BH, 1};
+    const uint32_t box[4] = {(uint32_t)BK, (uint32_t)BW, (uint32_t)BH, 1};
     rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "A", swz);
   } else {
     const uint64_t dims[5] = {2 * P, (uint64_t)W / 2, 2, (uint64_t)H / 2, (uint64_t)B};
@@ -1109,21 +568,16 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   }
   if (rc) return rc;
 
-  auto run = [&](auto blockn_tag, auto stages_tag, auto minb_tag, auto bk_tag, auto nstg_tag, auto gelu_tag, auto cta2_tag, auto fs_tag) -> int {
-    constexpr bool C2_ = decltype(cta2_tag)::value;
+  auto run = [&](auto blockn_tag, auto stages_tag, auto bk_tag, auto gelu_tag, auto fs_tag) -> int {
     constexpr bool FS_ = decltype(fs_tag)::value;
     constexpr int BN_ = decltype(blockn_tag)::value;
     constexpr int ST_ = decltype(stages_tag)::value;
-    constexpr int MB_ = decltype(minb_tag)::value;
     constexpr int BK_ = decltype(bk_tag)::value;
-    constexpr int NS_ = decltype(nstg_tag)::value;
+    constexpr int NS_ = 2;  // double-buffered output staging
     {
       const uint64_t dims[3] = {(uint64_t)p.K, (uint64_t)p.Cout, (uint64_t)p.B};
       const uint64_t str[3] = {1, (uint64_t)p.K, (uint64_t)p.w_bs};
-      static int dbg_env = -1;
-      if (dbg_env < 0) { const char* e = getenv("FB200_TC_DBG"); dbg_env = e ? atoi(e) : 0; }
-      const int split_b = (!C2_ && (dbg_env & 64) && BN_ >= 128) ? ((dbg_env & 128) ? 4 : 2) : 1;  // experiment: the B tile as 2 / 4 TMA instructions
-      const uint32_t box[3] = {(uint32_t)phys_k<BK_>(), (uint32_t)((C2_ ? BN_ / 2 : BN_) / split_b), 1};  // CTA pair: each CTA loads half of the N tile
+      const uint32_t box[3] = {(uint32_t)BK_, (uint32_t)BN_, 1};
       int r2 = encode(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, p.w_bs ? 3 : 2, const_cast<void*>(p.w), dims, str, box, "W", swz);
       if (r2) return r2;
     }
@@ -1155,116 +609,60 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
       const uint32_t box[4] = {(uint32_t)(out16 ? 64 : 32), (uint32_t)BW, (uint32_t)BH, 1};
       int r2 = encode(&td, out16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out16 ? 2 : 4, 4, p.out, dims, str, box, "D");
       if (r2) return r2;
-      td2 = td;
-    }
-    if (!outp) { tr = td; tr2 = td; }  // residual: same geometry as the output, its own pointer / pitch
-    if (p.res && !outp) {
-      const uint64_t RP = (uint64_t)p.res_pitch;
-      const uint64_t dims[4] = {(uint64_t)p.Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B};
-      const uint64_t str[4] = {1, RP, RP * Wo, RP * Wo * Ho};
-      const uint32_t box[4] = {(uint32_t)(out16 ? 64 : 32), (uint32_t)BW, (uint32_t)BH, 1};
-      int r2 = encode(&tr, out16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out16 ? 2 : 4, 4, const_cast<void*>(p.res), dims, str, box, "R");
-      if (r2) return r2;
+      td2 = td; tr = td; tr2 = td;  // residual: same geometry as the output, its own pointer / pitch
+      if (p.res) {
+        const uint64_t RP = (uint64_t)p.res_pitch;
+        const uint64_t rstr[4] = {1, RP, RP * Wo, RP * Wo * Ho};
+        r2 = encode(&tr, out16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out16 ? 2 : 4, 4, const_cast<void*>(p.res), dims, rstr, box, "R");
+        if (r2) return r2;
+      }
     }
     KParams k2 = kp;
-    if constexpr (FS_ && BK_ != 96) {  // fused split: k-blocks run over (tap, 64-channel chunk); the hi / lo halves of both operands travel together
-      k2.cchunks = Clog / 64;
+    if constexpr (FS_) {  // fused split: k-blocks run over (tap, channel chunk); the hi / lo halves of both operands travel together
+      k2.cchunks = Clog / BK_;
       k2.num_k_blocks = p.KH * p.KW * k2.cchunks;
       k2.seg_chunks = 0;
     }
     k2.n_tiles = (p.Cout + BN_ - 1) / BN_;
-    k2.nimg = B;
-    k2.trace = g_trace;
-    const int64_t total = (C2_ ? (m_tiles + 1) / 2 : m_tiles) * k2.n_tiles;
+    const int64_t total = m_tiles * k2.n_tiles;
     if (total > 0x7fffffffLL) { set_error("conv_tc: too many tiles (%lld)", (long long)total); return FB200_ERR_UNSUPPORTED; }
     k2.total_tiles = (int)total;
-    { static int dbg = -1; if (dbg < 0) { const char* e = getenv("FB200_TC_DBG"); dbg = e ? atoi(e) : 0; } k2.dbg = dbg; }
-    { static int rt = -1; if (rt < 0) { const char* e = getenv("FB200_TC_RES_TMA"); rt = e ? atoi(e) : 1; } k2.res_tma = (p.res && rt) ? 1 : 0; }
-    if (outp) k2.res_tma = p.res ? 1 : 0;  // pair residuals only come through TMA
-    { static int nc = -1; if (nc < 0) { const char* e = getenv("FB200_TC_NCAT"); nc = e ? atoi(e) : 1; } k2.ncat = (nc && !p.rowmax) ? 1 : 0; }
-    if constexpr (decltype(gelu_tag)::value) return launch<BN_, ST_, __half, MB_, BK_, NS_, true>(ta, tb, td, tr, td2, tr2, k2, st);
+    if constexpr (decltype(gelu_tag)::value) return launch<BN_, ST_, __half, BK_, NS_, true>(ta, tb, td, tr, td2, tr2, k2, st);
     else if constexpr (FS_) {  // fp32 or pair output (checked by the caller)
-      if constexpr (NS_ >= 2) { if (outp) return launch<BN_, ST_, PairOut, MB_, BK_, NS_, false, C2_, true>(ta, tb, td, tr, td2, tr2, k2, st); }
-      if (outp) { set_error("conv_tc: pair output needs a double-buffered staging configuration"); return FB200_ERR_UNSUPPORTED; }
-      return launch<BN_, ST_, float, MB_, BK_, NS_, false, C2_, true>(ta, tb, td, tr, td2, tr2, k2, st);
+      if (outp) return launch<BN_, ST_, PairOut, BK_, NS_, false, true>(ta, tb, td, tr, td2, tr2, k2, st);
+      return launch<BN_, ST_, float, BK_, NS_, false, true>(ta, tb, td, tr, td2, tr2, k2, st);
     } else {
       if (outp) { set_error("conv_tc: pair output is only produced by the fused-split configurations"); return FB200_ERR_UNSUPPORTED; }
-      if (out16) return launch<BN_, ST_, __half, MB_, BK_, NS_, false, C2_>(ta, tb, td, tr, td2, tr2, k2, st);
-      return launch<BN_, ST_, float, MB_, BK_, NS_, false, C2_>(ta, tb, td, tr, td2, tr2, k2, st);
+      if (out16) return launch<BN_, ST_, __half, BK_, NS_, false>(ta, tb, td, tr, td2, tr2, k2, st);
+      return launch<BN_, ST_, float, BK_, NS_, false>(ta, tb, td, tr, td2, tr2, k2, st);
     }
   };
-  typedef std::false_type C1;
-  typedef std::true_type C2;
+  using std::integral_constant;
   typedef std::false_type NF;  // segmented K (or no split)
   typedef std::true_type FS;   // fused split
-  using std::integral_constant;
   typedef integral_constant<int, 64> K64;
   typedef integral_constant<int, 32> K32;
-  typedef integral_constant<int, 1> I1;
-  typedef integral_constant<int, 2> I2;
+  typedef integral_constant<int, 128> N128;
+  typedef integral_constant<int, 64> N64;
+  typedef integral_constant<int, 4> S4;
+  typedef integral_constant<int, 3> S3;
   if ((p.act & 15) == FB200_ACT_GELU)  // exact-erf GELU: dedicated instantiation (fp16 out, Cin % 64 == 0; checked in conv2d_tc_supported)
-    return run(integral_constant<int, 128>{}, integral_constant<int, 4>{}, I1{}, K64{}, I2{}, std::true_type{}, C1{}, NF{});
-  typedef integral_constant<int, 96> K96;  // halo mode tag
-  if (halo && p.split3) {  // fp32-accurate: hi and lo strips, W_hi and W_lo of all nine taps resident (74 / 37 KiB), one CTA per SM
-    if (p.Cout > 32) return run(integral_constant<int, 64>{}, integral_constant<int, 4>{}, I1{}, K96{}, I2{}, std::false_type{}, C1{}, FS{});
-    return run(integral_constant<int, 32>{}, integral_constant<int, 4>{}, I1{}, K96{}, I2{}, std::false_type{}, C1{}, FS{});
-  }
-  if (halo) {
-    if (p.Cout > 32) return run(integral_constant<int, 64>{}, integral_constant<int, 4>{}, I2{}, K96{}, I2{}, std::false_type{}, C1{}, NF{});
-    return run(integral_constant<int, 32>{}, integral_constant<int, 4>{}, I2{}, K96{}, I2{}, std::false_type{}, C1{}, NF{});
-  }
-  if (BK == 32) {  // stem convs (Cin = 32): HBM-bound, two CTAs per SM
-    if (p.Cout > 32) return run(integral_constant<int, 64>{}, integral_constant<int, 4>{}, I2{}, K32{}, I2{}, std::false_type{}, C1{}, NF{});
-    return run(integral_constant<int, 32>{}, integral_constant<int, 4>{}, I2{}, K32{}, I2{}, std::false_type{}, C1{}, NF{});
-  }
-  static int force_bn = -1;  // tuning aid: FB200_TC_BN=64|128|256
-  if (force_bn < 0) { const char* e = getenv("FB200_TC_BN"); force_bn = e ? atoi(e) : 0; }
-  if (force_bn == 64) return run(integral_constant<int, 64>{}, integral_constant<int, 3>{}, I2{}, K64{}, I2{}, std::false_type{}, C1{}, NF{});
-  if (force_bn == 128) return run(integral_constant<int, 128>{}, integral_constant<int, 4>{}, I1{}, K64{}, I2{}, std::false_type{}, C1{}, NF{});
-  if (force_bn == 256) return run(integral_constant<int, 256>{}, integral_constant<int, 3>{}, I1{}, K64{}, I2{}, std::false_type{}, C1{}, NF{});
-  const int64_t tiles256 = m_tiles * ((p.Cout + 255) / 256);
-  // CTA pairs (cta_group::2): the 256 x BLOCK_N tile of two SMs needs each weight tile only ONCE per pair - the single-CTA kernel is bound by the L2->SM
-  // operand bandwidth on every tensor-bound layer (48 KB per 128x256x64 MMA block = 19 TB/s at the tensor peak vs ~12 TB/s of L2)
-  if (g_cta_pair_mode < 0) { const char* e = getenv("FB200_TC_CTA2"); g_cta_pair_mode = e ? atoi(e) : 1; }  // env default, fb200_set_option overrides
-  const bool pair_ok = g_cta_pair_mode != 0 && !p.rowmax && !kp.w_batched;
-  const bool force_pair = g_cta_pair_mode == 2;
-  static int cfg_env = -1;  // experiment knob FB200_TC_CFG: 1 = CTA pairs with a 5-deep ring and single staging buffers
-  if (cfg_env < 0) { const char* e = getenv("FB200_TC_CFG"); cfg_env = e ? atoi(e) : 0; }
-  // fp32-accurate mode on 64-channel chunks: fused split (one TMA pass over A_hi, A_lo, W_hi, W_lo per chunk instead of three segmented passes): the TMA
-  // engine delivers ~65-80 B/cycle/SM plus ~110 cycles per instruction (profiles/r02_conv_timeline.md), the segmented layout needs 96 B/cycle at the tensor peak
-  static int fs_env = -1;  // FB200_TC_FS=0 disables
-  if (fs_env < 0) { const char* e = getenv("FB200_TC_FS"); fs_env = e ? atoi(e) : 1; }
-  const bool out_pair = p.out_dtype == FB200_F16PAIR;
-  // (per-image weights: the single-CTA fused-split configurations only - the CTA-pair producer has no 3-D weight loads)
-  if (fs_env && p.split3 && BK == 64 && (p.out_dtype == FB200_F32 || out_pair) && (!kp.w_batched || (p.Cout <= 128 && !out_pair))) {
-    // deep K loops want the 3-stage ring (and have a long main loop to hide a single staging buffer behind); layers with a residual (fetched by TMA into the
-    // SECOND staging buffer) or a short K loop are bound by the epilogue / HBM: two stages, double-buffered staging
-    const bool deep = !p.res && !out_pair && p.KH * p.KW * (Clog / 64) > 4;  // (pair output needs both staging buffers: one per plane pair in flight)
-    if (p.Cout > 128 && g_cta_pair_mode != 0) {
-      if (deep) return run(integral_constant<int, 256>{}, integral_constant<int, 3>{}, I1{}, K64{}, I1{}, std::false_type{}, C2{}, FS{});   // pair: 3 x 64 + 32 KiB
-      return run(integral_constant<int, 256>{}, integral_constant<int, 2>{}, I1{}, K64{}, I2{}, std::false_type{}, C2{}, FS{});             // pair: 2 x 64 + 64 KiB
+    return run(N128{}, S4{}, K64{}, std::true_type{}, NF{});
+  // fp32-accurate mode: fused split (one TMA pass over A_hi, A_lo, W_hi, W_lo per chunk instead of three segmented passes over the operands)
+  if (p.split3 && (p.out_dtype == FB200_F32 || p.out_dtype == FB200_F16PAIR)) {
+    if (BK == 64) {
+      if (p.Cout > 64) return run(N128{}, S3{}, K64{}, std::false_type{}, FS{});   // 3 x 64 + 32 KiB
+      return run(N64{}, S4{}, K64{}, std::false_type{}, FS{});                     // 4 x 48 + 32 KiB
     }
-    if (p.Cout > 128 && !out_pair)
-      return run(integral_constant<int, 256>{}, integral_constant<int, 2>{}, I1{}, K64{}, I1{}, std::false_type{}, C1{}, FS{});   // 2 x 96 + 32 KiB
-    if (p.Cout > 64) {
-      if (deep) return run(integral_constant<int, 128>{}, integral_constant<int, 3>{}, I1{}, K64{}, I1{}, std::false_type{}, C1{}, FS{});   // 3 x 64 + 32 KiB
-      return run(integral_constant<int, 128>{}, integral_constant<int, 2>{}, I1{}, K64{}, I2{}, std::false_type{}, C1{}, FS{});             // 2 x 64 + 64 KiB
-    }
-    return run(integral_constant<int, 64>{}, integral_constant<int, 3>{}, I1{}, K64{}, I2{}, std::false_type{}, C1{}, FS{});      // 3 x 48 + 32 KiB (HBM-bound layers)
+    if (p.Cout > 64) return run(N128{}, S4{}, K32{}, std::false_type{}, FS{});     // 4 x 32 + 32 KiB
+    return run(N64{}, S4{}, K32{}, std::false_type{}, FS{});                       // 4 x 24 + 32 KiB
   }
-  if (cfg_env == 1 && pair_ok && p.Cout > 128 && !p.res)
-    return run(integral_constant<int, 256>{}, integral_constant<int, 5>{}, I1{}, K64{}, I1{}, std::false_type{}, C2{}, NF{});   // 5 x 32 + 32 KiB
-  // single-product pairs only pay on the deep 3x3 layers (K >= 2304); on 1x1 layers the pair's extra synchronisation costs more than the halved weight traffic gains
-  const bool pair_shape = force_pair || (p.KH == 3 && Clog >= 256);
-  if (pair_ok && pair_shape && p.Cout > 128 && (tiles256 >= 148 || force_pair))
-    return run(integral_constant<int, 256>{}, integral_constant<int, 4>{}, I1{}, K64{}, I2{}, std::false_type{}, C2{}, NF{});   // 4 x 32 + 64 KiB
-  if (pair_ok && force_pair && p.Cout > 64 && p.Cout <= 128)
-    return run(integral_constant<int, 128>{}, integral_constant<int, 6>{}, I1{}, K64{}, I2{}, std::false_type{}, C2{}, NF{});   // 6 x 24 + 64 KiB
-  if (p.Cout > 128 && tiles256 >= 148)
-    return run(integral_constant<int, 256>{}, integral_constant<int, 3>{}, I1{}, K64{}, I2{}, std::false_type{}, C1{}, NF{});   // 144 + 64 KiB
-  if (p.Cout > 64)
-    return run(integral_constant<int, 128>{}, integral_constant<int, 4>{}, I1{}, K64{}, I2{}, std::false_type{}, C1{}, NF{});   // 128 + 64 KiB
-  return run(integral_constant<int, 64>{}, integral_constant<int, 3>{}, I2{}, K64{}, I2{}, std::false_type{}, C1{}, NF{});      // 72 + 32 KiB, 2 CTAs/SM
+  if (BK == 32) {  // stem convs (Cin = 32)
+    if (p.Cout > 64) return run(N128{}, S4{}, K32{}, std::false_type{}, NF{});
+    return run(N64{}, S4{}, K32{}, std::false_type{}, NF{});
+  }
+  if (p.Cout > 64) return run(N128{}, S4{}, K64{}, std::false_type{}, NF{});       // 4 x 32 + 32 KiB
+  return run(N64{}, S4{}, K64{}, std::false_type{}, NF{});                         // 4 x 24 + 32 KiB
 }
 
 }  // namespace fb200

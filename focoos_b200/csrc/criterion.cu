@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(256) loss_boxes_kernel(const float* __restrict
 }
 
 // Varifocal loss over every (query, class) logit: weight * BCE-with-logits(x, iou * onehot), weight and target detached.
-constexpr int VFL_BLOCKS = 148;
+constexpr int VFL_BLOCKS = kNumSMs;
 __global__ void __launch_bounds__(256) loss_vfl_kernel(const float* __restrict__ logits, const int* __restrict__ tclass, const float* __restrict__ tscore,
                                                         int64_t rows, int C, float alpha, float gamma, float inv_nb, float* __restrict__ grad,
                                                         float* __restrict__ partial) {
@@ -284,7 +284,7 @@ extern "C" int fb200_detr_match_cost(const float* logits, const float* boxes, co
   FB_CHECK_ARG(logits && boxes && tgt_labels && tgt_boxes && tgt_offsets && cost, "detr_match_cost: null pointer");
   FB_CHECK_ARG(L > 0 && B > 0 && Q > 0 && C > 0 && T > 0, "detr_match_cost: bad sizes L=%d B=%d Q=%d C=%d T=%d", L, B, Q, C, T);
   const int64_t total = (int64_t)L * T * Q;
-  match_cost_kernel<<<(unsigned)std::min<int64_t>(cdiv(total, 256), 148 * 8), 256, 0, (cudaStream_t)stream>>>(
+  match_cost_kernel<<<(unsigned)std::min<int64_t>(cdiv(total, 256), kNumSMs * 8), 256, 0, (cudaStream_t)stream>>>(
       logits, boxes, tgt_labels, tgt_boxes, tgt_offsets, L, B, Q, C, T, w_class, w_bbox, w_giou, alpha, gamma, cost);
   FB_CHECK_LAUNCH("detr_match_cost");
   return FB200_OK;

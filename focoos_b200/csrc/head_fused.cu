@@ -176,7 +176,7 @@ __global__ void sigmoid_rows_kernel(const float* __restrict__ x, int x_pitch, in
 
 static inline unsigned grid_1d(int64_t work, int threads) {
   const int64_t b = cdiv(work, threads);
-  return (unsigned)(b < 1 ? 1 : (b > 148 * 32 ? 148 * 32 : b));
+  return (unsigned)(b < 1 ? 1 : (b > kNumSMs * 32 ? kNumSMs * 32 : b));
 }
 
 }  // namespace fb200

@@ -9,7 +9,7 @@ namespace fb200 {
 
 static inline unsigned grid_cap(int64_t total, int threads) {
   int64_t g = cdiv(total, threads);
-  const int64_t cap = 148LL * 32;
+  const int64_t cap = (int64_t)kNumSMs * 32;
   return (unsigned)(g < cap ? (g > 0 ? g : 1) : cap);
 }
 

@@ -192,7 +192,7 @@ extern "C" int fb200_attention_split(const float* q, int q_pitch, const float* k
 
 // ------------------------------------------------------------------------------------------------
 // fp16 tensor-core attention (head_dim 32): legacy mma.sync.m16n8k16 is the right tool here — per (batch, head) the
-// problem is 300..400 x 32, far below one tcgen05 tile; the whole K and V of a head stay in shared memory and each
+// problem is 300..400 x 32, far below one wgmma tile; the whole K and V of a head stay in shared memory and each
 // warp runs a flash-style online softmax over 64-key blocks for 16 queries.  4 warps = 64 queries per CTA.
 // ------------------------------------------------------------------------------------------------
 namespace fb200 {

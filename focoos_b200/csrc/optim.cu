@@ -10,7 +10,7 @@
 namespace fb200 {
 namespace {
 
-constexpr int STATS_BLOCKS = 148 * 4;
+constexpr int STATS_BLOCKS = kNumSMs * 4;
 
 __global__ void __launch_bounds__(256) grad_stats_kernel(const float* __restrict__ g, int64_t n, double* __restrict__ partial, int* __restrict__ flags) {
   const int tid = threadIdx.x;

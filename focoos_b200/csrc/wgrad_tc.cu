@@ -1,24 +1,25 @@
-// tcgen05 weight-gradient GEMM for sm_100a, fp32-accurate through split-precision fp16 products.
+// wgmma weight-gradient GEMM for sm_90a, fp32-accurate through split-precision fp16 products.
 //
 //   dW[co, kh, kw, ci] = sum over output pixels p of  dY[p, co] * X[pix(p, kh, kw), ci]          (stride-1 convs and linears)
 //
 // GEMM view per filter tap: D[M = Cout, N = Cin] = A^T B with the reduction over PIXELS.  In NHWC both operands are stored
 // pixel-major with channels contiguous, i.e. they are "MN-major" for the tensor core: a TMA box of 64 pixels x 64 channels lands in
 // shared memory as 8 swizzle atoms of (8 pixels x 128 B) - exactly the canonical SWIZZLE_128B MN-major layout
-// ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units (cute/atom/mma_traits_sm100.hpp), so no transpose is ever materialised:
-//   SBO = 1024 B (next 8-pixel group), LBO = 8192 B (next 64-channel block = the next TMA box), instruction descriptor with
-//   a_major = b_major = MN.  The X box is the dY box shifted by the tap offset; out-of-bounds rows/columns (conv zero padding, ragged
+// ((8,8,n),(8,k)):((1,8,LBO),(64,SBO)) in elements (cute/arch/mma_sm90_desc.hpp), so no transpose is ever materialised:
+//   SBO = 1024 B (next 8-pixel group), LBO = 8192 B (next 64-channel block = the next TMA box), wgmma with both operands
+//   transposed (MN-major).  The X box is the dY box shifted by the tap offset; out-of-bounds rows/columns (conv zero padding, ragged
 //   pixel tiles) are zero-filled by the TMA unit for BOTH operands, so ragged tiles contribute exact zeros.
 // fp32 accuracy: operands are the [hi | lo] fp16 pairs of the fp32 tensors (fb200_split_f32_pair); each 64-pixel K chunk issues
-//   dY_hi*X_hi + dY_hi*X_lo + dY_lo*X_hi  into the same fp32 TMEM accumulator (error ~2^-21 relative, like the forward mode).
-// Parallelism: work item = (128 x BLOCK_N weight tile, tap, pixel split); persistent CTAs, warp-specialised
-//   (TMA producer / MMA issuer / TMEM allocator / 4 epilogue warps), 3-stage smem ring, 2 TMEM accumulator stages;
+//   dY_hi*X_hi + dY_hi*X_lo + dY_lo*X_hi  into the same fp32 register accumulator (error ~2^-21 relative, like the forward mode).
+// Parallelism: work item = (128 x BLOCK_N weight tile, tap, pixel split); persistent CTAs, warp-specialised (one TMA producer thread,
+//   two consumer warp-groups that each own 64 output channels of the tile), 3-stage smem ring;
 //   split partials are reduced in a fixed order by wgrad_reduce_kernel (reproducible, no atomics).
 #include <cuda.h>
 
 #include <cstdlib>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace fb200 {
 namespace wg {
@@ -54,53 +55,27 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
                ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
-// MN-major SWIZZLE_128B shared-memory matrix descriptor: LBO = stride between 64-element MN blocks, SBO = stride between 8-row K groups
+// MN-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 format): LBO = stride between 64-element MN blocks, SBO = stride between 8-row K groups
 __device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)(BOX_BYTES >> 4) << 16;  // leading byte offset: next 64-channel block (next TMA box)
   d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset: next group of 8 pixels
-  d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                 // SWIZZLE_128B
   return d;
-}
-// instruction descriptor: D = F32, A = B = F16, A and B MN-major (bits 15, 16), N at bits 17.., M = 128 at bits 24..
-__host__ __device__ constexpr uint32_t make_idesc_mn(int n) {
-  return (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 template <int BLOCK_N> __host__ __device__ constexpr int a_boxes() { return 2 * (BLOCK_M / 64); }   // hi + lo, 64 channels per box
 template <int BLOCK_N> __host__ __device__ constexpr int b_boxes() { return 2 * (BLOCK_N / 64); }
 template <int BLOCK_N> __host__ __device__ constexpr int stage_bytes() { return (a_boxes<BLOCK_N>() + b_boxes<BLOCK_N>()) * BOX_BYTES; }
-template <int BLOCK_N> constexpr int smem_bytes() { return STAGES * stage_bytes<BLOCK_N>() + (2 * STAGES + 4) * 8 + 16 + 1024; }
+template <int BLOCK_N> constexpr int smem_bytes() { return STAGES * stage_bytes<BLOCK_N>() + 2 * STAGES * 8 + 1024; }
 
 template <int BLOCK_N>
-__global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x, const WParams p) {
+__global__ void __launch_bounds__(384, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x, const WParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int A_BOXES = a_boxes<BLOCK_N>(), B_BOXES = b_boxes<BLOCK_N>();
@@ -108,29 +83,15 @@ __global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant_
   constexpr int A_HALF = (A_BOXES / 2) * BOX_BYTES, B_HALF = (B_BOXES / 2) * BOX_BYTES;  // bytes of the hi (or lo) part
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;  // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;  // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t TMEM_COLS = 2 * BLOCK_N;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_dy) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full_bar[i], 1); mbar_init(&tmem_empty_bar[i], 4); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }  // one arrival per consumer warp
     fence_barrier_init();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int tiles_per_img = p.tiles_w * p.tiles_h;
 
   // work item -> (split, tap, n tile, m tile); n fastest so CTAs running together share dY boxes in L2
@@ -141,111 +102,87 @@ __global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant_
     split = item / p.taps;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {  // ================================================================= TMA producer
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
-        int mt, nt, tap, split;
-        decode(item, mt, nt, tap, split);
-        const int m0 = mt * BLOCK_M, n0 = nt * BLOCK_N;
-        const int kh = tap / p.KW, kw = tap - kh * p.KW;
-        const int pt_begin = split * p.pt_per_split, pt_end = min(p.pt_total, pt_begin + p.pt_per_split);
-        for (int pt = pt_begin; pt < pt_end; ++pt) {
-          const int img = pt / tiles_per_img, rem = pt - img * tiles_per_img;
-          const int h0 = (rem / p.tiles_w) * p.BH, w0 = (rem % p.tiles_w) * p.BW;
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)(p.single ? STAGE_BYTES / 2 : STAGE_BYTES));
-          uint8_t* sa = smem + stage * STAGE_BYTES;
-          uint8_t* sb = sa + A_BOXES * BOX_BYTES;
-          const int halves = p.single ? 1 : 2;
-          for (int half = 0; half < halves; ++half) {  // 0 = hi, 1 = lo (channel offset C in the pair tensor)
-#pragma unroll
-            for (int j = 0; j < BLOCK_M / 64; ++j)
-              tma_load_4d(&tmap_dy, &full_bar[stage], sa + half * A_HALF + j * BOX_BYTES, half * p.Cout + m0 + j * 64, w0, h0, img);
-#pragma unroll
-            for (int j = 0; j < BLOCK_N / 64; ++j)
-              tma_load_4d(&tmap_x, &full_bar[stage], sb + half * B_HALF + j * BOX_BYTES, half * p.Cin + n0 + j * 64, w0 * p.stride + kw - p.pad,
-                          h0 * p.stride + kh - p.pad, img);  // stride 2: the X map traverses every second pixel (TMA element strides)
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ================================================================= MMA issuer
-      constexpr uint32_t idesc = make_idesc_mn(BLOCK_N);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
-        int mt, nt, tap, split;
-        decode(item, mt, nt, tap, split);
-        const int pt_begin = split * p.pt_per_split, pt_end = min(p.pt_total, pt_begin + p.pt_per_split);
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BLOCK_N);
-        bool first = true;
-        for (int pt = pt_begin; pt < pt_end; ++pt) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES), sb = sa + A_BOXES * BOX_BYTES;
-          const uint64_t a_hi = make_desc_mn(sa), a_lo = make_desc_mn(sa + A_HALF);
-          const uint64_t b_hi = make_desc_mn(sb), b_lo = make_desc_mn(sb + B_HALF);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k) {  // 16 pixels = two 8-pixel groups = 2048 B: +128 in 16-byte units
-            const uint64_t adv = (uint64_t)(k * 128);
-            umma_f16(tmem_d, a_hi + adv, b_hi + adv, idesc, first ? 0u : 1u);
-            first = false;
-            if (!p.single) {
-              umma_f16(tmem_d, a_hi + adv, b_lo + adv, idesc, 1u);
-              umma_f16(tmem_d, a_lo + adv, b_hi + adv, idesc, 1u);
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {  // =================================================================== epilogue: TMEM -> split partial in global memory
-    const int ew = warp & 3;         // TMEM lane quarter this warp may access
-    const int row = ew * 32 + lane;  // accumulator row = output channel within the tile
-    int acc = 0;
-    uint32_t acc_phase = 0;
+  if (warp < 4) {
+    if (threadIdx.x != 0) return;  // ================================================================= TMA producer
+    int stage = 0;
+    uint32_t phase = 0;
     for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
       int mt, nt, tap, split;
       decode(item, mt, nt, tap, split);
-      const int co = mt * BLOCK_M + row, n0 = nt * BLOCK_N;
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tcgen05_fence_after();
-      float* dst = p.part + (((int64_t)split * p.Cout + co) * p.taps + tap) * p.Cin + n0;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc * BLOCK_N + c0), r);
-        if (co < p.Cout) {
-          if (n0 + c0 + 32 <= p.Cin && (p.Cin & 3) == 0) {
+      const int m0 = mt * BLOCK_M, n0 = nt * BLOCK_N;
+      const int kh = tap / p.KW, kw = tap - kh * p.KW;
+      const int pt_begin = split * p.pt_per_split, pt_end = min(p.pt_total, pt_begin + p.pt_per_split);
+      for (int pt = pt_begin; pt < pt_end; ++pt) {
+        const int img = pt / tiles_per_img, rem = pt - img * tiles_per_img;
+        const int h0 = (rem / p.tiles_w) * p.BH, w0 = (rem % p.tiles_w) * p.BW;
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)(p.single ? STAGE_BYTES / 2 : STAGE_BYTES));
+        uint8_t* sa = smem + stage * STAGE_BYTES;
+        uint8_t* sb = sa + A_BOXES * BOX_BYTES;
+        const int halves = p.single ? 1 : 2;
+        for (int half = 0; half < halves; ++half) {  // 0 = hi, 1 = lo (channel offset C in the pair tensor)
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) *reinterpret_cast<uint4*>(dst + c0 + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-          } else {
+          for (int j = 0; j < BLOCK_M / 64; ++j)
+            tma_load_4d(&tmap_dy, &full_bar[stage], sa + half * A_HALF + j * BOX_BYTES, half * p.Cout + m0 + j * 64, w0, h0, img);
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (n0 + c0 + j < p.Cin) dst[c0 + j] = __uint_as_float(r[j]);
-          }
+          for (int j = 0; j < BLOCK_N / 64; ++j)
+            tma_load_4d(&tmap_x, &full_bar[stage], sb + half * B_HALF + j * BOX_BYTES, half * p.Cin + n0 + j * 64, w0 * p.stride + kw - p.pad,
+                        h0 * p.stride + kh - p.pad, img);  // stride 2: the X map traverses every second pixel (TMA element strides)
+        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+    return;
+  }
+  // ===================================================================== consumers: warp-group g owns output channels m0 + 64g .. +63 (= dY box g)
+  const int ct = threadIdx.x - 128;
+  const int g = ct >> 7;
+  const int row = g * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2);  // accumulator rows row and row + 8
+  const int cq = 2 * (lane & 3);
+  float acc[BLOCK_N / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
+    int mt, nt, tap, split;
+    decode(item, mt, nt, tap, split);
+    const int pt_begin = split * p.pt_per_split, pt_end = min(p.pt_total, pt_begin + p.pt_per_split);
+    int prev = -1;
+    for (int pt = pt_begin; pt < pt_end; ++pt) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + (uint32_t)(g * BOX_BYTES), sb = smem_u32(smem + stage * STAGE_BYTES) + A_BOXES * BOX_BYTES;
+      const uint64_t a_hi = make_desc_mn(sa), a_lo = make_desc_mn(sa + A_HALF);
+      const uint64_t b_hi = make_desc_mn(sb), b_lo = make_desc_mn(sb + B_HALF);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / 16; ++k) {  // 16 pixels = two 8-pixel groups = 2048 B: +128 in 16-byte units
+        const uint64_t adv = (uint64_t)(k * 128);
+        Wgmma<BLOCK_N, 1>::mma(acc, a_hi + adv, b_hi + adv, (pt > pt_begin || k > 0) ? 1u : 0u);
+        if (!p.single) {
+          Wgmma<BLOCK_N, 1>::mma(acc, a_hi + adv, b_lo + adv, 1u);
+          Wgmma<BLOCK_N, 1>::mma(acc, a_lo + adv, b_hi + adv, 1u);
         }
       }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous chunk's products are done: its stage may be refilled
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+    wgmma_wait<0>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    // registers -> split partial in global memory (Cin % 8 == 0: a column pair never straddles the end of a row)
+    const int n0 = nt * BLOCK_N;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int co = mt * BLOCK_M + row + 8 * h;
+      if (co >= p.Cout) continue;
+      float* dst = p.part + (((int64_t)split * p.Cout + co) * p.taps + tap) * p.Cin + n0;
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int c = 8 * j + cq;
+        if (n0 + c < p.Cin) *reinterpret_cast<float2*>(dst + c) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
+    }
   }
 }
 
@@ -284,7 +221,7 @@ static int encode_pair(CUtensorMap* m, const void* base, int C2, int W, int H, i
 
 static int num_sms() {
   static int n = 0;
-  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
   return n;
 }
 
@@ -372,11 +309,11 @@ static int wgrad_tc_launch(const void* x_pair, int B, int H, int W, int Cin, con
     static bool cfg = false;
     if (!cfg) { cudaFuncSetAttribute(wgrad_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<128>()); cfg = true; }
     static_assert(smem_bytes<128>() <= 227 * 1024, "shared memory budget exceeded");
-    wgrad_tc_kernel<128><<<grid, 256, smem_bytes<128>(), st>>>(tdy, tx, p);
+    wgrad_tc_kernel<128><<<grid, 384, smem_bytes<128>(), st>>>(tdy, tx, p);
   } else {
     static bool cfg = false;
     if (!cfg) { cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<64>()); cfg = true; }
-    wgrad_tc_kernel<64><<<grid, 256, smem_bytes<64>(), st>>>(tdy, tx, p);
+    wgrad_tc_kernel<64><<<grid, 384, smem_bytes<64>(), st>>>(tdy, tx, p);
   }
   FB_CHECK_LAUNCH("conv_wgrad_tc");
   const int64_t n = (int64_t)Cout * taps * Cin;

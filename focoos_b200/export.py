@@ -1,7 +1,7 @@
-"""`model.export` of the B200 path (SURVEY §8f.4) — mirror of `focoos/models/focoos_model.py:60-85,418-573` (ExportableModel, FocoosModel.export),
+"""`model.export` of the CUDA path (SURVEY §8f.4) — mirror of `focoos/models/focoos_model.py:60-85,418-573` (ExportableModel, FocoosModel.export),
 `focoos/infer/runtimes/torchscript.py:15-80` (TorchscriptRuntime) and the slice of `focoos/infer/infer_model.py` that serves an exported file.
 
-The reference exports by `torch.jit.trace(ExportableModel(model), 128 * randn(1,3,H,W))`: a graph of ~1000 aten ops.  The B200 engine is not a graph of
+The reference exports by `torch.jit.trace(ExportableModel(model), 128 * randn(1,3,H,W))`: a graph of ~1000 aten ops.  The CUDA engine is not a graph of
 torch ops (its kernels are called through the C ABI), so the exported graph is ONE custom operator
 
     focoos_b200::model_forward(Tensor images, Tensor[] weights, str meta) -> Tensor[]
@@ -162,7 +162,7 @@ class InferModel:
 def export_model(focoos_model, runtime_type: str = "torchscript_32", out_dir: Optional[str] = None, device: str = "cuda", overwrite: bool = True,
                  image_size: Optional[Union[int, Tuple[int, int]]] = None) -> InferModel:
     """FocoosModel.export (focoos_model.py:418-573) for the TorchScript runtime types; ONNX / TensorRT are the reference's other backends and are not part
-    of the B200 path (ValueError, like the reference for unsupported formats)."""
+    of the CUDA path (ValueError, like the reference for unsupported formats)."""
     rt = str(getattr(runtime_type, "value", runtime_type)).lower()
     if "torchscript" not in rt:
         raise ValueError(f"focoos_b200 exports TorchScript only (got runtime_type={runtime_type!r}); ONNX/TensorRT belong to the reference's own runtimes")

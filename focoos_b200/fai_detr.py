@@ -3,7 +3,7 @@
 The module TREE below mirrors the reference's (same attribute names, same parameter shapes) so that a
 reference `state_dict` / `model_final.pth` loads unchanged (SURVEY.md Appendix B), but the modules are only
 parameter containers: `FAIDetr.forward` runs `DetrEngine`, a fused NHWC graph of `focoos_b200.ops`
-calls (hand-written sm_100a kernels) built once from the weights:
+calls (hand-written sm_90a kernels) built once from the weights:
 
   * BatchNorm folded into per-channel scale/bias applied in the conv epilogue (nn/layers/conv.py:89),
   * RepVggBlock re-parameterised to one 3x3 conv (the reference's own `get_equivalent_kernel_bias`,
@@ -343,7 +343,7 @@ class DetrEngine:
     """Packs a FAIDetr state_dict for one (device, precision) and runs the fused forward."""
 
     _host_w3 = None  # set per instance in fp32_tc mode (see _to)
-    fuse_shortcut_pool = False  # fold the vd shortcut's AvgPool2d into a 2x2/s2 conv (slower on B200, see _pack_backbone)
+    fuse_shortcut_pool = False  # fold the vd shortcut's AvgPool2d into a 2x2/s2 conv (off by default, see _pack_backbone)
 
     def __init__(self, sd: Dict[str, torch.Tensor], cfg: DETRConfig, device, precision: str = "fp16", algo: int = ops.ALGO_AUTO):
         assert precision in ("fp32", "fp16", "fp32_tc")
@@ -590,7 +590,7 @@ class DetrEngine:
         return x
 
     def pair_capable(self) -> bool:
-        """the pair-native fp32_tc data flow is available (three products in every stage, default algorithm choice, a tcgen05 device or the CPU test backend)"""
+        """the pair-native fp32_tc data flow is available (three products in every stage, default algorithm choice, a tensor-core (sm_90) device or the CPU test backend)"""
         return (self.precision == "fp32_tc" and self.pair_native and self.algo == ops.ALGO_AUTO and all(v == 3 for v in getattr(self, "mix", {}).values())
                 and (ops._backend is not None or ops.supports_tcgen05_cached()))
 
@@ -669,7 +669,7 @@ class DetrEngine:
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
         if H % 32 or W % 32:
-            # the reference's torch graph takes any size (odd feature maps from ceil-mode pools / stride-2 convs); the B200 kernels tile the stride-2 layers on even
+            # the reference's torch graph takes any size (odd feature maps from ceil-mode pools / stride-2 convs); the kernels tile the stride-2 layers on even
             # maps, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
             raise ValueError(f"focoos_b200: input size {H}x{W} is not a multiple of 32; resize/pad the image (e.g. ModelInfo.im_size) before the model")
         global _products
@@ -927,7 +927,7 @@ class FAIDetr(nn.Module):
 
     def forward(self, images: torch.Tensor, targets: list = [], taps: Optional[dict] = None) -> DETRModelOutput:
         if ops._backend is None and not images.is_cuda:
-            raise RuntimeError("focoos_b200.FAIDetr runs on CUDA (sm_100a) only — no CPU fallback; move the model and inputs to the GPU")
+            raise RuntimeError("focoos_b200.FAIDetr runs on CUDA (sm_90a) only — no CPU fallback; move the model and inputs to the GPU")
         if self.training:  # modelling.py:1354-1356: losses only, empty logits/boxes
             assert targets is not None and len(targets) > 0, "targets should not be None or empty - training mode"
             outputs = self.train_graph().forward(images)

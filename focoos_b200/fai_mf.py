@@ -317,7 +317,7 @@ class MFEngine(DetrEngine):
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
         if H % 32 or W % 32:
-            # the reference's torch graph takes any size (odd feature maps from ceil-mode pools / stride-2 convs); the B200 kernels tile the stride-2 layers on even
+            # the reference's torch graph takes any size (odd feature maps from ceil-mode pools / stride-2 convs); the kernels tile the stride-2 layers on even
             # maps, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
             raise ValueError(f"focoos_b200: input size {H}x{W} is not a multiple of 32; resize/pad the image (e.g. ModelInfo.im_size) before the model")
         pair = self.pair_capable() and all(getattr(c, "w3", None) is not None for c in [self.pd_in] + [self.adapter[i] for i in (1, 2, 3)])
@@ -488,7 +488,7 @@ class FAIMaskFormer(nn.Module):
         if self.training or (targets is not None and len(targets) > 0):
             raise NotImplementedError("focoos_b200: losses / fine-tuning are not part of the inference hot path")
         if ops._backend is None and not images.is_cuda:
-            raise RuntimeError("focoos_b200.FAIMaskFormer runs on CUDA (sm_100a) only — no CPU fallback")
+            raise RuntimeError("focoos_b200.FAIMaskFormer runs on CUDA (sm_90a) only — no CPU fallback")
         eng = self.engine()
         eng.lazy_masks = bool(getattr(self, "lazy_masks", False))
         probs, masks = eng.forward(images if images.dtype == torch.uint8 else images.to(torch.float32), taps)

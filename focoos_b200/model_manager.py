@@ -1,7 +1,7 @@
 """ModelManager / FocoosModel — the reference's L5 facade for the detection hot path
 (`focoos/model_manager.py:43-91`, `focoos/models/focoos_model.py:100,370,575`).
 
-`ModelManager.get(name)` builds the B200-native model from the same registry JSON the reference ships
+`ModelManager.get(name)` builds the H100-native model from the same registry JSON the reference ships
 (`focoos/model_registry/<name>.json`, `config` section; a copy of the architecture section for the fai-detr
 family is embedded below since the reference tree is not present on the GPU box).  No network: weights come from
 `model_info["weights_path"]`, an explicit `state_dict=` argument, or stay at their initial values.
@@ -64,7 +64,7 @@ class FocoosModel:
         _, _, proc_cls, resize = _FAMILIES[model_info.model_family]
         self.processor = proc_cls(model.config, image_size=model_info.im_size if resize else None).eval()
         self.model.eval()
-        if torch.cuda.is_available():
+        if torch.cuda.is_available() and ops._backend is None:  # the tests' CPU reference operators take host tensors only
             self.model.cuda()
         # CUDA-graph cache of model.forward per (input shape, dtype): the eager forward is ~240 launches of partly very short kernels (the
         # decoder runs ahead of a Python host), so replaying a captured graph removes the host from the critical path of `infer` / `__call__`
@@ -210,7 +210,7 @@ class FocoosModel:
         """focoos_model.py:221-275: fine-tune on `data_train` (single process, or `args.num_gpus` processes with the NCCL gradient exchange), write
         `<output_dir>/<run_name>/model_final.pth` + `model_info.json`, reload the trained weights and return to eval mode."""
         from .trainer import run_train_entry
-        assert hub is None, "Focoos Hub sync is outside the B200 hot path"
+        assert hub is None, "Focoos Hub sync is outside the CUDA hot path"
         return run_train_entry(self, args, data_train, data_val)
 
     def eval(self, args, data_test, save_json: bool = True):
@@ -266,7 +266,7 @@ class ModelManager:
             r = _REGISTRY[name]
             model_info = ModelInfo(name=name, model_family=r.get("family", "fai_detr"), im_size=r["im_size"], config=dict(r["config"]))
         if model_info.model_family not in _FAMILIES:
-            raise ValueError(f"Model family {model_info.model_family} is not on the B200 hot path ({sorted(_FAMILIES)})")
+            raise ValueError(f"Model family {model_info.model_family} is not on the CUDA hot path ({sorted(_FAMILIES)})")
         cfg_cls, model_cls, _, _ = _FAMILIES[model_info.model_family]
         if config is None:
             cd = dict(model_info.config)

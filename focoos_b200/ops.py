@@ -1,4 +1,4 @@
-"""Operator surface of focoos_b200: torch tensors in, hand-written sm_100a kernels underneath.
+"""Operator surface of focoos_b200: torch tensors in, hand-written sm_90a kernels underneath.
 
 Every function below validates/allocates on the host and then calls ONE entry point of the C ABI
 declared in `include/focoos_b200.h` (loaded with ctypes from `focoos_b200/lib/libfocoos_b200.so`,
@@ -64,7 +64,7 @@ def load_library():
 
 
 EXPORTED_SYMBOLS = (
-    "fb200_last_error", "fb200_version", "fb200_device_supports_tcgen05", "fb200_set_option", "fb200_set_conv_trace", "fb200_stem_conv3x3s2", "fb200_stem_conv3x3s2_u8", "fb200_conv2d", "fb200_conv2d_per_image_weights", "fb200_linear_rowmax", "fb200_image_resize",
+    "fb200_last_error", "fb200_version", "fb200_device_supports_tcgen05", "fb200_stem_conv3x3s2", "fb200_stem_conv3x3s2_u8", "fb200_conv2d", "fb200_conv2d_per_image_weights", "fb200_linear_rowmax", "fb200_image_resize",
     "fb200_split_f32_pair", "fb200_conv2d_pair", "fb200_pair_pool", "fb200_linear_rowmax_pair",
     "fb200_maxpool3x3s2", "fb200_avgpool2x2_ceil", "fb200_resize_bilinear", "fb200_add", "fb200_layernorm",
     "fb200_attention", "fb200_attention_split", "fb200_msda", "fb200_row_select", "fb200_rowmax", "fb200_topk", "fb200_gather_rows",
@@ -388,22 +388,6 @@ def _be():
     return _cuda_backend
 
 
-OPT_CONV_CTA_PAIR = 0
-
-
-def set_option(option: int, value: int) -> int:
-    """process-wide tuning option of the C library (include/focoos_b200.h fb200_option); returns the previous value"""
-    rc = load_library().fb200_set_option(int(option), int(value))
-    if rc < 0:
-        _check(rc, "set_option")
-    return rc
-
-
-def set_conv_trace(buf: Optional[torch.Tensor]):
-    """debug timeline of conv_tc launches (see include/focoos_b200.h fb200_set_conv_trace); buf: int64 CUDA tensor [>= 296 * 128] or None"""
-    _check(load_library().fb200_set_conv_trace(_p(buf)), "set_conv_trace")
-
-
 def supports_tcgen05() -> bool:
     return load_library().fb200_device_supports_tcgen05() == 1
 
@@ -412,7 +396,7 @@ _tc_ok = None
 
 
 def supports_tcgen05_cached() -> bool:
-    """tcgen05 path usable (real sm_100 device; False under the tests' CPU backend hook)"""
+    """tensor-core path usable (real sm_90 device; False under the tests' CPU backend hook)"""
     global _tc_ok
     if _backend is not None:
         return False
@@ -512,7 +496,7 @@ def to_pair(x) -> Pair:
 
 
 def conv2d_pair(x: Pair, w3, scale=None, bias=None, *, stride=1, pad=0, act=ACT_NONE, residual=None, out=None, out_pair: bool = True):
-    """fp32-accurate conv (three fp16 tcgen05 products) on a pair-format input.  `out_pair`: write the result as a Pair (for a following conv / pair pool) or
+    """fp32-accurate conv (three fp16 wgmma products) on a pair-format input.  `out_pair`: write the result as a Pair (for a following conv / pair pool) or
     as a plain fp32 tensor (for the non-conv consumers: LayerNorm, attention, deformable attention, selection).  The residual has the output's format."""
     assert isinstance(x, Pair) and w3.dtype == torch.float16 and w3.shape[3] == 3 * x.C, (w3.shape, x.C)
     B, H, W, _ = x.shape

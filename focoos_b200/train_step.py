@@ -4,7 +4,7 @@
   TrainerLoop.run_step / clip_grads        focoos/trainer/trainer.py:723-794       (GradScaler(init 2^10), clip 0.1 twice, AdamW)
   create_ddp_model                         focoos/utils/distributed/dist.py:138-157 (DistributedDataParallel -> bucketed gradient all-reduce)
 
-B200 design: every trainable tensor lives in ONE flat fp32 buffer (parameters, gradients, both Adam moments: 4 x 174 MB
+Design: every trainable tensor lives in ONE flat fp32 buffer (parameters, gradients, both Adam moments: 4 x 174 MB
 for fai-detr-l), so the whole optimiser step is three launches (ops.grad_stats -> ops.optim_finalize -> ops.adamw_step)
 with the loss scale, the clip coefficient and the skip-on-inf decision kept in a device-side control block (no host
 sync), and the data-parallel exchange is an NCCL all-reduce of contiguous slices of the flat gradient buffer, issued

@@ -111,7 +111,7 @@ def _train_worker(rank: int, world: int, fm, args: TrainerArgs, data_train, data
         os.environ.update(RANK=str(rank), LOCAL_RANK=str(rank), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(args.master_port))
         torch.cuda.set_device(rank)
         D.init_from_env("nccl", torch.device("cuda", rank))
-    if ops._backend is not None and not torch.cuda.is_available():  # tests: host logic on the CPU reference operators
+    if ops._backend is not None:  # tests: host logic on the CPU reference operators (host tensors only)
         dev = torch.device("cpu")
     else:
         dev = torch.device("cuda", rank if world > 1 else torch.cuda.current_device())
@@ -177,7 +177,7 @@ def run_train_entry(fm, args: TrainerArgs, data_train, data_val=None):
     if not os.path.exists(path):
         raise FileNotFoundError(f"Training did not end correctly, model file not found at {path}")  # focoos_model.py:265
     fm.model.load_state_dict(torch.load(path, map_location="cpu", weights_only=True))
-    if torch.cuda.is_available():
+    if torch.cuda.is_available() and ops._backend is None:
         fm.model.cuda()
     fm.model.eval()
     fm.processor.eval()

@@ -4,7 +4,7 @@ No pretrained checkpoint is reachable offline and the reference's default init i
 (zero sampling-offset / attention-weight / bbox-head weights, identity BN statistics: every score
 < 0.03, see SURVEY.md §8c).  `seeded_state_dict` re-randomises *every* tensor of a `state_dict`
 from its NAME and SHAPE only (one CPU generator per key, seeded by crc32(name) ^ seed), so the
-reference model (in the oracle container) and the B200 model (on the GPU box) get bit-identical
+reference model (in the oracle container) and this project's model (on the GPU) get bit-identical
 weights without shipping a 176 MB file.  CPU `torch.randn`/`rand` with a fixed generator seed is
 reproducible for a fixed torch build (same image on both sides).
 """

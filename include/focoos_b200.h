@@ -1,9 +1,9 @@
 /*
- * focoos_b200 — C ABI of the B200-native (sm_100a) kernels behind the Focoos detection hot path.
+ * focoos_b200 — C ABI of the H100-native (sm_90a) kernels behind the Focoos detection hot path.
  *
  * The reference (FocoosAI/focoos v0.25.0) is pure Python: it has NO FFI boundary for this path; every
  * operator below replaces a chain of torch library calls at the cited reference call site
- * (paths relative to /root/reference/focoos).  The Python side of the boundary is
+ * (paths relative to the reference's `focoos/` package).  The Python side of the boundary is
  * `focoos_b200/ops.py` (ctypes + torch.library registration `focoos_b200::*`); the binding a
  * reference maintainer would add is shown in INTEGRATION.md.
  *
@@ -14,7 +14,7 @@
  *     `pitch >= C` in ELEMENTS, which lets a kernel read/write a channel slice of a wider tensor
  *     (concat-free CSP/FPN blocks).  Token tensors [B,L,C] are the same thing with H=1.
  *   - `dtype`: FB200_F32 (fp32 SIMT kernels; the near-bit-exact parity mode) or FB200_F16
- *     (fp16 storage, fp32 accumulate; tcgen05 tensor cores for conv / linear).
+ *     (fp16 storage, fp32 accumulate; wgmma tensor cores for conv / linear).
  *   - Work is enqueued on `stream` (a cudaStream_t passed as void*); nothing synchronises.
  *     Stateless and re-entrant; one process per GPU.
  *   - Return value: 0 on success, negative fb200_status on error; message via fb200_last_error()
@@ -43,16 +43,8 @@ typedef enum { FB200_ALGO_AUTO = 0, FB200_ALGO_SIMT = 1, FB200_ALGO_TCGEN05 = 2,
 
 const char* fb200_last_error(void);
 int fb200_version(void);
-/* 1 if the current device is sm_100 (tcgen05 path usable), 0 otherwise, <0 on error. */
+/* 1 if the current device is sm_90 (the wgmma tensor-core path, FB200_ALGO_TCGEN05*, is usable), 0 otherwise, <0 on error. */
 int fb200_device_supports_tcgen05(void);
-/* Process-wide tuning options (host-only, no CUDA call).  Returns the previous value, FB200_ERR_INVALID for an unknown option.
- *   FB200_OPT_CONV_CTA_PAIR: 0 = tcgen05 convs never use CTA pairs, 1 (default) = `tcgen05.mma.cta_group::2` on 256-pixel x BLOCK_N tiles of two SMs
- *   whenever a layer has enough tiles to fill the chip, 2 = whenever the shape allows it (tests: small shapes, odd tile counts). */
-typedef enum { FB200_OPT_CONV_CTA_PAIR = 0 } fb200_option;
-int fb200_set_option(int option, int value);
-/* Debug timeline of the tcgen05 conv kernel (tools/conv_trace.py): while `device_buf` is not NULL every conv_tc launch writes 128 x uint64 clock64
- * stamps per CTA (grid x 128 x 8 bytes, at most 296 CTAs) - tile boundaries as seen by the MMA issuer, the producer and the epilogue.  NULL switches it off. */
-int fb200_set_conv_trace(void* device_buf);
 
 /* ---- a2: ResNet-vd stem, first conv fused with the input normalisation ------------------------
  * Replaces `(images - pixel_mean) / pixel_std` (models/fai_detr/modelling.py:1349) followed by
@@ -78,13 +70,13 @@ int fb200_stem_conv3x3s2_u8(const uint8_t* img_nhwc, int B, int H, int W, const 
  * (pitch res_pitch).  out dtype may differ from x dtype (fp32 heads on fp16 features).
  * out_batch_stride: elements between consecutive images of `out` (0 = dense Ho*Wo*out_pitch); lets a level's
  * projection be written straight into its rows of the concatenated [B, sum(HW), C] memory (modelling.py:1165).
- * algo: FB200_ALGO_AUTO picks tcgen05 when dtype==F16 and the shape qualifies. */
+ * algo: FB200_ALGO_AUTO picks the tensor-core kernel when dtype==F16 and the shape qualifies. */
 int fb200_conv2d(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int KH, int KW,
                  int stride, int pad, const float* scale, const float* bias, const void* residual, int res_pitch,
                  int act, void* out, int out_dtype, int out_pitch, int64_t out_batch_stride, int Cout, int algo, void* stream);
 
 /* fp32-accurate conv on pair-format activations (precision "fp32_tc"): x is the HI plane of a [hi | lo] pair tensor with C logical channels, its lo plane
- * `x_lo_off` elements further (pitch x_pitch covers both); w3 = [Cout][KH][KW][W_hi | W_lo | W_hi] (3C); three fp16 tcgen05 products per chunk, fp32 accumulation.
+ * `x_lo_off` elements further (pitch x_pitch covers both); w3 = [Cout][KH][KW][W_hi | W_lo | W_hi] (3C); three fp16 tensor-core products per chunk, fp32 accumulation.
  * out_dtype FB200_F32: fp32 output / residual as in fb200_conv2d.  out_dtype FB200_F16PAIR: the epilogue writes the result AS a pair (hi plane at `out`, lo plane
  * `out_lo_off` elements further, pitch out_pitch) and reads the residual as a pair (`res_lo_off`), so consecutive convs exchange activations without a split pass
  * (replaces the fb200_split_f32_pair launch in front of every conv: nn/layers/conv.py:78-98 chains such as resnet.py:106-121). */
@@ -338,8 +330,8 @@ int64_t fb200_conv_wgrad_workspace_bytes(int B, int Ho, int Wo, int Cin, int Cou
 int fb200_conv_wgrad(const float* x, int B, int H, int W, int Cin, int x_pitch, const float* dy, int Ho, int Wo, int Cout, int dy_pitch, int KH,
                      int KW, int stride, int pad, float* dw, int accumulate, void* workspace, void* stream);
 /* Same weight gradient on the tensor cores (k=1/3 stride-1 convs and linears, 3x3 stride-2 convs through TMA element strides; fb200_conv_wgrad_tc_supported says when): x_pair / dy_pair are
- * the dense [hi|lo] fp16 pairs (fb200_split_f32_pair) of x [B,H,W,Cin] and dy [B,H,W,Cout]; three tcgen05 products per 64-pixel chunk
- * (hi*hi + hi*lo + lo*hi, fp32 accumulation in TMEM) reproduce the fp32 result to ~2^-21. */
+ * the dense [hi|lo] fp16 pairs (fb200_split_f32_pair) of x [B,H,W,Cin] and dy [B,H,W,Cout]; three wgmma products per 64-pixel chunk
+ * (hi*hi + hi*lo + lo*hi, fp32 accumulation in registers) reproduce the fp32 result to ~2^-21. */
 int fb200_conv_wgrad_tc_supported(int B, int H, int W, int Cin, int Ho, int Wo, int Cout, int KH, int KW, int stride, int pad);
 int64_t fb200_conv_wgrad_tc_workspace_bytes(int B, int Ho, int Wo, int Cin, int Cout, int KH, int KW);
 int fb200_conv_wgrad_tc(const void* x_pair, int B, int H, int W, int Cin, const void* dy_pair, int Cout, int KH, int KW, int stride, int pad, float* dw,

@@ -10,6 +10,18 @@ import torch
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
+def update_report(name: str, entries: dict):
+    """merge `entries` into the JSON parity report `name` under $FB200_REPORT_DIR (default: a directory in the system temp dir), outside the source tree"""
+    import tempfile
+    d = os.environ.get("FB200_REPORT_DIR") or os.path.join(tempfile.gettempdir(), "focoos_b200_reports")
+    os.makedirs(d, exist_ok=True)
+    path = os.path.join(d, name)
+    rep = json.load(open(path)) if os.path.exists(path) else {}
+    rep.update(entries)
+    with open(path, "w") as f:
+        json.dump(rep, f, indent=1)
+
+
 def load_golden(tag: str):
     return np.load(os.path.join(GOLDEN, tag + ".npz"))
 

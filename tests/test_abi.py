@@ -1,4 +1,4 @@
-"""The C-ABI boundary without a GPU: the library builds for sm_100a, loads, and exports exactly the symbols include/focoos_b200.h declares;
+"""The C-ABI boundary without a GPU: the library builds for sm_90a, loads, and exports exactly the symbols include/focoos_b200.h declares;
 the Python marshalling layer binds all of them; host-only entry points work; compute entry points refuse CPU tensors (no fallback)."""
 import ctypes
 import os

@@ -199,7 +199,7 @@ def test_msda_grads():
 @pytest.mark.parametrize("B,H,W,Cin,Cout,k", [(2, 40, 40, 256, 256, 3), (2, 20, 20, 512, 128, 1), (1, 1, 600, 256, 1024, 1), (2, 16, 24, 64, 64, 3),
                                                (2, 20, 20, 96, 200, 3), (2, 23, 37, 128, 64, 3), (1, 1, 2400, 256, 80, 1), (4, 80, 80, 64, 256, 1)])
 def test_weight_gradient_on_tensor_cores(B, H, W, Cin, Cout, k):
-    """tcgen05 MN-major split-precision weight gradient vs torch's conv2d_weight in fp64 (and it must actually take the tensor-core path)."""
+    """wgmma MN-major split-precision weight gradient vs torch's conv2d_weight in fp64 (and it must actually take the tensor-core path)."""
     x, dy = rnd((B, H, W, Cin), 1), rnd((B, H, W, Cout), 2)
     pad = (k - 1) // 2
     ref = torch.nn.grad.conv2d_weight(nchw(x).double().contiguous(), (Cout, Cin, k, k), nchw(dy).double().contiguous(), stride=1, padding=pad).permute(0, 2, 3, 1)

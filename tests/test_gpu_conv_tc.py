@@ -1,4 +1,4 @@
-"""-m gpu: the tcgen05 implicit-GEMM conv/linear kernel against the CPU reference (fp32 accumulation of the same
+"""-m gpu: the wgmma implicit-GEMM conv/linear kernel against the CPU reference (fp32 accumulation of the same
 fp16 operands).  Kept in its own file: a descriptor bug would hang or trap, and must not take the SIMT tests down."""
 import math
 
@@ -34,7 +34,7 @@ def run_case(B, H, W, Cin, Cout, k, stride, act=0, use_res=False, use_scale=True
     a, b = out.float().cpu(), ref.float()
     err = float((a - b).abs().max())
     scale = max(1.0, float(b.abs().max()))
-    assert err <= tolerance * scale, f"tcgen05 conv B{B} {H}x{W} {Cin}->{Cout} k{k} s{stride}: max|d|={err:.3e} (scale {scale:.2e}); frac bad={(float(((a-b).abs()>tolerance*scale).float().mean())):.4f}"
+    assert err <= tolerance * scale, f"tensor-core conv B{B} {H}x{W} {Cin}->{Cout} k{k} s{stride}: max|d|={err:.3e} (scale {scale:.2e}); frac bad={(float(((a-b).abs()>tolerance*scale).float().mean())):.4f}"
 
 
 def test_tc_supported_flag():
@@ -97,7 +97,7 @@ def test_conv_cin32_swizzle64(H, W, Cin, Cout, k):
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout,k,stride,res", [(2, 20, 20, 256, 256, 3, 1, False), (1, 1, 1000, 256, 512, 1, 1, True), (2, 40, 40, 128, 128, 3, 2, False),
                                                           (2, 32, 32, 32, 64, 3, 1, False), (1, 1, 300, 1024, 256, 1, 1, True),
-                                                          (2, 40, 200, 32, 64, 3, 1, False), (1, 33, 130, 32, 32, 3, 1, False),   # halo strips (hi + lo), resident W_hi / W_lo
+                                                          (2, 40, 200, 32, 64, 3, 1, False), (1, 33, 130, 32, 32, 3, 1, False),   # fused split on 32-channel chunks
                                                           (2, 24, 40, 256, 64, 1, 1, False), (2, 40, 40, 64, 64, 3, 1, False),     # fused split, N = 64
                                                           (3, 20, 20, 512, 2048, 1, 1, True), (2, 80, 80, 256, 256, 3, 2, False)])  # pair + residual (2-stage ring), stride-2 pair
 def test_split_precision_conv_matches_fp32(B, H, W, Cin, Cout, k, stride, res):
@@ -125,7 +125,7 @@ def test_split_precision_conv_matches_fp32(B, H, W, Cin, Cout, k, stride, res):
 @pytest.mark.parametrize("dtype", [torch.float16, torch.float32])
 @pytest.mark.parametrize("B,H,W,C,Q", [(3, 40, 52, 256, 100), (2, 64, 128, 128, 100), (5, 8, 8, 64, 7)])
 def test_per_image_weights_product(B, H, W, C, Q, dtype):
-    """einsum('bqc,bchw->bqhw') as ONE launch with a per-image weight set (3-D weight tensor map on the tcgen05 path)."""
+    """einsum('bqc,bchw->bqhw') as ONE launch with a per-image weight set (3-D weight tensor map on the tensor-core path)."""
     x = rnd((B, H, W, C), dtype, 1)
     w = rnd((B, Q, 1, 1, C), dtype, 2, 1.0 / math.sqrt(C))
     ref = torch.einsum("bhwc,bqc->bhwq", x.float(), w.float().reshape(B, Q, C))
@@ -142,7 +142,7 @@ def test_per_image_weights_product(B, H, W, C, Q, dtype):
 @pytest.mark.parametrize("dtype", [torch.float16])
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 40, 40, 256, 512), (3, 16, 24, 512, 1024), (1, 80, 80, 64, 128)])
 def test_avgpool_folded_into_2x2_stride2_conv(B, H, W, Cin, Cout, dtype):
-    """AvgPool2d(2,2) + 1x1 conv == 2x2 stride-2 conv with W/4 on every tap (the vd shortcut, resnet.py:91-102) on the tcgen05 stride-2 view."""
+    """AvgPool2d(2,2) + 1x1 conv == 2x2 stride-2 conv with W/4 on every tap (the vd shortcut, resnet.py:91-102) on the tensor-core stride-2 view."""
     x = rnd((B, H, W, Cin), dtype, 1)
     w1 = rnd((Cout, 1, 1, Cin), dtype, 2, 1.0 / math.sqrt(Cin))
     sc, bi = torch.rand(Cout) + 0.5, rnd((Cout,), torch.float32, 3, 0.2)
@@ -157,7 +157,7 @@ def test_avgpool_folded_into_2x2_stride2_conv(B, H, W, Cin, Cout, dtype):
 
 @pytest.mark.parametrize("M,K,N", [(2 * 8400, 256, 365), (4800, 256, 80), (300, 512, 1000), (129, 64, 7)])
 def test_linear_rowmax_without_materialising_the_product(M, K, N):
-    """enc_outputs_class.max(-1): row maximum of x @ w.T + b computed in the tcgen05 epilogue (atomic max across column groups / N tiles)."""
+    """enc_outputs_class.max(-1): row maximum of x @ w.T + b computed in the tensor-core epilogue (atomic max across N tiles)."""
     x = rnd((M, K), torch.float16, 1)
     w = rnd((N, K), torch.float16, 2, 1.0 / math.sqrt(K))
     b = rnd((N,), torch.float32, 3, 2.0) - 3.0  # mostly negative rows: exercises the signed atomic max
@@ -168,7 +168,7 @@ def test_linear_rowmax_without_materialising_the_product(M, K, N):
 
 @pytest.mark.parametrize("B,H,W,Cout", [(2, 40, 200, 32), (1, 33, 320, 64), (2, 16, 64, 64), (3, 9, 131, 32)])
 def test_stem_halo_mode(B, H, W, Cout):
-    """32-channel 3x3 stride-1 convs (ResNet-vd conv1_2 / conv1_3): one (128+2)-pixel strip per filter row, the three kw taps as row-shifted UMMA descriptors."""
+    """32-channel 3x3 stride-1 convs (ResNet-vd conv1_2 / conv1_3): 32-channel chunks with 64-byte swizzled rows, ragged rows and images."""
     x = rnd((B, H, W, 32), torch.float16, 1)
     w = rnd((Cout, 3, 3, 32), torch.float16, 2, 1.0 / math.sqrt(288))
     sc, bi = torch.rand(Cout) + 0.5, rnd((Cout,), torch.float32, 3, 0.2)
@@ -177,50 +177,6 @@ def test_stem_halo_mode(B, H, W, Cout):
     out = ops.conv2d(x.to(DEV), w.to(DEV), sc.to(DEV), bi.to(DEV), stride=1, pad=1, act=1, algo=ops.ALGO_TCGEN05)
     err = float((out.float().cpu() - ref).abs().max())
     assert err <= 3e-3 * max(1.0, float(ref.abs().max())), err
-
-
-# ---- CTA pairs (tcgen05.mma.cta_group::2): every shape class again with the pair mode forced, plus bit-identity against the single-CTA kernel on
-# full-size layers (same operand order inside each MMA chain -> identical fp32 accumulators)
-@pytest.fixture()
-def force_pairs():
-    old = ops.set_option(ops.OPT_CONV_CTA_PAIR, 2)
-    yield
-    ops.set_option(ops.OPT_CONV_CTA_PAIR, old)
-
-
-def test_pair_mode_small_shapes(force_pairs):
-    run_case(1, 1, 1000, 256, 256, 1, 1, seed=1)                                   # 8 M tiles, ragged last tile
-    run_case(1, 1, 777, 1024, 256, 1, 1, seed=2)                                   # 7 M tiles: odd -> phantom tile in the last pair
-    run_case(1, 1, 128, 256, 512, 1, 1, seed=3)                                    # ONE M tile: the peer CTA only has a phantom
-    run_case(1, 1, 9600, 256, 1536, 1, 1, seed=4)                                  # 6 N tiles
-    run_case(2, 20, 20, 256, 256, 3, 1, act=1, seed=5)
-    run_case(2, 40, 40, 256, 256, 3, 1, act=2, seed=6)
-    run_case(3, 24, 40, 64, 128, 3, 1, act=1, seed=7)                              # BLOCK_N = 128 pairs, 3 images x odd tiles
-    run_case(2, 80, 80, 256, 256, 3, 2, act=1, seed=8)                             # stride-2 parity view
-    run_case(2, 20, 20, 256, 1024, 1, 1, act=1, use_res=True, seed=9)              # residual through TMA
-    run_case(2, 20, 20, 256, 256, 3, 1, act=2 | 16, use_res=True, use_scale=False, seed=10)
-    run_case(1, 1, 500, 256, 368, 1, 1, out_dtype=torch.float32, use_scale=False, tolerance=2e-3)  # Cout tail inside the second half of the N tile
-
-
-@pytest.mark.parametrize("B,H,W,Cin,Cout,k,stride,res", [(32, 80, 80, 256, 256, 3, 1, False), (32, 40, 40, 1024, 256, 1, 1, False), (32, 40, 40, 256, 1024, 1, 1, True),
-                                                          (32, 80, 80, 128, 128, 3, 1, False), (5, 40, 40, 512, 512, 3, 2, False), (1, 1, 268800, 256, 1536, 1, 1, False)])
-def test_pair_mode_bit_identical_to_single_cta(B, H, W, Cin, Cout, k, stride, res):
-    x = rnd((B, H, W, Cin), torch.float16, 1).to(DEV)
-    w = rnd((Cout, k, k, Cin), torch.float16, 2, 1.0 / math.sqrt(k * k * Cin)).to(DEV)
-    bi = rnd((Cout,), torch.float32, 3, 0.2).to(DEV)
-    pad = (k - 1) // 2
-    Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
-    r = rnd((B, Ho, Wo, Cout), torch.float16, 4).to(DEV) if res else None
-    outs = []
-    for mode in (0, 2):
-        old = ops.set_option(ops.OPT_CONV_CTA_PAIR, mode)
-        try:
-            outs.append(ops.conv2d(x, w, None, bi, stride=stride, pad=pad, act=1, residual=r, algo=ops.ALGO_TCGEN05))
-            torch.cuda.synchronize()
-        finally:
-            ops.set_option(ops.OPT_CONV_CTA_PAIR, old)
-    assert torch.equal(outs[0], outs[1])
-    assert float(outs[0].float().abs().max()) > 0
 
 
 # ---- pair-format activations: the conv epilogue writes [hi | lo] fp16 planes, reads pair residuals; pools / resize on pairs -------------------------

@@ -1,4 +1,4 @@
-"""-m gpu: one full fine-tune iteration of FAIDetr on the B200 (training-mode forward, criterion, backward through the hand-written
+"""-m gpu: one full fine-tune iteration of FAIDetr on the GPU (training-mode forward, criterion, backward through the hand-written
 kernels, clipping, AdamW) against the golden of the unmodified reference's training step (oracle/gen_golden_train.py)."""
 import numpy as np
 import pytest

@@ -1,5 +1,5 @@
 """Pins the CPU oracle (oracle/detr_oracle.py) to the committed golden fixtures produced by the
-UNMODIFIED reference (oracle/gen_golden.py), and — where /root/reference exists — to the reference itself."""
+UNMODIFIED reference (oracle/gen_golden.py, oracle/gen_golden_live_reference.py)."""
 import numpy as np
 import pytest
 import torch
@@ -69,19 +69,21 @@ def test_oracle_vs_golden_ragged(sd):
         assert np.abs(gb - ob).max() <= 1  # round() of a coordinate that sits within 1e-4 px of .5
 
 
-@pytest.mark.reference
 def test_oracle_vs_live_reference(sd):
-    from oracle import ref_import
+    """against the reference's own processor + model on a 480x640 image, stored by oracle/gen_golden_live_reference.py"""
+    import hashlib
+    import os
 
-    fm = ref_import.get_reference_model("fai-detr-l-obj365")
-    fm.model.load_state_dict(sd, strict=True)
+    from oracle.gen_golden_live_reference import x_sample_index
+
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live_reference.npz"))
     imgs = synth_images(7, [(480, 640)])
     with torch.no_grad():
-        x, _ = fm.processor.preprocess(imgs, device=torch.device("cpu"), dtype=torch.float32)
-        out = fm.model(x)
         xo = O.detr_preprocess(imgs, (640, 640))
         taps = {}
         s, b = O.detr_forward(sd, xo, O.DetrOracleConfig(), taps)
-    assert torch.equal(x, xo)
+    xf = xo.contiguous().numpy()
+    assert tuple(xo.shape) == tuple(g["x_shape"]) and np.array_equal(xf.ravel()[x_sample_index(xf.size)], g["x_sample"])
+    assert hashlib.sha256(xf.tobytes()).hexdigest() == str(g["x_sha256"]), "the pre-processed input differs from the reference's"
     # same SET of queries, per-query values equal up to fp32 reassociation
-    assert np.abs(np.sort(out.logits.numpy().max(-1), axis=1) - np.sort(s.numpy().max(-1), axis=1)).max() < 1e-4
+    assert np.abs(g["sorted_max_logit"] - np.sort(s.numpy().max(-1), axis=1)).max() < 1e-4

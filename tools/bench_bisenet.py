@@ -1,4 +1,4 @@
-"""Config 4 of BASELINE.json: bisenetformer-l-ade, bs=64, 1024x512 on one B200 (forward + GPU part of the semantic post-process).
+"""Config 4 of BASELINE.json: bisenetformer-l-ade, bs=64, 1024x512 on one GPU (forward + GPU part of the semantic post-process).
     python tools/bench_bisenet.py [batch] [H] [W]"""
 import json, os, sys, collections
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -39,7 +39,7 @@ agg = collections.defaultdict(lambda: [0, 0.0])
 for name, note, a, b in tr:
     agg[name][0] += 1; agg[name][1] += a.elapsed_time(b)
 tot = sum(v[1] for v in agg.values())
-print(json.dumps({"workload": f"bisenetformer-l-ade bs={B} {W}x{H} (BASELINE configs[3])", "images_per_s": B / ms * 1e3, "ms_per_step": ms, "unfused_images_per_s": B / ms_unfused * 1e3, "unfused_ms_per_step": ms_unfused, "dtype": {"fp16": "f16", "fp32_tc": "f32 (3x f16 tcgen05 products)", "fp32": "f32 SIMT"}[PREC], "precision": PREC, "launches": len(tr),
+print(json.dumps({"workload": f"bisenetformer-l-ade bs={B} {W}x{H} (BASELINE configs[3])", "images_per_s": B / ms * 1e3, "ms_per_step": ms, "unfused_images_per_s": B / ms_unfused * 1e3, "unfused_ms_per_step": ms_unfused, "dtype": {"fp16": "f16", "fp32_tc": "f32 (3x f16 wgmma products)", "fp32": "f32 SIMT"}[PREC], "precision": PREC, "launches": len(tr),
                   "peak_mem_gb": torch.cuda.max_memory_allocated() / 1e9}))
 for k, (c, t) in sorted(agg.items(), key=lambda kv: -kv[1][1]):
     print(f"{t:9.2f} ms {100*t/tot:5.1f}%  n={c:4d}  {k}")

@@ -1,4 +1,4 @@
-"""Config 3 of BASELINE.json: fai-mf-l-coco-ins, bs=16, 800x800 on one B200 — images/s of FAIMaskFormer.forward (+ GPU part of the
+"""Config 3 of BASELINE.json: fai-mf-l-coco-ins, bs=16, 800x800 on one GPU — images/s of FAIMaskFormer.forward (+ GPU part of the
 instance post-process), CUDA events, plus a per-kernel-symbol time breakdown of one eager forward.
     python tools/bench_mf.py [batch] [size]"""
 import json, os, sys, collections
@@ -39,7 +39,7 @@ agg = collections.defaultdict(lambda: [0, 0.0])
 for name, note, a, b in tr:
     agg[name][0] += 1; agg[name][1] += a.elapsed_time(b)
 tot = sum(v[1] for v in agg.values())
-print(json.dumps({"workload": f"fai-mf-l-coco-ins bs={B} {S}x{S} (BASELINE configs[2])", "images_per_s": B / ms * 1e3, "ms_per_step": ms, "unfused_images_per_s": B / ms_unfused * 1e3, "unfused_ms_per_step": ms_unfused, "dtype": {"fp16": "f16", "fp32_tc": "f32 (3x f16 tcgen05 products)", "fp32": "f32 SIMT"}[PREC], "precision": PREC, "launches": len(tr),
+print(json.dumps({"workload": f"fai-mf-l-coco-ins bs={B} {S}x{S} (BASELINE configs[2])", "images_per_s": B / ms * 1e3, "ms_per_step": ms, "unfused_images_per_s": B / ms_unfused * 1e3, "unfused_ms_per_step": ms_unfused, "dtype": {"fp16": "f16", "fp32_tc": "f32 (3x f16 wgmma products)", "fp32": "f32 SIMT"}[PREC], "precision": PREC, "launches": len(tr),
                   "peak_mem_gb": torch.cuda.max_memory_allocated() / 1e9}))
 for k, (c, t) in sorted(agg.items(), key=lambda kv: -kv[1][1]):
     print(f"{t:9.2f} ms {100*t/tot:5.1f}%  n={c:4d}  {k}")

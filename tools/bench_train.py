@@ -93,8 +93,8 @@ def run_leg(batch=16, size=640, steps=5, warmup=2, precision="fp32_tc", by_symbo
         by_sym["_kernels_ms"] = round(sum(v["ms"] for k, v in by_sym.items() if isinstance(v, dict)), 3)
     total = float(sum(v.detach() for v in losses.values()))
     res = {"metric": "images/sec fai-detr-l fine-tune step (fwd + criterion + bwd + all-reduce + AdamW)", "value": batch * world / (ms / 1e3), "unit": "images/s",
-           "n_gpus": world, "ms_per_step": ms, "steps": steps, "warmup": warmup, "scaling": "weak", "dtype": "f32 storage; " + {"fp32_tc": "3x f16 tcgen05 products for conv/linear forward, data and weight gradients", "fp32": "SIMT f32",
-                                                                      "amp": "ONE f16 tcgen05 product (fp16-rounded operands, f32 accumulation) for conv/linear forward, data and weight gradients - the reference's torch.autocast(fp16) + GradScaler arithmetic (trainer/trainer.py:735)"}[precision],
+           "n_gpus": world, "ms_per_step": ms, "steps": steps, "warmup": warmup, "scaling": "weak", "dtype": "f32 storage; " + {"fp32_tc": "3x f16 wgmma products for conv/linear forward, data and weight gradients", "fp32": "SIMT f32",
+                                                                      "amp": "ONE f16 wgmma product (fp16-rounded operands, f32 accumulation) for conv/linear forward, data and weight gradients - the reference's torch.autocast(fp16) + GradScaler arithmetic (trainer/trainer.py:735)"}[precision],
            "precision": precision,
            "config": {"workload": f"fai-detr-l (80 classes) bs={batch}/GPU {size}x{size} synthetic COCO-shape targets (BASELINE configs[4])", "global_batch": batch * world,
                       "sync_bn": bool(getattr(m, "sync_bn", False)) and world > 1},

@@ -1,4 +1,4 @@
-"""Times the tcgen05 weight-gradient kernel alone on the heaviest training shapes (run under ncu for the tensor-pipe evidence)."""
+"""Times the wgmma weight-gradient kernel alone on the heaviest training shapes."""
 import sys, os
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
