@@ -163,6 +163,33 @@ __device__ __forceinline__ float act_fwd(int act, float z) {
   return z;
 }
 
+// MODE 3 (single-pass mean / variance): each thread sums (x - q) and (x - q)^2 about its OWN first row q, so the squares never cancel against a
+// pivot far from the data; per thread that gives (n, mean, M2 = sum of squared deviations from the mean), which the block merges over its row
+// lanes with Chan's pairwise update.  The part written is p0 = sum (x - x[0,c]) (the mean relative to the global pivot row) and p1 = M2 about
+// the part's own mean; bn_stats_finalize_kernel adds the between-part term in double.  (One pivot for all rows, row 0, lost the variance to
+// fp32 cancellation when row 0 lay far from the mean: ~1e-5 relative at 40 sigma.)
+struct LaneRows {  // rows of the lane starting at row r0 < rstep (a grid-stride walk r0, r0 + rstep, ... < R): full or full + 1
+  float full;
+  int64_t rem;
+  __device__ __forceinline__ LaneRows(int64_t R, int64_t rstep) : full((float)(R / rstep)), rem(R % rstep) {}
+  __device__ __forceinline__ float operator()(int64_t r0) const { return full + (r0 < rem ? 1.f : 0.f); }
+};
+struct Moments {
+  float n, mean, m2;  // rows, mean relative to the global pivot, sum of squared deviations from `mean`
+  __device__ __forceinline__ void merge(float nb, float mb, float m2b) {
+    if (nb == 0.f) return;
+    const float nt = n + nb, d = mb - mean, w = nb * __frcp_rn(nt);
+    mean += d * w;
+    m2 += m2b + d * d * n * w;
+    n = nt;
+  }
+};
+__device__ __forceinline__ void lane_moments(float n, float q_rel, float s0, float s1, float& mean, float& m2) {  // (x - q) sums -> mean, M2
+  const float m = n > 0.f ? s0 * __frcp_rn(n) : 0.f;
+  mean = q_rel + m;
+  m2 = fmaxf(s1 - s0 * m, 0.f);
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(256) col_partial_kernel(const float* __restrict__ x, int x_pitch, int64_t R, int C, const float* __restrict__ mean,
                                                           const float* __restrict__ rstd, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -170,14 +197,15 @@ __global__ void __launch_bounds__(256) col_partial_kernel(const float* __restric
                                                           float* __restrict__ p0, float* __restrict__ p1) {
   const int c = blockIdx.x * 32 + (threadIdx.x & 31);
   const int lane_r = threadIdx.x >> 5;  // 0..7
-  float s0 = 0.f, s1 = 0.f;
+  const int64_t rstep = (int64_t)gridDim.y * 8;
+  float s0 = 0.f, s1 = 0.f, q_rel = 0.f;
   if (c < C) {
     const float mu = (MODE >= 1) ? mean[c] : 0.f;
     const float rs = (MODE == 2) ? rstd[c] : 0.f;
     const float ga = (MODE == 2) ? gamma[c] : 0.f, be = (MODE == 2) ? beta[c] : 0.f;
-    const float pivot = (MODE == 3) ? x[c] : 0.f;  // single-pass mean/variance: sums of (x - x[0,c]) and its square (shift kills the cancellation)
-    const int64_t rstep = (int64_t)gridDim.y * 8;
     int64_t r = (int64_t)blockIdx.y * 8 + lane_r;
+    const float pivot = (MODE == 3 && r < R) ? x[r * x_pitch + c] : 0.f;  // this thread's first row
+    if (MODE == 3) q_rel = pivot - x[c];
     if (MODE == 2) {  // four independent rows per iteration: 8-12 loads in flight per thread instead of 2-3 (the kernel is latency-, not bandwidth-bound otherwise)
       for (; r + 3 * rstep < R; r += 4 * rstep) {
         float xv[4], gv[4], yv[4];
@@ -225,14 +253,23 @@ __global__ void __launch_bounds__(256) col_partial_kernel(const float* __restric
       }
     }
   }
+  const LaneRows rows(R, rstep);
+  if (MODE == 3) lane_moments(rows((int64_t)blockIdx.y * 8 + lane_r), q_rel, s0, s1, s0, s1);
   __shared__ float r0[8][33], r1[8][33];
   r0[lane_r][threadIdx.x & 31] = s0;
   r1[lane_r][threadIdx.x & 31] = s1;
   __syncthreads();
   if (lane_r == 0 && c < C) {
     float a = 0.f, b = 0.f;
+    if (MODE == 3) {
+      Moments m{0.f, 0.f, 0.f};
+      for (int k = 0; k < 8; ++k) m.merge(rows((int64_t)blockIdx.y * 8 + k), r0[k][threadIdx.x], r1[k][threadIdx.x]);
+      a = m.n * m.mean;
+      b = m.m2;
+    } else {
 #pragma unroll
-    for (int k = 0; k < 8; ++k) { a += r0[k][threadIdx.x]; b += r1[k][threadIdx.x]; }
+      for (int k = 0; k < 8; ++k) { a += r0[k][threadIdx.x]; b += r1[k][threadIdx.x]; }
+    }
     p0[(int64_t)blockIdx.y * C + c] = a;
     if (MODE >= 2) p1[(int64_t)blockIdx.y * C + c] = b;
   }
@@ -255,10 +292,17 @@ __global__ void __launch_bounds__(256) col_partial4_kernel(const float* __restri
   float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
   float mu[4] = {0.f, 0.f, 0.f, 0.f}, rs[4] = {0.f, 0.f, 0.f, 0.f}, ga[4] = {0.f, 0.f, 0.f, 0.f}, be[4] = {0.f, 0.f, 0.f, 0.f}, pv[4] = {0.f, 0.f, 0.f, 0.f};
   if (MODE == 2) { load4(mean + c, mu); load4(rstd + c, rs); load4(gamma + c, ga); load4(beta + c, be); }
-  if (MODE == 3) load4(x + c, pv);  // pivot row (see col_partial_kernel)
   const bool has_y = (MODE == 2) && act != FB200_ACT_NONE && y != nullptr;
   const int64_t rstep = (int64_t)gridDim.y * RPB;
   int64_t r = (int64_t)blockIdx.y * RPB + tr;
+  float q_rel[4] = {0.f, 0.f, 0.f, 0.f};
+  if (MODE == 3) {  // pivot: this thread's first row (see col_partial_kernel)
+    float p_row0[4];
+    load4(x + c, p_row0);
+    if (r < R) load4(x + r * x_pitch + c, pv);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) q_rel[j] = pv[j] - p_row0[j];
+  }
   auto accum = [&](const float (&xv)[4], const float (&gv)[4], const float (&yv)[4]) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -294,13 +338,26 @@ __global__ void __launch_bounds__(256) col_partial4_kernel(const float* __restri
     if (MODE == 2 && has_y) load4(y + r * y_pitch + c, yv);
     accum(xv, gv, yv);
   }
+  const LaneRows rows(R, rstep);
+  if (MODE == 3) {
+    const float n = rows((int64_t)blockIdx.y * RPB + tr);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) lane_moments(n, q_rel[j], s0[j], s1[j], s0[j], s1[j]);
+  }
   __shared__ float red0[32][129], red1[32][129];   // [row lane][channel of the chunk]
 #pragma unroll
   for (int j = 0; j < 4; ++j) { red0[tr][tc * 4 + j] = s0[j]; if (MODE >= 2) red1[tr][tc * 4 + j] = s1[j]; }
   __syncthreads();
   if ((int)threadIdx.x < CW) {
     float a = 0.f, b = 0.f;
-    for (int k = 0; k < RPB; ++k) { a += red0[k][threadIdx.x]; if (MODE >= 2) b += red1[k][threadIdx.x]; }
+    if (MODE == 3) {
+      Moments m{0.f, 0.f, 0.f};
+      for (int k = 0; k < RPB; ++k) m.merge(rows((int64_t)blockIdx.y * RPB + k), red0[k][threadIdx.x], red1[k][threadIdx.x]);
+      a = m.n * m.mean;
+      b = m.m2;
+    } else {
+      for (int k = 0; k < RPB; ++k) { a += red0[k][threadIdx.x]; if (MODE >= 2) b += red1[k][threadIdx.x]; }
+    }
     const int co = blockIdx.x * CW + threadIdx.x;
     p0[(int64_t)blockIdx.y * C + co] = a;
     if (MODE >= 2) p1[(int64_t)blockIdx.y * C + co] = b;
@@ -336,24 +393,53 @@ __global__ void col_finalize_kernel(const float* __restrict__ p0, const float* _
     out0[c] = accumulate ? out0[c] + (float)a : (float)a;
     out1[c] = accumulate ? out1[c] + (float)b : (float)b;
   }
-  if (FIN == 4) {  // single-pass BN statistics from shifted sums: a = sum(x - pivot), b = sum((x - pivot)^2); `mean` carries the pivot row
-    const double m1 = a / R;
-    double var = b / R - m1 * m1;
-    if (var < 0.0) var = 0.0;
-    const float mu = (float)((double)mean[c] + m1);
-    out0[c] = mu;
-    out1[c] = (float)(1.0 / sqrt(var + (double)eps));
-    if (run_mean) {
-      run_mean[c] = (1.f - momentum) * run_mean[c] + momentum * mu;
-      run_var[c] = (1.f - momentum) * run_var[c] + momentum * (float)(R > 1.0 ? var * R / (R - 1.0) : var);
-    }
+}
+
+__device__ __forceinline__ double warp_sum_f64(double v) {  // butterfly: the same fixed order on every lane
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// BN statistics from col_partial<3>'s parts: p0 = sum (x - pivot row), p1 = squared deviations about the part's own mean, in part k the rows whose
+// (r mod nparts * rpb) lies in [k * rpb, (k + 1) * rpb).  Total squared deviations = sum p1_k + sum n_k (mean_k - mean)^2, the latter as
+// sum p0_k^2 / n_k - (sum p0_k)^2 / R in double.  One warp per channel (lanes take every 32nd part, then a butterfly sum), so the walk over the
+// parts is not one long chain of dependent loads.
+// FIN 4: out0 = mean, out1 = rstd, running statistics updated (bn_train_fwd); `mean` carries the pivot row
+// FIN 5: out0 = mean, out1 = BIASED variance: the raw local moments SyncBatchNorm exchanges (fb200_bn_stats)
+template <int FIN>
+__global__ void __launch_bounds__(256) bn_stats_finalize_kernel(const float* __restrict__ p0, const float* __restrict__ p1, int nparts, int rpb, int C, int64_t R,
+                                                                float eps, float momentum, const float* __restrict__ pivot, float* __restrict__ run_mean,
+                                                                float* __restrict__ run_var, float* __restrict__ out0, float* __restrict__ out1) {
+  const int c = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (c >= C) return;
+  // with rem = R mod (nparts * rpb), part k holds nfull rows, plus rpb for k < kpart and rem mod rpb for k == kpart
+  const int64_t rstep = (int64_t)nparts * rpb, rem = R % rstep, nfull = (R / rstep) * rpb, npart = nfull + rem % rpb;
+  const int kpart = (int)(rem / rpb);
+  const double inv_more = 1.0 / (double)(nfull + rpb), inv_part = npart > 0 ? 1.0 / (double)npart : 0.0, inv_full = nfull > 0 ? 1.0 / (double)nfull : 0.0;
+  double a = 0.0, b = 0.0, e = 0.0;
+  for (int k = lane; k < nparts; k += 32) {
+    const double p = (double)p0[(int64_t)k * C + c];
+    a += p;
+    b += (double)p1[(int64_t)k * C + c];
+    e += p * p * (k < kpart ? inv_more : k == kpart ? inv_part : inv_full);
   }
-  if (FIN == 5) {  // like 4, but the raw local moments: out0 = mean, out1 = BIASED variance (SyncBatchNorm exchanges these, fb200_bn_stats)
-    const double m1 = a / R;
-    double var = b / R - m1 * m1;
-    if (var < 0.0) var = 0.0;
-    out0[c] = (float)((double)mean[c] + m1);
+  a = warp_sum_f64(a);
+  b = warp_sum_f64(b);
+  e = warp_sum_f64(e);
+  if (lane != 0) return;
+  const double Rd = (double)R, m1 = a / Rd;
+  const double var = (b + fmax(e - a * m1, 0.0)) / Rd;
+  const float mu = (float)((double)pivot[c] + m1);
+  out0[c] = mu;
+  if (FIN == 5) {
     out1[c] = (float)var;
+    return;
+  }
+  out1[c] = (float)(1.0 / sqrt(var + (double)eps));
+  if (run_mean) {
+    run_mean[c] = (1.f - momentum) * run_mean[c] + momentum * mu;
+    run_var[c] = (1.f - momentum) * run_var[c] + momentum * (float)(R > 1 ? var * Rd / (Rd - 1.0) : var);
   }
 }
 
@@ -800,18 +886,21 @@ static void bn_apply_launch(const float* x, int x_pitch, const float* res, int r
   else bn_apply_kernel<<<grid_for(R * (C / 4)), 256, 0, st>>>(x, x_pitch, res, res_pitch, R, C, mean, rstd, gamma, beta, act, y, y_pitch);
 }
 
-// one column pass (MODE 0 colsum / 2 BN backward sums / 3 shifted moments) -> partials p0 / p1 [parts][C]; returns the number of parts
+// one column pass (MODE 0 colsum / 2 BN backward sums / 3 moments) -> partials p0 / p1 [parts][C]; returns the number of parts (and in *rpb the rows
+// each part takes per row step)
 template <int MODE>
 static int col_partial_launch(const float* x, int x_pitch, int64_t R, int C, const float* mean, const float* rstd, const float* gamma, const float* beta, const float* dy,
-                              int dy_pitch, const float* y, int y_pitch, int act, float* p0, float* p1, cudaStream_t st) {
+                              int dy_pitch, const float* y, int y_pitch, int act, float* p0, float* p1, cudaStream_t st, int* rpb = nullptr) {
   if (col_vec_ok(C, x, x_pitch, dy, dy_pitch, y, y_pitch)) {
     const int CW = C < 128 ? C : 128, RPB = 256 / (CW / 4);
     const dim3 g((unsigned)(C / CW), (unsigned)std::min<int64_t>(CR_ROWS, cdiv(R, (int64_t)RPB)));
     col_partial4_kernel<MODE><<<g, 256, 0, st>>>(x, x_pitch, R, C, mean, rstd, gamma, beta, dy, dy_pitch, y, y_pitch, act, p0, p1);
+    if (rpb) *rpb = RPB;
     return (int)g.y;
   }
   const dim3 g = col_grid(C, R);
   col_partial_kernel<MODE><<<g, 256, 0, st>>>(x, x_pitch, R, C, mean, rstd, gamma, beta, dy, dy_pitch, y, y_pitch, act, p0, p1);
+  if (rpb) *rpb = 8;
   return (int)g.y;
 }
 
@@ -834,9 +923,10 @@ extern "C" int fb200_bn_train_fwd(const float* x, int x_pitch, int64_t R, int C,
   cudaStream_t st = (cudaStream_t)stream;
   float* p0 = reinterpret_cast<float*>(workspace);
   float* p1 = p0 + (int64_t)CR_ROWS * C;
-  // ONE pass over x for both moments (sums shifted by the first row, finalised in double); `x` itself serves as the pivot row for the finaliser
-  const int parts = col_partial_launch<3>(x, x_pitch, R, C, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, 0, 0, p0, p1, st);
-  col_finalize_kernel<4><<<cdiv(C, 128), 128, 0, st>>>(p0, p1, parts, C, (double)R, eps, momentum, x, running_mean, running_var, save_mean, save_rstd, 0);
+  // ONE pass over x for both moments (per-part mean and squared deviations, combined in double); `x` itself serves as the pivot row for the finaliser
+  int rpb = 0;
+  const int parts = col_partial_launch<3>(x, x_pitch, R, C, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, 0, 0, p0, p1, st, &rpb);
+  bn_stats_finalize_kernel<4><<<cdiv(C, 8), 256, 0, st>>>(p0, p1, parts, rpb, C, R, eps, momentum, x, running_mean, running_var, save_mean, save_rstd);
   bn_apply_launch(x, x_pitch, res, res_pitch, R, C, save_mean, save_rstd, gamma, beta, act, y, y_pitch, st);
   FB_CHECK_LAUNCH("bn_train_fwd");
   return FB200_OK;
@@ -877,8 +967,9 @@ extern "C" int fb200_bn_stats(const float* x, int x_pitch, int64_t R, int C, flo
   cudaStream_t st = (cudaStream_t)stream;
   float* p0 = reinterpret_cast<float*>(workspace);
   float* p1 = p0 + (int64_t)CR_ROWS * C;
-  const int parts = col_partial_launch<3>(x, x_pitch, R, C, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, 0, 0, p0, p1, st);
-  col_finalize_kernel<5><<<cdiv(C, 128), 128, 0, st>>>(p0, p1, parts, C, (double)R, 0.f, 0.f, x, nullptr, nullptr, mean, var_biased, 0);
+  int rpb = 0;
+  const int parts = col_partial_launch<3>(x, x_pitch, R, C, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, 0, 0, p0, p1, st, &rpb);
+  bn_stats_finalize_kernel<5><<<cdiv(C, 8), 256, 0, st>>>(p0, p1, parts, rpb, C, R, 0.f, 0.f, x, nullptr, nullptr, mean, var_biased);
   FB_CHECK_LAUNCH("bn_stats");
   return FB200_OK;
 }

@@ -87,6 +87,44 @@ def test_batchnorm_train_grads(act, res):
         close(rg.grad, rr.grad, "bn dres")
 
 
+@pytest.mark.parametrize("R,C", [(102400, 256), (4800, 365)])
+def test_colsum_at_fine_tune_rows(R, C):
+    """bias gradients of Conv2dFn / LinearFn at fine-tune row counts, against an fp64 column sum.  R = 102,400 at C = 256 runs col_partial4's
+    unrolled four-row loop (R > 3 * 264 * 8) and its tail; 365 (the class head) is not a width the vector kernel takes, so the scalar kernel runs.
+    Zero-mean data: a dropped or doubled row moves a column sum by O(1) against a scale of O(sqrt(R)), far above the bar."""
+    x = rnd((R, C), 1)
+    ref = x.double().sum(0)
+    xg = x.to(DEV)
+    out, again = torch.empty(C, device=DEV), torch.empty(C, device=DEV)
+    ops._be().colsum(xg, out)
+    ops._be().colsum(xg, again)
+    close(out, ref, "colsum", 2e-5)
+    assert torch.equal(out, again), "colsum is not bitwise reproducible"
+
+
+@pytest.mark.parametrize("res", [False, True])
+@pytest.mark.parametrize("M", [16 * 300, 16 * 400])
+def test_layernorm_grads_at_fine_tune_rows(M, res):
+    """LayerNormFn backward at the decoder (bs 16 x 300 queries) and AIFI (bs 16 x 20 x 20) row counts, against fp64 autograd: the grid is capped
+    at 264 blocks of 8 warps, so each warp walks several rows and the per-block parameter-gradient partials sum over them"""
+    C = 256
+    x, r = rnd((M, C), 1), rnd((M, C), 2)
+    g, b = rnd((C,), 3).abs() + 0.5, rnd((C,), 4)
+    xr, rr, gr, br = (t.double().requires_grad_(True) for t in (x, r, g, b))
+    yr = F.layer_norm(xr + rr if res else xr, (C,), gr, br, 1e-5)
+    dy = rnd((M, C), 5)
+    yr.backward(dy.double())
+    xg, rg, gg, bg = leaf(x, DEV), leaf(r, DEV), leaf(g, DEV), leaf(b, DEV)
+    yg = A.LayerNormFn.apply(xg, rg if res else None, gg, bg, 1e-5)
+    yg.backward(dy.to(DEV))
+    close(yg, yr, "ln fwd")
+    close(xg.grad, xr.grad, "ln dx")
+    if res:
+        close(rg.grad, rr.grad, "ln dres")
+    close(gg.grad, gr.grad, "ln dgamma")
+    close(bg.grad, br.grad, "ln dbeta")
+
+
 def test_layernorm_linear_addact_grads():
     M, C, N = 2 * 37, 256, 96
     x, r = rnd((2, 37, C), 1), rnd((2, 37, C), 2)
@@ -197,9 +235,11 @@ def test_msda_grads():
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout,k", [(2, 40, 40, 256, 256, 3), (2, 20, 20, 512, 128, 1), (1, 1, 600, 256, 1024, 1), (2, 16, 24, 64, 64, 3),
-                                               (2, 20, 20, 96, 200, 3), (2, 23, 37, 128, 64, 3), (1, 1, 2400, 256, 80, 1), (4, 80, 80, 64, 256, 1)])
+                                               (2, 20, 20, 96, 200, 3), (2, 23, 37, 128, 64, 3), (1, 1, 2400, 256, 80, 1), (4, 80, 80, 64, 256, 1),
+                                               (2, 96, 96, 32, 32, 3), (2, 96, 96, 32, 64, 3)])
 def test_weight_gradient_on_tensor_cores(B, H, W, Cin, Cout, k):
-    """wgmma MN-major split-precision weight gradient vs torch's conv2d_weight in fp64 (and it must actually take the tensor-core path)."""
+    """wgmma MN-major split-precision weight gradient vs torch's conv2d_weight in fp64 (and it must actually take the tensor-core path).
+    The 32-channel stem convs (conv1_2: 32 -> 32, conv1_3: 32 -> 64) fill only half of a 64-channel TMA box with the operand's hi (or lo) plane."""
     x, dy = rnd((B, H, W, Cin), 1), rnd((B, H, W, Cout), 2)
     pad = (k - 1) // 2
     ref = torch.nn.grad.conv2d_weight(nchw(x).double().contiguous(), (Cout, Cin, k, k), nchw(dy).double().contiguous(), stride=1, padding=pad).permute(0, 2, 3, 1)
@@ -223,7 +263,8 @@ def test_stride2_weight_gradient_on_tensor_cores(B, H, W, Cin, Cout):
     close(got, ref.float(), "wgrad tc stride 2", 2e-5)
 
 
-@pytest.mark.parametrize("B,H,W,Cin,Cout,k,stride", [(2, 40, 40, 256, 256, 3, 1), (1, 1, 600, 256, 1024, 1, 1), (2, 23, 37, 128, 64, 3, 1), (2, 31, 45, 64, 256, 3, 2)])
+@pytest.mark.parametrize("B,H,W,Cin,Cout,k,stride", [(2, 40, 40, 256, 256, 3, 1), (1, 1, 600, 256, 1024, 1, 1), (2, 23, 37, 128, 64, 3, 1), (2, 31, 45, 64, 256, 3, 2),
+                                                      (2, 96, 96, 32, 32, 3, 1), (2, 96, 96, 32, 64, 3, 1)])
 def test_weight_gradient_single_product(B, H, W, Cin, Cout, k, stride):
     """"amp" training precision: ONE tensor-core product on fp16-rounded operands (fb200_conv_wgrad_tc_f16), fp32 accumulation: exact (to fp32 summation order)
     for operands that ARE fp16 values, and within the fp16 operand rounding (2^-11 relative per element) of the fp32 gradient otherwise."""
