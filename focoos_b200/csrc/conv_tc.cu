@@ -11,7 +11,8 @@
 //                  padding, and ragged tile edges) are zero-filled by the TMA unit.  Stride-2 convs use a 5-D view
 //                  (c', w/2, h&1, h/2, b) of the same tensor so that every tap is again a dense box.  1x1 convs and linears are the
 //                  degenerate W = M, H = 1 case.  Smem tiles land in the canonical K-major SWIZZLE_128B (or _64B for 32-channel
-//                  chunks) layout wgmma reads through its shared-memory descriptors.
+//                  chunks) layout wgmma reads through its shared-memory descriptors.  After a tile's last k-block the producer loads
+//                  the tile's residual (if any) into the next ring entries, so it is in flight while the consumers finish the previous tile.
 //   warp-groups 1-2  consumers: group g owns tile rows 64g..64g+63.  Per k-block it issues BLOCK_K/16 x wgmma.m64nBLOCK_Nk16
 //                  (three per step in the fp32-accurate fused-split mode) into its register accumulator and releases the ring stage
 //                  one k-block later (wgmma.wait_group 1).  The epilogue of its rows follows: folded-BN scale/bias, residual (before
@@ -176,7 +177,23 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   uint8_t* staging = smem_b + STAGES * B_STAGE_BYTES;  // NSTG x 16 KiB
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + NSTG * STAGING_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* res_bar = empty_bar + STAGES;  // residual chunk landed in the staging buffer
+  uint64_t* res_bar = empty_bar + STAGES;  // residual chunk landed in the staging buffer (configurations without ring slots only)
+
+  // Residual tile: a 16 KiB box per staging chunk (CHUNK_COLS columns x 128 rows).  Where a ring stage has room for such boxes (A part first, then B part),
+  // the producer loads the whole residual tile into the ring entries that follow the tile's last k-block, so it is in flight while the previous tile's
+  // epilogue runs; the consumers release each entry after reading its last chunk.  The 32-channel non-split stages (8 KiB parts) have no room: there
+  // one consumer thread loads each chunk into the staging buffer inside the epilogue.
+  constexpr int CHUNK_COLS = 128 / (int)sizeof(TOut);  // output columns per 128-byte staging row
+  constexpr int NCHUNKS = (BLOCK_N + CHUNK_COLS - 1) / CHUNK_COLS;
+  constexpr int RES_SLOTS_A = A_STAGE_BYTES / STAGING_BYTES;
+  constexpr int RES_SLOTS = RES_SLOTS_A + B_STAGE_BYTES / STAGING_BYTES;  // residual chunks per ring entry
+  constexpr bool RES_RING = RES_SLOTS > 0;
+  const bool res_ring = RES_RING && p.res != nullptr && p.rowmax == nullptr;
+  auto res_slot = [&](int s, int slot) -> uint8_t* {
+    return slot < RES_SLOTS_A ? smem_a + s * A_STAGE_BYTES + slot * STAGING_BYTES : smem_b + s * B_STAGE_BYTES + (slot - RES_SLOTS_A) * STAGING_BYTES;
+  };
+  // chunks of the N tile at n0 that hold output columns (the Cout tail of the last N tile has fewer)
+  auto chunks_of = [&](int n0) { return min(NCHUNKS, (p.Cout - n0 + CHUNK_COLS - 1) / CHUNK_COLS); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -184,7 +201,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_d) : "memory");
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], CONSUMER_WARPS); }
-    mbar_init(res_bar, 1);
+    if constexpr (!RES_RING) mbar_init(res_bar, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -264,6 +281,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      if constexpr (RES_RING) if (res_ring) {  // the residual tile: RES_SLOTS chunk boxes per ring entry
+        const int nch = chunks_of(tc.n0);
+        for (int ch = 0; ch < nch; ++ch) {
+          const int slot = ch % RES_SLOTS;
+          if (slot == 0) {
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)(min(RES_SLOTS, nch - ch) * p.BW * p.BH * 128));
+          }
+          uint8_t* dst = res_slot(stage, slot);
+          tma_load_4d(&tmap_r, &full_bar[stage], dst, tc.n0 + ch * CHUNK_COLS, tc.w0, tc.h0, tc.img);
+          if constexpr (PAIR) tma_load_4d(&tmap_r2, &full_bar[stage], dst + STAGING_BYTES / 2, tc.n0 + ch * CHUNK_COLS, tc.w0, tc.h0, tc.img);
+          if (slot == RES_SLOTS - 1 || ch == nch - 1) {
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
     }
     return;
   }
@@ -274,7 +307,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   const int r0 = g * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2);  // accumulator rows r0 and r0 + 8 of this thread
   const int cq = 2 * (lane & 3);              // first of the two adjacent accumulator columns
   constexpr int NACC = BLOCK_N / 2;
-  constexpr int CHUNK_COLS = 128 / (int)sizeof(TOut);  // output columns per 128-byte staging row
   const bool post = (p.act & FB200_ACT_RESIDUAL_AFTER) != 0;
   const bool has_res = p.res != nullptr;
   float acc[NACC];
@@ -340,21 +372,31 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       }
       continue;
     }
+    const int nch = chunks_of(tc.n0);
 #pragma unroll
-    for (int ch = 0; ch < (BLOCK_N + CHUNK_COLS - 1) / CHUNK_COLS; ++ch) {
+    for (int ch = 0; ch < NCHUNKS; ++ch) {
       const int c0 = ch * CHUNK_COLS;
-      if (tc.n0 + c0 >= p.Cout) break;  // uniform across the consumers
+      if (ch >= nch) break;  // uniform across the consumers
       uint8_t* stg = staging + (chunk_ctr % NSTG) * STAGING_BYTES;
+      const uint8_t* res = stg;  // residual chunk, same swizzled layout as the staging tile
       if (ct == 0) {
         tma_store_wait_read<NSTG - 1>();  // the TMA store that last used this staging buffer has finished READING it
-        if (has_res) {  // the [BW x BH x CHUNK_COLS] residual box lands in the staging buffer; each thread adds and overwrites its own elements
+        if constexpr (!RES_RING) if (has_res) {  // the [BW x BH x CHUNK_COLS] residual box lands in the staging buffer; each thread adds and overwrites its own elements
           mbar_arrive_expect_tx(res_bar, (uint32_t)(p.BW * p.BH * 128));
           tma_load_4d(&tmap_r, res_bar, stg, tc.n0 + c0, tc.w0, tc.h0, tc.img);
           if constexpr (PAIR) tma_load_4d(&tmap_r2, res_bar, stg + STAGING_BYTES / 2, tc.n0 + c0, tc.w0, tc.h0, tc.img);
         }
       }
       consumer_bar();
-      if (has_res) { mbar_wait(res_bar, res_phase); res_phase ^= 1; }
+      if constexpr (RES_RING) {
+        if (res_ring) {
+          if (ch % RES_SLOTS == 0) mbar_wait(&full_bar[stage], phase);
+          res = res_slot(stage, ch % RES_SLOTS);
+        }
+      } else if (has_res) {
+        mbar_wait(res_bar, res_phase);
+        res_phase ^= 1;
+      }
 #pragma unroll
       for (int jj = 0; jj < CHUNK_COLS / 8; ++jj) {
         const int j = c0 / 8 + jj;
@@ -374,16 +416,16 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           auto add_residual = [&]() {
             if (!has_res) return;
             if constexpr (PAIR) {
-              const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(stg + off));
-              const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(stg + STAGING_BYTES / 2 + off));
+              const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(res + off));
+              const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(res + STAGING_BYTES / 2 + off));
               v0 += fh.x + fl.x;
               v1 += fh.y + fl.y;
             } else if constexpr (sizeof(TOut) == 2) {
-              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(stg + off));
+              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res + off));
               v0 += f.x;
               v1 += f.y;
             } else {
-              const float2 f = *reinterpret_cast<const float2*>(stg + off);
+              const float2 f = *reinterpret_cast<const float2*>(res + off);
               v0 += f.x;
               v1 += f.y;
             }
@@ -402,6 +444,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           } else {
             *reinterpret_cast<float2*>(stg + off) = make_float2(v0, v1);
           }
+        }
+      }
+      if constexpr (RES_RING) {
+        if (res_ring && (ch % RES_SLOTS == RES_SLOTS - 1 || ch == nch - 1)) {  // last chunk of this ring entry read by the whole warp: release it
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
       fence_proxy_async();
