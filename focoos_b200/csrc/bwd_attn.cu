@@ -222,11 +222,18 @@ extern "C" int fb200_msda_bwd(const float* value, int v_pitch, const float* oa, 
                               const int* shapes_host, int L, int P, int B, int S, int Q, int heads, float* dvalue, int dv_pitch, float* doa, int doa_pitch,
                               void* stream) {
   FB_CHECK_ARG(value && oa && ref && dout && shapes_host && dvalue && doa, "msda_bwd: null pointer");
-  FB_CHECK_ARG(L >= 1 && L <= MSDA_MAX_LEVELS && L * P <= 32, "msda_bwd: levels*points must be <= 32");
+  FB_CHECK_ARG(L >= 1 && L <= MSDA_MAX_LEVELS && L * P <= 32, "msda_bwd: levels*points must be <= 32 (L=%d P=%d)", L, P);
   MsdaShapesB sh;
   int start = 0;
   for (int l = 0; l < L; ++l) { sh.h[l] = shapes_host[2 * l]; sh.w[l] = shapes_host[2 * l + 1]; sh.start[l] = start; start += sh.h[l] * sh.w[l]; }
   FB_CHECK_ARG(start == S, "msda_bwd: sum of level sizes (%d) != S (%d)", start, S);
+  // a pitch below the row width would make the warps of neighbouring rows read, and accumulate into, each other's elements
+  const int oa_w = heads * L * P * 3, v_w = heads * 32;
+  FB_CHECK_ARG(oa_pitch >= oa_w, "msda_bwd: oa_pitch (%d) < heads*L*P*3 (%d)", oa_pitch, oa_w);
+  FB_CHECK_ARG(doa_pitch >= oa_w, "msda_bwd: doa_pitch (%d) < heads*L*P*3 (%d)", doa_pitch, oa_w);
+  FB_CHECK_ARG(v_pitch >= v_w, "msda_bwd: v_pitch (%d) < heads*32 (%d)", v_pitch, v_w);
+  FB_CHECK_ARG(dv_pitch >= v_w, "msda_bwd: dv_pitch (%d) < heads*32 (%d)", dv_pitch, v_w);
+  FB_CHECK_ARG(do_pitch >= v_w, "msda_bwd: do_pitch (%d) < heads*32 (%d)", do_pitch, v_w);
   const int64_t total = (int64_t)B * Q * heads;
   msda_bwd_kernel<<<(unsigned)cdiv(total, 8), 256, 0, (cudaStream_t)stream>>>(value, v_pitch, oa, oa_pitch, ref, dout, do_pitch, sh, L, P, S, Q, heads, total, dvalue,
                                                                              dv_pitch, doa, doa_pitch);

@@ -384,7 +384,8 @@ int fb200_layernorm_bwd(const float* x, const float* res, const float* gamma, co
 int fb200_attention_bwd(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, const float* o, int o_pitch,
                         const float* dout, int do_pitch, int B, int Lq, int Lk, int heads, int head_dim, float scale, float* dq, int dq_pitch,
                         float* dk, int dk_pitch, float* dv, int dv_pitch, void* stream);
-/* adjoint of fb200_msda: dvalue [B,S,heads*32] must be zero-initialised (accumulated with atomics); doa like oa */
+/* adjoint of fb200_msda (fp32): the gradient is ADDED to dvalue [B,S,heads*32] with atomics (zero it for a plain gradient); doa like oa, overwritten.
+ * Pitches: v_pitch, do_pitch, dv_pitch >= heads*32 and oa_pitch, doa_pitch >= heads*L*P*3, else FB200_ERR_INVALID without a launch. */
 int fb200_msda_bwd(const float* value, int v_pitch, const float* oa, int oa_pitch, const float* ref, const float* dout, int do_pitch,
                    const int* shapes_host, int L, int P, int B, int S, int Q, int heads, float* dvalue, int dv_pitch, float* doa, int doa_pitch,
                    void* stream);
