@@ -195,6 +195,17 @@ extern "C" int fb200_attention_bwd(const float* q, int q_pitch, const float* k, 
                                    float* dk, int dk_pitch, float* dv, int dv_pitch, void* stream) {
   FB_CHECK_ARG(q && k && v && o && dout && dq && dk && dv, "attention_bwd: null pointer");
   FB_CHECK_ARG(head_dim == HD, "attention_bwd: head_dim must be 32");
+  FB_CHECK_ARG(B > 0 && Lq > 0 && Lk > 0 && heads > 0, "attention_bwd: B, Lq, Lk and heads must be positive (got %d, %d, %d, %d)", B, Lq, Lk, heads);
+  // a pitch below the row width would make neighbouring rows overlap (and the gradients of one row overwrite another's)
+  const int w = heads * HD;
+  FB_CHECK_ARG(q_pitch >= w, "attention_bwd: q_pitch (%d) < heads*32 (%d)", q_pitch, w);
+  FB_CHECK_ARG(k_pitch >= w, "attention_bwd: k_pitch (%d) < heads*32 (%d)", k_pitch, w);
+  FB_CHECK_ARG(v_pitch >= w, "attention_bwd: v_pitch (%d) < heads*32 (%d)", v_pitch, w);
+  FB_CHECK_ARG(o_pitch >= w, "attention_bwd: o_pitch (%d) < heads*32 (%d)", o_pitch, w);
+  FB_CHECK_ARG(do_pitch >= w, "attention_bwd: do_pitch (%d) < heads*32 (%d)", do_pitch, w);
+  FB_CHECK_ARG(dq_pitch >= w, "attention_bwd: dq_pitch (%d) < heads*32 (%d)", dq_pitch, w);
+  FB_CHECK_ARG(dk_pitch >= w, "attention_bwd: dk_pitch (%d) < heads*32 (%d)", dk_pitch, w);
+  FB_CHECK_ARG(dv_pitch >= w, "attention_bwd: dv_pitch (%d) < heads*32 (%d)", dv_pitch, w);
   auto bytes = [&](int pitch) { return ((size_t)2 * Lq * pitch + (size_t)2 * Lk * pitch + 2 * Lq) * sizeof(float); };
   const bool vec = bytes(36) <= 227 * 1024;   // float4 rows when the four planes fit at the 36-float pitch, else the 33-float scalar layout
   const size_t smem = bytes(vec ? 36 : 33);

@@ -134,6 +134,15 @@ __global__ void __launch_bounds__(256) attention_masked_kernel(const T* __restri
   if (q_ok) out[((int64_t)b * Lq + qi) * out_pitch + h * 32 + lane] = from_f<T>(o / l_run);
 }
 
+// fp32 / fp16 rows (k / v pitches multiples of 4); also the streaming fallback of fb200_attention (mask == nullptr) above the resident kernel's key count
+int attention_masked_simt(const void* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, const uint8_t* mask, int LkP, const int* allowed, void* out,
+                          int out_pitch, int dtype, int B, int Lq, int Lk, int heads, float scale, cudaStream_t st) {
+  dim3 grid((unsigned)(B * heads), (unsigned)cdiv(Lq, MA_QPB));
+  FB_DISPATCH_DTYPE(dtype, T, (attention_masked_kernel<T><<<grid, 256, 0, st>>>((const T*)q, q_pitch, (const T*)k, k_pitch, (const T*)v, v_pitch, mask, LkP, allowed, (T*)out, out_pitch, Lq, Lk, heads, scale)));
+  FB_CHECK_LAUNCH("attention_masked");
+  return FB200_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // out[r, 0..N-2] = softmax(x[r, 0..N-1])[..., :-1]     (one warp per row)
 // ---------------------------------------------------------------------------------------------------------------------
@@ -486,15 +495,19 @@ extern "C" int fb200_attention_masked(const void* q, int q_pitch, const void* k,
                                       void* stream) {
   FB_CHECK_ARG(q && k && v && out && head_dim == 32, "attention_masked: null pointer or head_dim != 32");
   FB_CHECK_ARG((mask == nullptr) == (allowed == nullptr), "attention_masked: mask and allowed go together");
+  FB_CHECK_ARG(B > 0 && Lq > 0 && Lk > 0 && heads > 0, "attention_masked: B, Lq, Lk and heads must be positive (got %d, %d, %d, %d)", B, Lq, Lk, heads);
   FB_CHECK_ARG(k_pitch % 4 == 0 && v_pitch % 4 == 0, "attention_masked: k/v pitches must be multiples of 4");
+  const int w = heads * 32;  // a pitch below the row width would make neighbouring rows overlap
+  FB_CHECK_ARG(q_pitch >= w, "attention_masked: q_pitch (%d) < heads*32 (%d)", q_pitch, w);
+  FB_CHECK_ARG(k_pitch >= w, "attention_masked: k_pitch (%d) < heads*32 (%d)", k_pitch, w);
+  FB_CHECK_ARG(v_pitch >= w, "attention_masked: v_pitch (%d) < heads*32 (%d)", v_pitch, w);
+  FB_CHECK_ARG(out_pitch >= w, "attention_masked: out_pitch (%d) < heads*32 (%d)", out_pitch, w);
+  FB_CHECK_ARG(mask == nullptr || LkP >= Lk, "attention_masked: LkP (%d) < Lk (%d): every key needs a mask byte", LkP, Lk);
   if (dtype == FB200_F16 && q_pitch % 8 == 0 && k_pitch % 8 == 0 && v_pitch % 8 == 0 && out_pitch % 2 == 0 && (mask == nullptr || LkP % 4 == 0) &&
       (((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0 && ((uintptr_t)out & 3) == 0)  // tensor-core path (norm_attn.cu)
     return attention_mma_stream((const __half*)q, q_pitch, (const __half*)k, k_pitch, (const __half*)v, v_pitch, mask, LkP, allowed, (__half*)out, out_pitch,
                                 B, Lq, Lk, heads, scale, (cudaStream_t)stream);
-  dim3 grid((unsigned)(B * heads), (unsigned)cdiv(Lq, MA_QPB));
-  FB_DISPATCH_DTYPE(dtype, T, (attention_masked_kernel<T><<<grid, 256, 0, (cudaStream_t)stream>>>((const T*)q, q_pitch, (const T*)k, k_pitch, (const T*)v, v_pitch, mask, LkP, allowed, (T*)out, out_pitch, Lq, Lk, heads, scale)));
-  FB_CHECK_LAUNCH("attention_masked");
-  return FB200_OK;
+  return attention_masked_simt(q, q_pitch, k, k_pitch, v, v_pitch, mask, LkP, allowed, out, out_pitch, dtype, B, Lq, Lk, heads, scale, (cudaStream_t)stream);
 }
 
 extern "C" int fb200_softmax_drop_last(const float* x, int64_t rows, int N, int pitch, float* out, void* stream) {

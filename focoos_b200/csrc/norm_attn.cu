@@ -116,6 +116,19 @@ int attention_mma(const __half* q, int q_pitch, const __half* k, int k_pitch, co
                   int Lq, int Lk, int heads, float scale, cudaStream_t st);
 int attention_mma_split_stream(const float* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, int kv_pair, int kv_lo_off, const uint8_t* mask, int MP,
                                const int* allowed, float* out, int out_pitch, int B, int Lq, int Lk, int heads, float scale, cudaStream_t st);
+int attention_mma_stream(const __half* q, int q_pitch, const __half* k, int k_pitch, const __half* v, int v_pitch, const uint8_t* mask, int LkP,
+                         const int* allowed, __half* out, int out_pitch, int B, int Lq, int Lk, int heads, float scale, cudaStream_t st);
+int attention_masked_simt(const void* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, const uint8_t* mask, int LkP, const int* allowed, void* out,
+                          int out_pitch, int dtype, int B, int Lq, int Lk, int heads, float scale, cudaStream_t st);  // mf_ops.cu
+
+// Shared memory of the resident kernels, which stage the whole K and V of a (batch, head): above 227 KiB per block the entry points take the streaming kernels instead.
+constexpr size_t kAttnSmemMax = 227 * 1024;
+constexpr int AM_PITCH = 40;  // halves per smem row of the tensor-core kernels (32 + 8 pad): conflict-free ldmatrix
+inline size_t attention_simt_smem(int Lk) { return ((size_t)Lk * 33 + (size_t)Lk * 32 + (size_t)8 * Lk + 8 * 32) * sizeof(float); }  // attention_kernel: Lk <= 792
+inline size_t attention_mma_smem(int Lk) { return ((size_t)2 * ((Lk + 63) & ~63) + 64) * AM_PITCH * sizeof(__half); }                 // attention_mma_kernel: Lk <= 1408
+// attention_mma_split_kernel with NW warps (16 queries each) per CTA: L <= 640 for self-attention, Lk <= 704 for Lq <= 32
+inline size_t attention_split_smem(int Lk, int NW) { return ((size_t)4 * ((Lk + 63) & ~63) + 2 * 16 * NW) * AM_PITCH * sizeof(__half); }
+int attention_split_warps(int Lq);
 }  // namespace fb200
 using namespace fb200;
 
@@ -136,13 +149,25 @@ extern "C" int fb200_attention(const void* q, int q_pitch, const void* k, int k_
                                void* stream) {
   FB_CHECK_ARG(q && k && v && out, "attention: null pointer");
   FB_CHECK_ARG(head_dim == 32, "attention: head_dim must be 32 (got %d)", head_dim);
+  FB_CHECK_ARG(B > 0 && Lq > 0 && Lk > 0 && heads > 0, "attention: B, Lq, Lk and heads must be positive (got %d, %d, %d, %d)", B, Lq, Lk, heads);
   FB_CHECK_ARG(q_pitch % 4 == 0 && k_pitch % 4 == 0 && v_pitch % 4 == 0, "attention: pitches must be multiples of 4");
+  const int w = heads * 32;  // a pitch below the row width would make neighbouring rows overlap
+  FB_CHECK_ARG(q_pitch >= w, "attention: q_pitch (%d) < heads*32 (%d)", q_pitch, w);
+  FB_CHECK_ARG(k_pitch >= w, "attention: k_pitch (%d) < heads*32 (%d)", k_pitch, w);
+  FB_CHECK_ARG(v_pitch >= w, "attention: v_pitch (%d) < heads*32 (%d)", v_pitch, w);
+  FB_CHECK_ARG(out_pitch >= w, "attention: out_pitch (%d) < heads*32 (%d)", out_pitch, w);
   if (dtype == FB200_F16 && q_pitch % 8 == 0 && k_pitch % 8 == 0 && v_pitch % 8 == 0 && out_pitch % 2 == 0 &&
-      (((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0 && ((uintptr_t)out & 3) == 0)
-    return attention_mma((const __half*)q, q_pitch, (const __half*)k, k_pitch, (const __half*)v, v_pitch, (__half*)out, out_pitch, B, Lq, Lk, heads, scale,
-                         (cudaStream_t)stream);
-  const size_t smem = ((size_t)Lk * 33 + (size_t)Lk * 32 + (size_t)8 * Lk + 8 * 32) * sizeof(float);
-  FB_CHECK_ARG(smem <= 227 * 1024, "attention: Lk=%d does not fit shared memory", Lk);
+      (((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0 && ((uintptr_t)out & 3) == 0) {
+    if (attention_mma_smem(Lk) <= kAttnSmemMax)
+      return attention_mma((const __half*)q, q_pitch, (const __half*)k, k_pitch, (const __half*)v, v_pitch, (__half*)out, out_pitch, B, Lq, Lk, heads, scale,
+                           (cudaStream_t)stream);
+    return attention_mma_stream((const __half*)q, q_pitch, (const __half*)k, k_pitch, (const __half*)v, v_pitch, nullptr, 0, nullptr, (__half*)out, out_pitch, B, Lq, Lk,
+                                heads, scale, (cudaStream_t)stream);
+  }
+  if (attention_simt_smem(Lk) > kAttnSmemMax)  // keys streamed 128 at a time by the masked kernel, without a mask
+    return attention_masked_simt(q, q_pitch, k, k_pitch, v, v_pitch, nullptr, 0, nullptr, out, out_pitch, dtype, B, Lq, Lk, heads, scale, (cudaStream_t)stream);
+  const size_t smem = attention_simt_smem(Lk);
+  FB_CHECK_ARG(smem <= kAttnSmemMax, "attention: Lk=%d does not fit shared memory", Lk);
   dim3 grid(B * heads, (unsigned)cdiv(Lq, ATT_QT));
   cudaStream_t st = (cudaStream_t)stream;
   static bool configured = false;
@@ -168,8 +193,11 @@ extern "C" int fb200_attention_masked_split(const float* q, int q_pitch, const v
   FB_CHECK_ARG(kv_dtype == FB200_F32 || kv_dtype == FB200_F16PAIR, "attention_masked_split: k / v are fp32 tensors or fp16 [hi|lo] pairs");
   FB_CHECK_ARG(B > 0 && Lq > 0 && Lk > 0 && heads > 0, "attention_masked_split: bad shape");
   FB_CHECK_ARG(q_pitch % 4 == 0 && out_pitch % 2 == 0 && ((uintptr_t)q & 15) == 0 && ((uintptr_t)out & 7) == 0, "attention_masked_split: q / out pitches / alignment");
+  FB_CHECK_ARG(q_pitch >= heads * 32, "attention_masked_split: q_pitch (%d) < heads*32 (%d)", q_pitch, heads * 32);
+  FB_CHECK_ARG(out_pitch >= heads * 32, "attention_masked_split: out_pitch (%d) < heads*32 (%d)", out_pitch, heads * 32);
   if (kv_dtype == FB200_F32) {
     FB_CHECK_ARG(k_pitch % 4 == 0 && v_pitch % 4 == 0 && (((uintptr_t)k | (uintptr_t)v) & 15) == 0, "attention_masked_split: k / v pitches / alignment");
+    FB_CHECK_ARG(k_pitch >= heads * 32 && v_pitch >= heads * 32, "attention_masked_split: k_pitch (%d) / v_pitch (%d) < heads*32 (%d)", k_pitch, v_pitch, heads * 32);
   } else {  // pair rows: hi plane at the pointer, lo plane kv_lo_off halves further, 16-byte copies
     FB_CHECK_ARG(k_pitch % 8 == 0 && v_pitch % 8 == 0 && kv_lo_off % 8 == 0 && kv_lo_off >= heads * 32 && k_pitch >= kv_lo_off + heads * 32 && v_pitch >= kv_lo_off + heads * 32 &&
                      (((uintptr_t)k | (uintptr_t)v) & 15) == 0, "attention_masked_split: pair k / v need 16-byte aligned planes inside the row pitch");
@@ -183,10 +211,19 @@ extern "C" int fb200_attention_split(const float* q, int q_pitch, const float* k
                                      int Lq, int Lk, int heads, int head_dim, float scale, void* stream) {
   FB_CHECK_ARG(q && k && v && out, "attention_split: null pointer");
   FB_CHECK_ARG(head_dim == 32, "attention_split: head_dim must be 32 (got %d)", head_dim);
+  FB_CHECK_ARG(B > 0 && Lq > 0 && Lk > 0 && heads > 0, "attention_split: B, Lq, Lk and heads must be positive (got %d, %d, %d, %d)", B, Lq, Lk, heads);
   FB_CHECK_ARG(q_pitch % 4 == 0 && k_pitch % 4 == 0 && v_pitch % 4 == 0 && out_pitch % 2 == 0 && (((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0 &&
                    ((uintptr_t)out & 7) == 0, "attention_split: pitches / alignment");
   FB_CHECK_ARG(out_dtype == FB200_F32 || out_dtype == FB200_F16PAIR, "attention_split: out_dtype must be F32 or F16PAIR");
+  const int w = heads * 32;  // a pitch below the row width would make neighbouring rows overlap
+  FB_CHECK_ARG(q_pitch >= w, "attention_split: q_pitch (%d) < heads*32 (%d)", q_pitch, w);
+  FB_CHECK_ARG(k_pitch >= w, "attention_split: k_pitch (%d) < heads*32 (%d)", k_pitch, w);
+  FB_CHECK_ARG(v_pitch >= w, "attention_split: v_pitch (%d) < heads*32 (%d)", v_pitch, w);
+  FB_CHECK_ARG(out_pitch >= w, "attention_split: out_pitch (%d) < heads*32 (%d)", out_pitch, w);
   FB_CHECK_ARG(out_dtype != FB200_F16PAIR || out_pitch >= 2 * heads * 32, "attention_split: pair rows are [hi(heads*32) | lo(heads*32)]");
+  // fp32 rows above the resident kernel's shared memory: the masked streaming kernel without a mask (keys staged 256 at a time); pair rows are refused there
+  if (out_dtype == FB200_F32 && attention_split_smem(Lk, attention_split_warps(Lq)) > kAttnSmemMax)
+    return attention_mma_split_stream(q, q_pitch, k, k_pitch, v, v_pitch, 0, 0, nullptr, 0, nullptr, (float*)out, out_pitch, B, Lq, Lk, heads, scale, (cudaStream_t)stream);
   return attention_mma_split(q, q_pitch, k, k_pitch, v, v_pitch, (float*)out, out_pitch, B, Lq, Lk, heads, scale, out_dtype == FB200_F16PAIR ? 1 : 0, (cudaStream_t)stream);
 }
 
@@ -196,8 +233,6 @@ extern "C" int fb200_attention_split(const float* q, int q_pitch, const float* k
 // warp runs a flash-style online softmax over 64-key blocks for 16 queries.  4 warps = 64 queries per CTA.
 // ------------------------------------------------------------------------------------------------
 namespace fb200 {
-
-constexpr int AM_PITCH = 40;  // halves per smem row (32 + 8 pad): conflict-free ldmatrix
 
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], const __half* p) {
   const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
@@ -468,16 +503,19 @@ __global__ void __launch_bounds__(384) attention_mma_split_kernel(const float* _
   }
 }
 
-int attention_mma_split(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, float* out, int out_pitch, int B, int Lq, int Lk,
-                        int heads, float scale, int out_pair, cudaStream_t st) {
-  const int LkP = (Lk + 63) & ~63;
+int attention_split_warps(int Lq) {
   // queries per CTA: as few CTAs per (batch, head) as 16 warps allow (each CTA stages the whole K and V of its head), warps rounded to what the last block needs
   static int max_q = -1;  // FB200_ATTN_QB: upper bound of queries per CTA (multiple of 16, <= 192); tuning knob
   if (max_q < 0) { const char* e = getenv("FB200_ATTN_QB"); max_q = e ? atoi(e) : 192; if (max_q < 16 || max_q > 192) max_q = 192; }
   const int nblk = (int)cdiv(Lq, max_q);
-  const int NW = (int)cdiv(cdiv(Lq, nblk), 16);
-  const size_t smem = ((size_t)4 * LkP + 2 * 16 * NW) * AM_PITCH * sizeof(__half);
-  if (smem > 227 * 1024) { set_error("attention(split): Lk=%d does not fit shared memory", Lk); return FB200_ERR_UNSUPPORTED; }
+  return (int)cdiv(cdiv(Lq, nblk), 16);
+}
+
+int attention_mma_split(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, float* out, int out_pitch, int B, int Lq, int Lk,
+                        int heads, float scale, int out_pair, cudaStream_t st) {
+  const int NW = attention_split_warps(Lq);
+  const size_t smem = attention_split_smem(Lk, NW);
+  if (smem > kAttnSmemMax) { set_error("attention(split): Lk=%d does not fit shared memory", Lk); return FB200_ERR_UNSUPPORTED; }
   static bool configured = false;
   if (!configured) {
     cudaFuncSetAttribute(attention_mma_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
@@ -692,9 +730,8 @@ int attention_mma_split_stream(const float* q, int q_pitch, const void* k, int k
 
 int attention_mma(const __half* q, int q_pitch, const __half* k, int k_pitch, const __half* v, int v_pitch, __half* out, int out_pitch, int B,
                   int Lq, int Lk, int heads, float scale, cudaStream_t st) {
-  const int LkP = (Lk + 63) & ~63;
-  const size_t smem = ((size_t)2 * LkP + 64) * AM_PITCH * sizeof(__half);
-  if (smem > 227 * 1024) { set_error("attention(mma): Lk=%d does not fit shared memory", Lk); return FB200_ERR_UNSUPPORTED; }
+  const size_t smem = attention_mma_smem(Lk);
+  if (smem > kAttnSmemMax) { set_error("attention(mma): Lk=%d does not fit shared memory", Lk); return FB200_ERR_UNSUPPORTED; }
   static bool configured = false;
   if (!configured) {
     cudaFuncSetAttribute(attention_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);

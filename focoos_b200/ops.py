@@ -556,8 +556,8 @@ class CudaBackend:
     def attention_bwd(self, q, k, v, o, do, heads, scale, dq, dk, dv):
         self._cuda(q, k, v, o, do, dq, dk, dv)
         B, Lq, C = q.shape
-        self._call("fb200_attention_bwd", _p(q), q.stride(1), _p(k), k.stride(1), _p(v), v.stride(1), _p(o), o.stride(1), _p(do), do.stride(1), B, Lq, k.shape[1], heads,
-                   C // heads, scale, _p(dq), dq.stride(1), _p(dk), dk.stride(1), _p(dv), dv.stride(1), _stream())
+        self._call("fb200_attention_bwd", _p(q), _pitch(q), _p(k), _pitch(k), _p(v), _pitch(v), _p(o), _pitch(o), _p(do), _pitch(do), B, Lq, k.shape[1], heads,
+                   C // heads, scale, _p(dq), _pitch(dq), _p(dk), _pitch(dk), _p(dv), _pitch(dv), _stream())
 
     def msda_bwd(self, value, oa, ref, do, shapes, P, heads, dvalue, doa):
         self._cuda(value, oa, ref, do, dvalue, doa)

@@ -150,12 +150,17 @@ int fb200_box_refine_qpos(const float* delta, const float* ref_in, float* ref_ou
 int fb200_sigmoid_rows(const float* x, int x_pitch, int64_t M, int C, float* out, void* stream);
 
 /* ---- a4,a9: softmax(Q K^T * scale) V per (batch, head); nn.MultiheadAttention core
- * (SURVEY A.6).  q/k/v/out rows are tokens; head h uses columns [h*hd, (h+1)*hd). hd must be 32. */
+ * (SURVEY A.6).  q/k/v/out rows are tokens; head h uses columns [h*hd, (h+1)*hd). hd must be 32.
+ * B, Lq, Lk, heads > 0 and every pitch >= heads*32, else FB200_ERR_INVALID without a launch.  Any Lk: the kernels that keep a head's K and V in shared memory
+ * take Lk <= 792 (fp32, or fp16 rows that are not 16-byte aligned) and Lk <= 1408 (fp16 tensor cores); longer keys are streamed by the kernels of
+ * fb200_attention_masked without a mask. */
 int fb200_attention(const void* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, void* out,
                     int out_pitch, int dtype, int B, int Lq, int Lk, int heads, int head_dim, float scale, void* stream);
 /* fp32 tensors on the fp16 tensor cores (precision="fp32_tc"): Q, K, V are split into [hi|lo] halves on the way into shared memory and every product
  * is formed as hi*hi + hi*lo + lo*hi with fp32 accumulation (mma.sync m16n8k16), softmax in fp32.  Same semantics as fb200_attention(FB200_F32).
- * out_dtype FB200_F32: fp32 rows.  FB200_F16PAIR: rows written as [hi(heads*32) | lo(heads*32)] fp16 (out_pitch in halves) - the operand of the out_proj linear. */
+ * out_dtype FB200_F32: fp32 rows.  FB200_F16PAIR: rows written as [hi(heads*32) | lo(heads*32)] fp16 (out_pitch in halves) - the operand of the out_proj linear.
+ * The resident kernel takes self-attention up to L = 640 (Lk = 704 for Lq <= 32); above that fp32 rows are streamed by the kernel of fb200_attention_masked_split
+ * without a mask, and pair rows are refused with FB200_ERR_UNSUPPORTED (no caller writes pair rows at such lengths). */
 int fb200_attention_split(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, void* out, int out_dtype, int out_pitch, int B,
                           int Lq, int Lk, int heads, int head_dim, float scale, void* stream);
 
@@ -218,7 +223,8 @@ int fb200_attn_mask_build(const void* x, int dtype, int B, int Lk, int Qp, int Q
 
 /* softmax(q k^T * scale + mask) v per (batch, head), keys streamed (Lk up to H/8*W/8), head_dim 32; mask/allowed as above and shared
  * by all heads (the reference replicates a [B*heads,Q,Lk] bool tensor, :513); mask == NULL -> unmasked.
- * nn.MultiheadAttention inside CrossAttentionLayer (nn/layers/transformer.py:206-238). */
+ * nn.MultiheadAttention inside CrossAttentionLayer (nn/layers/transformer.py:206-238).
+ * B, Lq, Lk, heads > 0, every pitch >= heads*32 and (with a mask) LkP >= Lk, else FB200_ERR_INVALID without a launch. */
 int fb200_attention_masked(const void* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, const uint8_t* mask, int LkP,
                            const int* allowed, void* out, int out_pitch, int dtype, int B, int Lq, int Lk, int heads, int head_dim, float scale,
                            void* stream);
@@ -380,7 +386,8 @@ int fb200_resize_bilinear_bwd(const float* dy, int dy_pitch, int B, int H, int W
 /* nn.LayerNorm backward over s = x (+ res): dx is the gradient w.r.t. s */
 int fb200_layernorm_bwd(const float* x, const float* res, const float* gamma, const float* dy, int64_t M, int C, float eps, float* dx, float* dgamma,
                         float* dbeta, int accumulate, void* workspace, void* stream);
-/* nn.MultiheadAttention core backward (o = forward output) */
+/* nn.MultiheadAttention core backward (o = forward output).  Q, K, V and dO of a (batch, head) stay in shared memory: Lq = Lk up to 433.
+ * B, Lq, Lk, heads > 0 and every pitch >= heads*32, else FB200_ERR_INVALID without a launch. */
 int fb200_attention_bwd(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, const float* o, int o_pitch,
                         const float* dout, int do_pitch, int B, int Lq, int Lk, int heads, int head_dim, float scale, float* dq, int dq_pitch,
                         float* dk, int dk_pitch, float* dv, int dv_pitch, void* stream);
