@@ -860,18 +860,14 @@ extern "C" int64_t fb200_col_workspace_bytes(int C) { return (int64_t)(2 * CR_RO
 static inline dim3 col_grid(int C, int64_t R) { return dim3((unsigned)cdiv(C, 32), (unsigned)std::min<int64_t>(CR_ROWS, cdiv(R, 8))); }
 
 static inline bool col_vec_ok(int C, const void* x, int x_pitch, const void* dy, int dy_pitch, const void* y, int y_pitch) {
-  static int on = -1;  // FB200_COL_VEC=0: the scalar kernels (A/B)
-  if (on < 0) { const char* e = getenv("FB200_COL_VEC"); on = e ? atoi(e) : 1; }
-  if (!on || !(C == 32 || C == 64 || C == 128 || (C > 128 && C % 128 == 0))) return false;
+  if (!(C == 32 || C == 64 || C == 128 || (C > 128 && C % 128 == 0))) return false;
   if (x_pitch % 4 || (dy && dy_pitch % 4) || (y && y_pitch % 4)) return false;
   return ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
 }
 // grid of the column-fixed element-wise kernels: a multiple of C/4 threads (0 = use the generic kernel)
 static inline unsigned cf_grid(int64_t R, int C) {
-  static int on = -1;  // FB200_BN_CF=0: the generic kernels (A/B)
-  if (on < 0) { const char* e = getenv("FB200_BN_CF"); on = e ? atoi(e) : 1; }
   const int cv = C / 4;
-  if (!on || C % 4 || cv <= 0) return 0;
+  if (C % 4 || cv <= 0) return 0;
   int64_t blocks = std::min<int64_t>(cdiv(R * cv, 256), kNumSMs * 16);
   if (cv <= 256) { if (256 % cv) return 0; }           // every block holds whole rows' worth of column groups
   else { if (cv % 256) return 0; const int64_t m = cv / 256; blocks = blocks / m * m; }

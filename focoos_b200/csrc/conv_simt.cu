@@ -17,84 +17,9 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-// ------------------------------------------------------------------------------------------------
-// stem: one thread = one output pixel x CO_PER_THREAD channels. Input NCHW fp32 raw.
-// ------------------------------------------------------------------------------------------------
-template <typename TOut, int COUT, bool U8_NHWC>
-__global__ void __launch_bounds__(128) stem_conv_kernel(const void* __restrict__ img_, int B, int H, int W,
-                                                        const float* __restrict__ w, const float* __restrict__ scale,
-                                                        const float* __restrict__ bias, float m0, float m1, float m2,
-                                                        float s0, float s1, float s2, int act, TOut* __restrict__ out) {
-  __shared__ float ws[27 * COUT];  // [tap*3+ci][co]
-  __shared__ float sc[COUT], bi[COUT];
-  for (int i = threadIdx.x; i < 27 * COUT; i += blockDim.x) {
-    int co = i % COUT, t = i / COUT;  // t = (kh*3+kw)*3+ci ; w layout [co][kh][kw][ci]
-    ws[i] = w[co * 27 + t];
-  }
-  for (int i = threadIdx.x; i < COUT; i += blockDim.x) {
-    sc[i] = scale ? scale[i] : 1.f;
-    bi[i] = bias ? bias[i] : 0.f;
-  }
-  __syncthreads();
-  const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
-  const int64_t total = (int64_t)B * Ho * Wo;
-  const int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (pix >= total) return;
-  const int wo = pix % Wo, ho = (pix / Wo) % Ho, b = pix / ((int64_t)Wo * Ho);
-  const float mean[3] = {m0, m1, m2}, stdv[3] = {s0, s1, s2};
-  float acc[COUT];
-#pragma unroll
-  for (int i = 0; i < COUT; ++i) acc[i] = 0.f;
-  const float* ib = reinterpret_cast<const float*>(img_) + (int64_t)b * 3 * H * W;           // NCHW fp32
-  const uint8_t* ub = reinterpret_cast<const uint8_t*>(img_) + (int64_t)b * H * W * 3;        // NHWC uint8
-#pragma unroll
-  for (int kh = 0; kh < 3; ++kh) {
-    const int hi = ho * 2 - 1 + kh;
-#pragma unroll
-    for (int kw = 0; kw < 3; ++kw) {
-      const int wi = wo * 2 - 1 + kw;
-      const bool ok = hi >= 0 && hi < H && wi >= 0 && wi < W;
-#pragma unroll
-      for (int ci = 0; ci < 3; ++ci) {
-        // same arithmetic as the reference: (x - mean) / std, then the conv sees 0 outside the image
-        float raw = 0.f;
-        if (ok) raw = U8_NHWC ? (float)ub[((int64_t)hi * W + wi) * 3 + ci] : ib[((int64_t)ci * H + hi) * W + wi];
-        const float v = ok ? (raw - mean[ci]) / stdv[ci] : 0.f;
-        const float* wr = &ws[((kh * 3 + kw) * 3 + ci) * COUT];
-#pragma unroll
-        for (int co = 0; co < COUT; ++co) acc[co] = fmaf(v, wr[co], acc[co]);
-      }
-    }
-  }
-  if (act & 256) {  // FB200_F16PAIR output: [hi(COUT) | lo(COUT)] fp16 per pixel (TOut is __half)
-    __half* o = reinterpret_cast<__half*>(out) + pix * 2 * COUT;
-#pragma unroll
-    for (int co = 0; co < COUT; co += 4) {
-      float v[4], h[4], l[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        v[j] = apply_act(acc[co + j] * sc[co + j] + bi[co + j], act);
-        h[j] = __half2float(__float2half_rn(v[j]));
-        l[j] = v[j] - h[j];
-      }
-      store4(o + co, h);
-      store4(o + COUT + co, l);
-    }
-    return;
-  }
-  TOut* o = out + pix * COUT;
-#pragma unroll
-  for (int co = 0; co < COUT; co += 4) {
-    float v[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) v[j] = apply_act(acc[co + j] * sc[co + j] + bi[co + j], act);
-    store4(o + co, v);
-  }
-}
-
 // Tiled stem: a CTA computes a 16 x 16 tile of output pixels.  The 33 x 33 x 3 input patch is read ONCE (coalesced rows), normalised ONCE per input pixel and kept in
 // shared memory as even / odd column planes (the stride-2 taps of 16 neighbouring threads then hit 16 consecutive floats: no bank conflicts); the 27 x 32 weights are
-// read as float4 broadcasts.  The per-pixel kernel above re-loaded and re-normalised (with a division) every input byte for each of the up to nine taps that use it.
+// read as float4 broadcasts.  Each input byte is loaded and normalised (with a division) once, not once for each of the up to nine taps that use it.
 template <typename TOut, bool U8_NHWC, bool RELU>   // RELU: the activation is known to be ReLU (every model family's stem): no generic activation code in the kernel at all
 __global__ void __launch_bounds__(256) stem_conv_tiled_kernel(const void* __restrict__ img_, int B, int H, int W, const float* __restrict__ w,
                                                               const float* __restrict__ scale, const float* __restrict__ bias, float m0, float m1, float m2,
@@ -494,21 +419,18 @@ static int stem_launch(const void* img, bool u8, int B, int H, int W, const floa
   FB_CHECK_ARG(Cout == 32, "stem_conv: only Cout=32 is instantiated (got %d)", Cout);
   FB_CHECK_ARG(B > 0 && H > 0 && W > 0, "stem_conv: bad shape");
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-  const int64_t total = (int64_t)B * Ho * Wo;
   cudaStream_t st = (cudaStream_t)stream;
   const float* m = mean3; const float* s = std3;  // HOST pointers (3 floats each)
   const int tiles_w = (Wo + 15) / 16, tiles_h = (Ho + 15) / 16;
-  static int tiled = -1;  // FB200_STEM_TILED: 0 = the per-pixel kernel, 1 = the tiled one-pixel-per-thread kernel, 2 (default) = two pixels per thread where it applies (A/B)
-  if (tiled < 0) { const char* e = getenv("FB200_STEM_TILED"); tiled = e ? atoi(e) : 2; }
-  const unsigned grid = tiled ? (unsigned)((int64_t)B * tiles_w * tiles_h) : (unsigned)cdiv(total, 128);
+  const unsigned grid = (unsigned)((int64_t)B * tiles_w * tiles_h);
+  // uint8 input with ReLU: two pixels per thread; everything else: one pixel per thread
 #define STEM_LAUNCH(T, U8)                                                                                                                                              \
   do {                                                                                                                                                                  \
-    if (tiled == 2 && U8 && (act & 15) == FB200_ACT_RELU) {                                                                                                               \
+    if (U8 && (act & 15) == FB200_ACT_RELU) {                                                                                                                           \
       if (act & 256) stem_conv_tiled2_kernel<T, true><<<grid, 128, 0, st>>>((const uint8_t*)img, B, H, W, w, scale, bias, m[0], m[1], m[2], s[0], s[1], s[2], (T*)out, tiles_w, tiles_h);   \
       else stem_conv_tiled2_kernel<T, false><<<grid, 128, 0, st>>>((const uint8_t*)img, B, H, W, w, scale, bias, m[0], m[1], m[2], s[0], s[1], s[2], (T*)out, tiles_w, tiles_h);           \
-    } else if (tiled && (act & 15) == FB200_ACT_RELU) stem_conv_tiled_kernel<T, U8, true><<<grid, 256, 0, st>>>(img, B, H, W, w, scale, bias, m[0], m[1], m[2], s[0], s[1], s[2], act, (T*)out, tiles_w, tiles_h);   \
-    else if (tiled) stem_conv_tiled_kernel<T, U8, false><<<grid, 256, 0, st>>>(img, B, H, W, w, scale, bias, m[0], m[1], m[2], s[0], s[1], s[2], act, (T*)out, tiles_w, tiles_h);   \
-    else stem_conv_kernel<T, 32, U8><<<grid, 128, 0, st>>>(img, B, H, W, w, scale, bias, m[0], m[1], m[2], s[0], s[1], s[2], act, (T*)out);                              \
+    } else if ((act & 15) == FB200_ACT_RELU) stem_conv_tiled_kernel<T, U8, true><<<grid, 256, 0, st>>>(img, B, H, W, w, scale, bias, m[0], m[1], m[2], s[0], s[1], s[2], act, (T*)out, tiles_w, tiles_h);   \
+    else stem_conv_tiled_kernel<T, U8, false><<<grid, 256, 0, st>>>(img, B, H, W, w, scale, bias, m[0], m[1], m[2], s[0], s[1], s[2], act, (T*)out, tiles_w, tiles_h);   \
   } while (0)
   if (out_dtype == FB200_F32) { if (u8) STEM_LAUNCH(float, true); else STEM_LAUNCH(float, false); }
   else if (out_dtype == FB200_F16) { if (u8) STEM_LAUNCH(__half, true); else STEM_LAUNCH(__half, false); }

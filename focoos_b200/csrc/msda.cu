@@ -2,8 +2,6 @@
 //   softmax over levels*points  +  sampling-location arithmetic  +  bilinear gather  +  weighted sum.
 // One warp per (batch, query, head); lane = channel of the 32-wide head, so each bilinear tap is one
 // coalesced 64/128-byte row segment of `value` (L2-resident: B*S*256 elements).  Gather/latency bound.
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace fb200 {
@@ -166,11 +164,9 @@ extern "C" int fb200_msda(const void* value, int v_dtype, int v_pitch, const voi
   const int64_t total = (int64_t)B * Q * heads;
   const unsigned grid = (unsigned)cdiv(total, 8);
   cudaStream_t st = (cudaStream_t)stream;
-  // 4-channel vector loads need 8/16-byte aligned rows; FB200_MSDA_SCALAR=1 selects the one-tap-per-load kernel (A/B timing, debugging)
-  static int scalar = -1;
-  if (scalar < 0) { const char* e = getenv("FB200_MSDA_SCALAR"); scalar = e ? atoi(e) : 0; }
+  // 4-channel vector loads need 8/16-byte aligned rows; other rows take the one-tap-per-load kernel
   const size_t velt = v_dtype == FB200_F16 ? 2 : 4, oelt = out_dtype == FB200_F32 ? 4 : 2;
-  const bool quad = !scalar && (v_pitch * velt) % (4 * velt) == 0 && (reinterpret_cast<uintptr_t>(value) % (4 * velt)) == 0 && (out_pitch * oelt) % (4 * oelt) == 0 &&
+  const bool quad = (v_pitch * velt) % (4 * velt) == 0 && (reinterpret_cast<uintptr_t>(value) % (4 * velt)) == 0 && (out_pitch * oelt) % (4 * oelt) == 0 &&
                     (reinterpret_cast<uintptr_t>(out) % (4 * oelt)) == 0;
 #define MSDA_LAUNCH(TV, TOA, TO)                                                                                                                                   \
   do {                                                                                                                                                             \

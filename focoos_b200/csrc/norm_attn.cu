@@ -1,6 +1,4 @@
 // LayerNorm(+residual) and small-sequence multi-head attention (L = 300/400, head_dim = 32).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace fb200 {
@@ -505,8 +503,7 @@ __global__ void __launch_bounds__(384) attention_mma_split_kernel(const float* _
 
 int attention_split_warps(int Lq) {
   // queries per CTA: as few CTAs per (batch, head) as 16 warps allow (each CTA stages the whole K and V of its head), warps rounded to what the last block needs
-  static int max_q = -1;  // FB200_ATTN_QB: upper bound of queries per CTA (multiple of 16, <= 192); tuning knob
-  if (max_q < 0) { const char* e = getenv("FB200_ATTN_QB"); max_q = e ? atoi(e) : 192; if (max_q < 16 || max_q > 192) max_q = 192; }
+  constexpr int max_q = 192;  // upper bound of queries per CTA (multiple of 16)
   const int nblk = (int)cdiv(Lq, max_q);
   return (int)cdiv(cdiv(Lq, nblk), 16);
 }
@@ -703,9 +700,8 @@ __global__ void __launch_bounds__(384) attention_mma_split_stream_kernel(const f
 
 int attention_mma_split_stream(const float* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, int kv_pair, int kv_lo_off, const uint8_t* mask, int MP,
                                const int* allowed, float* out, int out_pitch, int B, int Lq, int Lk, int heads, float scale, cudaStream_t st) {
-
-  static int qb = -1;  // FB200_MATTN_QB: upper bound of queries per CTA (multiple of 16); tuning knob
-  if (qb < 0) { const char* e = getenv("FB200_MATTN_QB"); qb = e ? atoi(e) : 128; if (qb < 16 || qb > 192) qb = 128; }  // one CTA per (batch, head) for the 100-query decoders: K / V staged once (trip 52: 3.12 ms vs 3.31 at 64, 7.15 at 32)
+  // upper bound of queries per CTA (multiple of 16): one CTA per (batch, head) for the 100-query decoders, K / V staged once (trip 52: 3.12 ms vs 3.31 at 64, 7.15 at 32)
+  constexpr int qb = 128;
   const int nblk = (int)cdiv(Lq, qb);
   const int NW = (int)cdiv(cdiv(Lq, nblk), 16);
   static bool configured = false;

@@ -231,12 +231,6 @@ def _split3_weights(w):
     return torch.cat([hi, lo, hi], dim=-1).contiguous()
 
 
-# number of fp16 tensor-core products per conv/linear in precision="fp32_tc" (DetrEngine.mix sets it per stage; tools/error_budget.py measures what each
-# choice costs in parity):  3 = x_hi*W_hi + x_hi*W_lo + x_lo*W_hi (fp32-accurate),  2 = x_hi*W_hi + x_lo*W_hi (weights rounded to fp16),
-# 1 = x_hi*W_hi only (fp16 operands, fp32 storage: the "fp32 residual stream" variant)
-_products = 3
-
-
 def _split3_ok(x, w3, act, algo):
     a = (act & 15)
     return (w3 is not None and algo != ops.ALGO_SIMT and x.dtype == torch.float32 and (x.is_cuda or ops._backend is not None) and a not in (ops.ACT_GELU, 4)
@@ -261,8 +255,6 @@ class _Conv:
     def __call__(self, x, residual=None, out=None, out_dtype=None, act=None, algo=ops.ALGO_AUTO):
         act = self.act if act is None else act
         if _split3_ok(x, self.w3, act, algo) and (out_dtype in (None, torch.float32)):
-            if _products != 3:
-                return _reduced_products(self, x, ops.conv2d, dict(stride=self.stride, pad=self.pad), self.scale, act, residual, out)
             return ops.conv2d(ops.split_pair(x), self.w3, self.scale, self.bias, stride=self.stride, pad=self.pad, act=act, residual=residual, out=out,
                               out_dtype=torch.float32, algo=ops.ALGO_TCGEN05_SPLIT3)
         return ops.conv2d(x, self.w, self.scale, self.bias, stride=self.stride, pad=self.pad, act=act, residual=residual, out=out, out_dtype=out_dtype, algo=algo)
@@ -289,32 +281,8 @@ class _Linear:
             ops._be().add_act(y, None, None, ops.ACT_GELU, y)
             return y
         if _split3_ok(x, self.w3, act, algo) and (out_dtype in (None, torch.float32)):
-            if _products != 3:
-                return _reduced_products(self, x, ops.linear, {}, None, act, residual, out)
             return ops.linear(ops.split_pair(x), self.w3, self.bias, act=act, residual=residual, out_dtype=torch.float32, out=out, algo=ops.ALGO_TCGEN05_SPLIT3)
         return ops.linear(x, self.w, self.bias, act=act, residual=residual, out_dtype=out_dtype, out=out, algo=algo)
-
-
-_reduced_cache = {}
-
-
-def _reduced_products(layer, x, fn, kw, scale, act, residual, out):
-    """fp32_tc layer with fewer than three products (see `_products`); weights derived lazily from the split triple."""
-    C = layer.w3.shape[-1] // 3
-    key = (id(layer.w3), _products)  # the entry keeps w3 alive, so its id cannot be recycled by another layer
-    w = _reduced_cache.get(key, (None, None))[1]
-    if w is None:
-        if _products == 2:
-            w = layer.w3.clone()
-            w[..., C:2 * C] = 0
-        else:
-            w = layer.w3[..., :C].contiguous()
-        _reduced_cache[key] = (layer.w3, w)
-    xp = ops.split_pair(x)
-    pos = (scale, layer.bias) if fn is ops.conv2d else (layer.bias,)
-    if _products == 2:
-        return fn(xp, w, *pos, act=act, residual=residual, out=out, out_dtype=torch.float32, algo=ops.ALGO_TCGEN05_SPLIT3, **kw)
-    return fn(xp[..., :C], w, *pos, act=act, residual=residual, out=out, out_dtype=torch.float32, algo=ops.ALGO_TCGEN05, **kw)
 
 
 def _enable_split3(obj, seen=None, host_w3=None):
@@ -343,7 +311,6 @@ class DetrEngine:
     """Packs a FAIDetr state_dict for one (device, precision) and runs the fused forward."""
 
     _host_w3 = None  # set per instance in fp32_tc mode (see _to)
-    fuse_shortcut_pool = False  # fold the vd shortcut's AvgPool2d into a 2x2/s2 conv (off by default, see _pack_backbone)
 
     def __init__(self, sd: Dict[str, torch.Tensor], cfg: DETRConfig, device, precision: str = "fp16", algo: int = ops.ALGO_AUTO):
         assert precision in ("fp32", "fp16", "fp32_tc")
@@ -354,7 +321,6 @@ class DetrEngine:
         self.d = cfg.transformer_predictor_hidden_dim
         self._consts: Dict[Tuple[int, int], dict] = {}
         self._host_w3 = {} if precision == "fp32_tc" else None  # id(packed device weight) -> [W_hi|W_lo|W_hi] split on the host in _to()
-        self.mix = {"backbone": 3, "encoder": 3, "select": 3, "decoder": 3}  # fp32_tc only: tensor-core products per stage (see `_products`)
         # pack on the HOST (BN folding, re-parameterisation, concatenations are a few hundred tiny tensor ops: as device launches they were ~700 `at::`
         # kernels in front of the first forward); only the packed tensors travel to the device
         sd = {k: v.detach().to("cpu") for k, v in sd.items()}
@@ -423,12 +389,6 @@ class DetrEngine:
                        "c": self._cnl(sd, p + ".branch2c", "relu"), "stride": stride, "short": None}
                 if bi == 0:
                     blk["short"] = self._cnl(sd, p + (".short.conv" if stride == 2 else ".short"), None)
-                    if stride == 2 and self.precision != "fp32" and self.fuse_shortcut_pool:
-                        # AvgPool2d(2,2) followed by a 1x1 conv (resnet.py:91-102) IS a 2x2 stride-2 conv whose four taps are W/4 (an exact
-                        # power-of-two scaling).  Measured (trip 43): 11.39 vs 11.22 ms/step - the four 5-D TMA boxes per K chunk cost more than the
-                        # pooling launch saves - so it is OFF by default (DetrEngine.fuse_shortcut_pool); kept as a tested kernel capability.
-                        c = blk["short"]
-                        blk["short_fused"] = _Conv((c.w * 0.25).expand(-1, 2, 2, -1).contiguous(), c.scale, c.bias, 2, 0, c.act)
                 blocks.append(blk)
             self.stages.append(blocks)
 
@@ -442,13 +402,7 @@ class DetrEngine:
         for blocks in self.stages:
             for blk in blocks:
                 y = blk["b"](blk["a"](x, algo=A), algo=A)
-                if blk["short"] is None:
-                    short = x
-                else:
-                    if "short_fused" in blk and x.shape[1] % 2 == 0 and x.shape[2] % 2 == 0 and (x.is_cuda or ops._backend is not None):
-                        short = blk["short_fused"](x, algo=A)
-                    else:
-                        short = blk["short"](ops.avgpool2x2(x) if blk["stride"] == 2 else x, algo=A)
+                short = x if blk["short"] is None else blk["short"](ops.avgpool2x2(x) if blk["stride"] == 2 else x, algo=A)
                 x = blk["c"](y, residual=short, algo=A)
             feats.append(x)
         return feats
@@ -536,8 +490,6 @@ class DetrEngine:
 
     # ---- pair-native fp32_tc path: conv activations stay in the fp16 [hi | lo] pair format between convs (written by the conv epilogue), so the split kernel
     # only runs where a non-conv operator (LayerNorm, attention, selection) produced fp32 --------------------------------------------------------------
-    pair_native = True  # precision == "fp32_tc" only; False = fp32 storage + one split launch in front of every conv (the round-1 data flow)
-
     def _pc(self, conv, x, residual=None, out=None, out_pair=True, act=None):
         """packed _Conv on a pair-format input (an fp32 tensor is split first) -> Pair, or fp32 tensor with out_pair=False"""
         return ops.conv2d_pair(ops.to_pair(x), conv.w3, conv.scale, conv.bias, stride=conv.stride, pad=conv.pad, act=conv.act if act is None else act,
@@ -562,8 +514,6 @@ class DetrEngine:
 
     # fused row glue (csrc/head_fused.cu): LayerNorm / positional add / GELU / gather / mask kernels write the pair operand of the next tensor-core linear themselves
     # (and attention / deformable attention write pair rows), so no split_f32_pair / add / row_select launch remains in the AIFI, selection and decoder chains
-    fused_glue = True
-
     def _aifi_pair(self, src, pos):
         """AIFI encoder layer (nn/layers/transformer.py:583-601, post-norm, GELU) on fp32 tokens [B,L,d] -> (fp32 tokens, their Pair)"""
         blk, d = self.aifi, src.shape[-1]
@@ -590,9 +540,8 @@ class DetrEngine:
         return x
 
     def pair_capable(self) -> bool:
-        """the pair-native fp32_tc data flow is available (three products in every stage, default algorithm choice, a tensor-core (sm_90) device or the CPU test backend)"""
-        return (self.precision == "fp32_tc" and self.pair_native and self.algo == ops.ALGO_AUTO and all(v == 3 for v in getattr(self, "mix", {}).values())
-                and (ops._backend is not None or ops.supports_tcgen05_cached()))
+        """the pair-native fp32_tc data flow is available (default algorithm choice, a tensor-core (sm_90) device or the CPU test backend)"""
+        return self.precision == "fp32_tc" and self.algo == ops.ALGO_AUTO and (ops._backend is not None or ops.supports_tcgen05_cached())
 
     def _run_backbone_pair(self, images):
         """ResNet-vd in the pair format -> [res2, res3, res4, res5] as Pairs (nn/backbone/resnet.py:252-266); shared by every model family with this backbone"""
@@ -626,16 +575,9 @@ class DetrEngine:
         self._pc(self.enc_in[0], res3, out=cat2.slice(C, 2 * C))
         self._pc(self.enc_in[1], res4, out=cat1.slice(C, 2 * C))
         p5 = self._pc(self.enc_in[2], res5, out_pair=False)          # fp32 tokens for the AIFI block (LayerNorm / attention work on fp32)
-        src = p5.reshape(B, h32 * w32, C)
-        if self.fused_glue:
-            src, src_p = self._aifi_pair(src, K["pos"])
-            p5 = src.reshape(B, h32, w32, C)
-            lat0 = self._pc(self.lateral[0], P(src_p.buf.reshape(B, h32, w32, 2 * C)), out=cat4.slice(C, 2 * C))
-        else:
-            src = self._mha(self.aifi, src, K["pos"])
-            src = self._ffn(self.aifi, src, ops.ACT_GELU)
-            p5 = src.reshape(B, h32, w32, C)
-            lat0 = self._pc(self.lateral[0], p5, out=cat4.slice(C, 2 * C))
+        src, src_p = self._aifi_pair(p5.reshape(B, h32 * w32, C), K["pos"])
+        p5 = src.reshape(B, h32, w32, C)
+        lat0 = self._pc(self.lateral[0], P(src_p.buf.reshape(B, h32, w32, 2 * C)), out=cat4.slice(C, 2 * C))
         ops.pair_resize_bilinear(lat0, (h32 * 2, w32 * 2), out=cat1.slice(0, C))
         fpn0 = self._csp_run_pair(self.fpn[0], cat1)
         lat1 = self._pc(self.lateral[1], fpn0, out=cat3.slice(C, 2 * C))
@@ -672,21 +614,12 @@ class DetrEngine:
             # the reference's torch graph takes any size (odd feature maps from ceil-mode pools / stride-2 convs); the kernels tile the stride-2 layers on even
             # maps, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
             raise ValueError(f"focoos_b200: input size {H}x{W} is not a multiple of 32; resize/pad the image (e.g. ModelInfo.im_size) before the model")
-        global _products
-        use_pair = self.pair_capable()
-        if use_pair:
+        if self.pair_capable():
             mem_pair, shapes, K = self._forward_pair_trunk(images, taps)
-            dev = images.device
-            S, d = mem_pair.buf.shape[1], self.d
             value_all = self._plin(self.value_all, mem_pair)
             t = self._plin(self.enc_output, mem_pair)
-            memory = None
-            if self.fused_glue:
-                return self._forward_head_pair(t, value_all, shapes, K, B, S, taps, mem_pair)
-            return self._forward_head(t, value_all, memory, shapes, K, B, S, taps, mem_pair)
-        _products = self.mix["backbone"]
+            return self._forward_head_pair(t, value_all, shapes, K, B, mem_pair.buf.shape[1], taps, mem_pair)
         feats = self._run_backbone(images)
-        _products = self.mix["encoder"]
         res3, res4, res5 = feats[1], feats[2], feats[3]
         h32, w32 = res5.shape[1], res5.shape[2]
         K = self._constants(h32, w32)
@@ -723,7 +656,6 @@ class DetrEngine:
         shapes = K["shapes"]
         S = sum(h * w for h, w in shapes)
         d = self.d
-        _products = self.mix["select"]
         memory = torch.empty((B, S, d), dtype=dt, device=dev)
         start = 0
         for i, (f, (h, w)) in enumerate(zip(enc_outs, shapes)):
@@ -732,20 +664,16 @@ class DetrEngine:
         value_all = self.value_all(memory, algo=A)  # [B,S,6*d], layer i uses columns [i*d,(i+1)*d)
         # query selection (modelling.py:1191-1232)
         t = self.enc_output(memory, algo=A)
-        return self._forward_head(t, value_all, memory, shapes, K, B, S, taps, None)
+        return self._forward_head(t, value_all, memory, shapes, K, B, S, taps)
 
-    def _forward_head(self, t, value_all, memory, shapes, K, B, S, taps, mem_pair):
-        """query selection + decoder + head on the encoder memory (shared by the fp16 / fp32 / pair-native trunks)"""
-        global _products
+    def _forward_head(self, t, value_all, memory, shapes, K, B, S, taps):
+        """query selection + decoder + head on the encoder memory (every flow but the pair-native fp32_tc one, which runs _forward_head_pair)"""
         cfg, dt, A, d = self.cfg, self.dt, self.algo, self.d
         dev = t.device
         t = ops.row_select(t, K["valid"], self.enc_output.bias)
         output_memory = ops.layernorm(t, *self.enc_output_ln)
         ncls = cfg.num_classes
-        if mem_pair is not None and self.enc_score.w3 is not None:
-            # fp32-accurate row maxima straight from the tensor-core epilogue: the [B,S,365] fp32 logits (393 MB at bs=32) are never written
-            scores = ops.linear_rowmax_pair(ops.to_pair(output_memory), self.enc_score.w3, self.enc_score.bias)
-        elif self.precision == "fp16" and A == ops.ALGO_AUTO and ops.supports_tcgen05_cached():
+        if self.precision == "fp16" and A == ops.ALGO_AUTO and ops.supports_tcgen05_cached():
             # only the per-anchor maximum is ever used in eval (modelling.py:1210-1214): the [B,S,365] fp32 logits (395 MB at bs=32) are never materialised
             scores = ops.linear_rowmax(output_memory, self.enc_score.w, self.enc_score.bias)
         else:
@@ -758,9 +686,8 @@ class DetrEngine:
         ref_unact = ops.box_add_anchors(bb, K["anchors"], topk_ind)
         ref = ops.box_sigmoid(ref_unact)
         if taps is not None:
-            taps.update(memory=memory if mem_pair is None else mem_pair.float(), enc_scores=scores, topk_ind=topk_ind, target=tgt, ref_unact=ref_unact)
+            taps.update(memory=memory, enc_scores=scores, topk_ind=topk_ind, target=tgt, ref_unact=ref_unact)
         # decoder (modelling.py:969-1020, eval: logits only from the last layer)
-        _products = self.mix["decoder"]
         for i, blk in enumerate(self.dec):
             pos = self.qpos[1](self.qpos[0](ref, act=ops.ACT_RELU, out_dtype=dt, algo=ops.ALGO_SIMT), algo=A)
             tgt = self._mha(blk, tgt, pos)
@@ -776,7 +703,6 @@ class DetrEngine:
         logits = self.dec_score(tgt, out_dtype=torch.float32, algo=ops.ALGO_SIMT)  # [B,Q,C] contiguous
         if taps is not None:
             taps.update(pred_logits=logits, pred_boxes_cxcywh=ref)
-        _products = 3
         return ops.box_sigmoid(logits), ops.box_cxcywh_to_xyxy(ref)
 
 

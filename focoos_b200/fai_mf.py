@@ -279,11 +279,12 @@ class MFEngine(DetrEngine):
             self._consts[key] = self._to(position_embedding_sine_normalized(h, w, self.d // 2))
         return self._consts[key]
 
-    def _heads(self, out, mask_features, size, want_class):
-        """PredictionHeads.forward (:69-112) -> (class logits fp32 or None, mask logits NHWC [B,h4,w4,Qp], (mask, allowed) or None)."""
+    def _heads(self, out, mask_features, mf_pair, fused, size, want_class):
+        """PredictionHeads.forward (:69-112) -> (class logits fp32 or None, mask logits NHWC [B,h4,w4,Qp], (mask, allowed) or None).
+        mf_pair: mask_features as fp16 [hi | lo] planes (fp32_tc) or None; fused: the fused row glue of the fp32_tc decoder (see _run_decoder)."""
         A, dt = self.algo, self.dt
         B, Q, d = out.shape
-        if getattr(self, "_fused_glue", False):  # fp32_tc: LayerNorm writes the pair operand of the mask MLP, whose hidden layers stay in the pair format
+        if fused:  # fp32_tc: LayerNorm writes the pair operand of the mask MLP, whose hidden layers stay in the pair format
             dn, dnp, _ = ops.layernorm_ex(out, *self.head_norm, want_f32=want_class)
             cls = self.classifier(dn, out_dtype=torch.float32, algo=ops.ALGO_SIMT) if want_class else None
             me = self._plin(self.mask_mlp[2], self._plin(self.mask_mlp[1], self._plin(self.mask_mlp[0], dnp, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True))
@@ -295,11 +296,10 @@ class MFEngine(DetrEngine):
         Qp = (Q + 7) // 8 * 8
         masks = torch.zeros((B, h4, w4, Qp), dtype=dt, device=out.device)
         # einsum("bqc,bchw->bqhw"): a [h4*w4, C] x [C, Q] GEMM per image whose "weights" (the mask embeddings) differ per image - ONE launch
-        mfp = getattr(self, "_mf_pair", None)
-        if mfp is not None and mfp[0] is mask_features:
+        if mf_pair is not None:
             # fp32_tc: the same GEMM as three fp16 tensor-core products - mask_features split ONCE per forward (_run_decoder), the per-image embeddings as
             # [W_hi | W_lo | W_hi] triples.  (On the CUDA-core fp32 kernel this product was a third of the parity-mode step: 16.9 of 50.4 ms at bs=16 800x800.)
-            ops.conv2d_per_image(mfp[1], _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=masks[..., :Q], algo=ops.ALGO_TCGEN05_SPLIT3)
+            ops.conv2d_per_image(mf_pair, _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=masks[..., :Q], algo=ops.ALGO_TCGEN05_SPLIT3)
         else:
             ops.conv2d_per_image(mask_features, me.reshape(B, Q, 1, 1, C), out=masks[..., :Q], algo=A)
         attn = None
@@ -366,12 +366,12 @@ class MFEngine(DetrEngine):
         d, nh = self.d, self.nhead
         scale = 1.0 / math.sqrt(d // nh)
         nl = len(ms)
-        self._mf_pair = None
+        mf_pair = None
         if isinstance(mask_features, ops.Pair):  # written as a pair by its conv (MFEngine.forward)
-            self._mf_pair = (mask_features, mask_features.buf)
+            mf_pair = mask_features.buf
         elif (self.precision == "fp32_tc" and A == ops.ALGO_AUTO and mask_features.dtype == torch.float32 and mask_features.shape[-1] % 64 == 0
                 and (ops._backend is not None or ops.supports_tcgen05_cached())):
-            self._mf_pair = (mask_features, ops.split_pair(mask_features))  # consumed by every _heads call of this forward
+            mf_pair = ops.split_pair(mask_features)  # consumed by every _heads call of this forward
         srcs, kpos, sizes = [], [], []
         for i in range(nl):
             hh, ww = ms[i].shape[1], ms[i].shape[2]
@@ -391,13 +391,13 @@ class MFEngine(DetrEngine):
         # fused row glue (csrc/head_fused.cu, the kernels of the fai-detr head): every LayerNorm writes the pair operand(s) of the linears behind it - LN(x) and
         # LN(x) + query_pos in one launch - and the FFN / mask-MLP hidden layers stay in the pair format: no add / split launches between two tensor-core linears
         lins = [b_[k] for b_ in self.dec for k in ("cq", "cout", "sqk", "sv", "sout", "l1", "l2")] + list(self.mask_mlp)
-        self._fused_glue = bool(pair_kv and self.fused_glue and all(getattr(l_, "w3", None) is not None for l_ in lins))
-        _, masks, attn = self._heads(out, mask_features, sizes[0], False)
+        fused = bool(pair_kv and all(getattr(l_, "w3", None) is not None for l_ in lins))
+        _, masks, attn = self._heads(out, mask_features, mf_pair, fused, sizes[0], False)
         L = len(self.dec)
         cls = None
         for i, blk in enumerate(self.dec):
             lvl = i % nl
-            if self._fused_glue:
+            if fused:
                 _, _, tq = ops.layernorm_ex(out, *blk["cn"], pos=qpos, want_f32=False, want_pair=False, want_pair_pos=True)
                 q = self._plin(blk["cq"], tq)
                 kk, vv = self._plin(blk["ck"], kpos_p[lvl], out_pair=True), self._plin(blk["cv"], srcs_p[lvl], out_pair=True)
@@ -410,7 +410,7 @@ class MFEngine(DetrEngine):
                 _, t2p, _ = ops.layernorm_ex(out, *blk["fn"], want_f32=False)
                 out = self._plin(blk["l2"], self._plin(blk["l1"], t2p, act=ops.ACT_RELU, out_pair=True), residual=out)
                 last = i == L - 1
-                cls, masks, attn = self._heads(out, mask_features, None if last else sizes[(i + 1) % nl], last)
+                cls, masks, attn = self._heads(out, mask_features, mf_pair, fused, None if last else sizes[(i + 1) % nl], last)
                 if taps is not None:
                     taps[f"dec{i}_out"] = out
                 continue
@@ -429,14 +429,13 @@ class MFEngine(DetrEngine):
             t2 = ops.layernorm(out, *blk["fn"])
             out = blk["l2"](blk["l1"](t2, act=ops.ACT_RELU, algo=A), residual=out, algo=A)
             last = i == L - 1
-            cls, masks, attn = self._heads(out, mask_features, None if last else sizes[(i + 1) % nl], last)
+            cls, masks, attn = self._heads(out, mask_features, mf_pair, fused, None if last else sizes[(i + 1) % nl], last)
             if taps is not None:
                 taps[f"dec{i}_out"] = out
         if taps is not None:
             taps.update(pred_logits=cls, pred_masks=masks)  # masks: NHWC [B,h4,w4,Qp] pre-sigmoid logits
         probs = ops.softmax_drop_last(cls)
         lazy = LazyMasks(masks, Q, (H, W))
-        self._mf_pair, self._fused_glue = None, False
         return probs, (lazy if self.lazy_masks else lazy.materialize())
 
 

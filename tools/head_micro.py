@@ -1,7 +1,7 @@
 """In-graph timing of the two halves of the fp32_tc DETR forward (trunk = backbone + hybrid encoder + decoder input projection; head = value / enc_output
-projections + query selection + 6 decoder layers + score head), each captured in its own CUDA graph, with the fused row glue on and off.
-    python tools/head_micro.py          # trunk / head split, fused_glue on / off
-    python tools/head_micro.py attn     # the split-precision attention kernel alone (decoder 300x300 and AIFI 400x400 shapes), env FB200_ATTN_QB
+projections + query selection + 6 decoder layers + score head), each captured in its own CUDA graph.
+    python tools/head_micro.py          # trunk / head split
+    python tools/head_micro.py attn     # the split-precision attention kernel alone (decoder 300x300 and AIFI 400x400 shapes)
 """
 import math
 import os
@@ -42,7 +42,7 @@ if "attn" in sys.argv:
         qk = torch.randn((B, L, 512), device=dev)
         v = torch.randn((B, L, 256), device=dev)
         f = lambda: ops.attention(qk[..., :256], qk[..., 256:], v, 8, 1.0 / math.sqrt(32), split=True, out_pair=True)
-        print(f"attention_split B={B} L={L}: {time_graph(f, 50) * 1e3:8.1f} us  (FB200_ATTN_QB={os.environ.get('FB200_ATTN_QB', 'default')})")
+        print(f"attention_split B={B} L={L}: {time_graph(f, 50) * 1e3:8.1f} us")
     sys.exit(0)
 
 B = 32
@@ -53,28 +53,23 @@ eng = model.engine()
 x = torch.from_numpy(np.random.default_rng(1).integers(0, 256, (B, 640, 640, 3), dtype=np.uint8)).to(dev)
 
 with torch.no_grad():
-    for fused in (True, False):
-        eng.fused_glue = fused
-        state = {}
+    state = {}
 
-        def trunk():
-            state["mem"], state["shapes"], state["K"] = eng._forward_pair_trunk(x, None)
+    def trunk():
+        state["mem"], state["shapes"], state["K"] = eng._forward_pair_trunk(x, None)
 
-        def head():
-            mem, shapes, K = state["mem"], state["shapes"], state["K"]
-            S = mem.buf.shape[1]
-            value_all = eng._plin(eng.value_all, mem)
-            t = eng._plin(eng.enc_output, mem)
-            if fused:
-                return eng._forward_head_pair(t, value_all, shapes, K, B, S, None, mem)
-            return eng._forward_head(t, value_all, None, shapes, K, B, S, None, mem)
+    def head():
+        mem, shapes, K = state["mem"], state["shapes"], state["K"]
+        value_all = eng._plin(eng.value_all, mem)
+        t = eng._plin(eng.enc_output, mem)
+        return eng._forward_head_pair(t, value_all, shapes, K, B, mem.buf.shape[1], None, mem)
 
-        l0 = ops.launch_count()
-        trunk()
-        l1 = ops.launch_count()
-        head()
-        l2 = ops.launch_count()
-        t_tr = time_graph(trunk)
-        t_hd = time_graph(head)
-        t_all = time_graph(lambda: model(x))
-        print(f"fused_glue={fused}: trunk {t_tr:7.3f} ms ({l1 - l0} launches)  head {t_hd:7.3f} ms ({l2 - l1} launches)  whole forward {t_all:7.3f} ms")
+    l0 = ops.launch_count()
+    trunk()
+    l1 = ops.launch_count()
+    head()
+    l2 = ops.launch_count()
+    t_tr = time_graph(trunk)
+    t_hd = time_graph(head)
+    t_all = time_graph(lambda: model(x))
+    print(f"trunk {t_tr:7.3f} ms ({l1 - l0} launches)  head {t_hd:7.3f} ms ({l2 - l1} launches)  whole forward {t_all:7.3f} ms")
