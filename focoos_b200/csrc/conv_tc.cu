@@ -108,13 +108,6 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap* map, uint64_t* ba
   asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
                ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
 }
-// L2 prefetch of a box (no smem, no barrier): keeps the DRAM latency of the NEXT tile off the critical path
-__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global [%0, {%1, %2, %3, %4}];" ::"l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_5d(const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.prefetch.tensor.5d.L2.global [%0, {%1, %2, %3, %4, %5}];" ::"l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
                ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
@@ -246,21 +239,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     uint32_t phase = 0;
     for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
       const TileXY tc = tile_of(t);
-      {  // L2 prefetch for the tile this CTA will process next (one box per channel chunk; taps overlap)
-        const int tn = t + gridDim.x;
-        if (tn < p.total_tiles && (tn / p.n_tiles) != (t / p.n_tiles)) {
-          const TileXY tnx = tile_of(tn);
-          const int nchunks = FS ? 2 * p.cchunks : p.cchunks;
-          for (int cc = 0; cc < nchunks; ++cc) {
-            const int a_c0 = FS ? (cc < p.cchunks ? cc * BLOCK_K : p.lo_off + (cc - p.cchunks) * BLOCK_K) : a_chan(cc);
-            if (!p.stride2) tma_prefetch_4d(&tmap_a, a_c0, tnx.w0, tnx.h0, tnx.img);
-            else {
-              for (int par = 0; par < 4; ++par)  // the four (h, w) parities of the 2x2 input cell
-                tma_prefetch_5d(&tmap_a, (par & 1) * p.x_pitch + a_c0, tnx.w0, par >> 1, tnx.h0, tnx.img);
-            }
-          }
-        }
-      }
+      // No L2 prefetch of the next tile's A: every CTA of the persistent grid would pull a whole tile ahead (256 KiB of A for a 512-channel pair input),
+      // about as much again as the tiles in flight, into the 50 MB L2.  On H100 that made the HBM-bound 1x1 convs slower (1x1 512->128 @80^2: 0.27 ms without, 0.34 with).
       for (int kb = 0; kb < p.num_k_blocks; ++kb) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
         const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
