@@ -305,10 +305,7 @@ class BisenetEngine(MFEngine):
         else:
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
-        if H % 32 or W % 32:
-            # the reference's torch graph takes any size (odd feature maps from ceil-mode pools / stride-2 convs); the kernels tile the stride-2 layers on even
-            # maps, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
-            raise ValueError(f"focoos_b200: input size {H}x{W} is not a multiple of 32; resize/pad the image (e.g. ModelInfo.im_size) before the model")
+        # any H x W, like the reference (its processor does not resize): odd maps from the stride-2 convs and pools run on the same kernels
         x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, dt)
         x = self.stem2(x, algo=A)  # res2
         feats = []

@@ -8,8 +8,11 @@
 //   warp-group 0   TMA producer (one thread).  A is never materialised as im2col: an M-tile is a BW x BH rectangle of output
 //                  pixels of one image, and the A block for filter tap (kh,kw), channel chunk c0 is the SAME rectangle of the
 //                  NHWC input shifted by (kh-pad, kw-pad) — one 4-D tiled TMA load whose out-of-bounds rows/columns (the conv zero
-//                  padding, and ragged tile edges) are zero-filled by the TMA unit.  Stride-2 convs use a 5-D view
-//                  (c', w/2, h&1, h/2, b) of the same tensor so that every tap is again a dense box.  1x1 convs and linears are the
+//                  padding, and ragged tile edges) are zero-filled by the TMA unit.  Stride-2 convs on even maps use a 5-D view
+//                  (c', w/2, h&1, h/2, b) of the same tensor so that every tap is again a dense box.  That view cannot describe an odd
+//                  H or W, so 3x3 stride-2 convs on odd maps use the 4-D (c, w, h, b) view with traversal strides {1, 2, 2, 1}: tap
+//                  (kh,kw) is the box at (2*w0 + kw - pad, 2*h0 + kh - pad) taking every other pixel, zero-filled against the true
+//                  W x H, and it lands as the same dense smem tile.  1x1 convs and linears are the
 //                  degenerate W = M, H = 1 case.  Smem tiles land in the canonical K-major SWIZZLE_128B (or _64B for 32-channel
 //                  chunks) layout wgmma reads through its shared-memory descriptors.  After a tile's last k-block the producer loads
 //                  the tile's residual (if any) into the next ring entries, so it is in flight while the consumers finish the previous tile.
@@ -54,7 +57,7 @@ struct KParams {
   int BW, BH, tiles_w, tiles_h;    // output tile rectangle and tile counts per image
   int Ho, Wo;                      // output spatial size (validity of rows)
   int x_pitch;                     // stride-2 view only (c' = wp * pitch + c)
-  int stride2;                     // 0: 4-D stride-1 view, 1: 5-D stride-2 view
+  int stride2;                     // 0: 4-D stride-1 view, 1: 5-D stride-2 view (even maps), 2: 4-D view with traversal stride 2 (odd maps)
   int num_k_blocks;
   int n_tiles, total_tiles;        // N tiles per M tile; total = m_tiles * n_tiles
   float* rowmax;                   // not null: row-max-only epilogue (query selection scores), nothing is stored
@@ -225,6 +228,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     auto load_a = [&](uint64_t* bar, void* dst, int c, int kh, int kw, int h0, int w0, int img) {
       if (!p.stride2) {
         tma_load_4d(&tmap_a, bar, dst, c, w0 + kw - p.pad, h0 + kh - p.pad, img);
+      } else if (p.stride2 == 2) {  // every other pixel of a 2BW x 2BH box from the tap's first input pixel
+        tma_load_4d(&tmap_a, bar, dst, c, 2 * w0 + kw - p.pad, 2 * h0 + kh - p.pad, img);
       } else {
         // input h = 2*ho + kh - pad -> (h>>1, h&1).  3x3/pad 1: kh=0 -> (ho-1,1); 1 -> (ho,0); 2 -> (ho,1).  2x2/pad 0: kh -> (ho,kh)
         const int th = kh - p.pad, tw = kw - p.pad;  // arithmetic shift: -1 -> (-1, 1)
@@ -462,12 +467,14 @@ static EncodeTiledFn get_encode() {
 }
 
 static int encode(CUtensorMap* m, CUtensorMapDataType dt, int elt, int rank, void* base, const uint64_t* dims, const uint64_t* strides_elts,
-                  const uint32_t* box, const char* what, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+                  const uint32_t* box, const char* what, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B,
+                  const uint32_t* elem_strides = nullptr) {
+  // elem_strides (null = all 1): traversal stride per dimension; a load then takes ceil(box[i] / elem_strides[i]) elements along dimension i
   EncodeTiledFn fn = get_encode();
   if (!fn) { set_error("conv_tc: cuTensorMapEncodeTiled unavailable"); return FB200_ERR_CUDA; }
   cuuint64_t gdim[5], gstr[4];
   cuuint32_t bdim[5], estr[5];
-  for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bdim[i] = box[i]; estr[i] = 1; }
+  for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bdim[i] = box[i]; estr[i] = elem_strides ? elem_strides[i] : 1; }
   for (int i = 1; i < rank; ++i) gstr[i - 1] = strides_elts[i] * (uint64_t)elt;  // bytes; dim0 stride is implicit
   CUresult r = fn(m, dt, (cuuint32_t)rank, base, gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -549,7 +556,10 @@ bool conv2d_tc_supported(const ConvParams& p, int x_dtype, int out_dtype) {
   if ((p.act & 15) == FB200_ACT_SIGMOID) return false;  // gates are [B, C] vectors: SIMT path
   if ((p.out_bs * oelt) % 16 != 0) return false;
   if (p.stride == 1) return (2 * p.pad == p.KH - 1) || (p.KH == 1 && p.pad == 0);
-  if (p.stride == 2) return ((p.KH == 3 && p.pad == 1) || (p.KH == 2 && p.pad == 0)) && p.H % 2 == 0 && p.W % 2 == 0;
+  if (p.stride == 2) {
+    if (p.KH == 3 && p.pad == 1) return true;  // even maps: the 5-D parity view; odd H or W: the strided 4-D view (one box <= 256 per dimension: 2 * BW, 2 * BH)
+    return p.KH == 2 && p.pad == 0 && p.H % 2 == 0 && p.W % 2 == 0;
+  }
   return false;
 }
 
@@ -565,7 +575,7 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   kp.w_seg = Clog;
   const CUtensorMapSwizzle swz = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   kp.cchunks = p.Cin / BK; kp.x_pitch = p.x_pitch;
-  kp.stride2 = (p.stride == 2) ? 1 : 0;
+  kp.stride2 = (p.stride != 2) ? 0 : (p.H % 2 == 0 && p.W % 2 == 0) ? 1 : 2;
   kp.num_k_blocks = p.KH * p.KW * kp.cchunks;
   // geometry: 1x1 stride-1 convs and linears flatten to W = M, H = 1, B = 1
   int B = p.B, H = p.H, W = p.W, Ho = p.Ho, Wo = p.Wo;
@@ -589,6 +599,14 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
     const uint64_t str[4] = {1, P, P * W, P * W * H};
     const uint32_t box[4] = {(uint32_t)BK, (uint32_t)BW, (uint32_t)BH, 1};
     rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "A", swz);
+  } else if (kp.stride2 == 2) {
+    // odd H or W: the true (c, w, h, b) geometry, every other pixel of a 2BW x 2BH box.  The last tile's box runs one row / column past the
+    // map, which the TMA unit zero-fills like the conv padding.  choose_tile keeps BW, BH <= 128, so the box stays within 256.
+    const uint64_t dims[4] = {(uint64_t)(p.split3 ? kp.lo_off + Clog : p.Cin), (uint64_t)W, (uint64_t)H, (uint64_t)B};
+    const uint64_t str[4] = {1, P, P * W, P * W * H};
+    const uint32_t box[4] = {(uint32_t)BK, 2 * (uint32_t)BW, 2 * (uint32_t)BH, 1};
+    const uint32_t estr[4] = {1, 2, 2, 1};
+    rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "A(s2 odd)", swz, estr);
   } else {
     const uint64_t dims[5] = {2 * P, (uint64_t)W / 2, 2, (uint64_t)H / 2, (uint64_t)B};
     const uint64_t str[5] = {1, 2 * P, P * W, 2 * P * W, P * W * H};

@@ -611,8 +611,8 @@ class DetrEngine:
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
         if H % 32 or W % 32:
-            # the reference's torch graph takes any size (odd feature maps from ceil-mode pools / stride-2 convs); the kernels tile the stride-2 layers on even
-            # maps, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
+            # DETRProcessor resizes to im_size; the encoder buffers, anchors and positional constants are laid out for 1/8 and 1/16 maps of exactly 4x and
+            # 2x the 1/32 map, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
             raise ValueError(f"focoos_b200: input size {H}x{W} is not a multiple of 32; resize/pad the image (e.g. ModelInfo.im_size) before the model")
         if self.pair_capable():
             mem_pair, shapes, K = self._forward_pair_trunk(images, taps)

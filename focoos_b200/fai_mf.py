@@ -316,10 +316,7 @@ class MFEngine(DetrEngine):
         else:
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
-        if H % 32 or W % 32:
-            # the reference's torch graph takes any size (odd feature maps from ceil-mode pools / stride-2 convs); the kernels tile the stride-2 layers on even
-            # maps, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
-            raise ValueError(f"focoos_b200: input size {H}x{W} is not a multiple of 32; resize/pad the image (e.g. ModelInfo.im_size) before the model")
+        # any H x W, like the reference (its processor does not resize): odd maps from the stride-2 convs and ceil-mode pools run on the same kernels
         pair = self.pair_capable() and all(getattr(c, "w3", None) is not None for c in [self.pd_in] + [self.adapter[i] for i in (1, 2, 3)])
         if pair:
             # fp32_tc: the backbone keeps its activations as fp16 [hi | lo] planes between convs (no split pass in front of every conv, DetrEngine._run_backbone_pair);
