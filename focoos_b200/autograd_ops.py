@@ -25,16 +25,10 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import ops
+from .fai_detr import _split3_weights
 
 
 # ---- conv through either fp32 engine ----------------------------------------------------------------------------------
-def _split3_weights(w):
-    """[Cout,KH,KW,C] fp32 -> [Cout,KH,KW,3C] fp16 = [W_hi | W_lo | W_hi] (operand layout of ALGO_TCGEN05_SPLIT3)."""
-    hi = w.half()
-    lo = (w - hi.float()).half()
-    return torch.cat([hi, lo, hi], dim=-1).contiguous()
-
-
 def _to_half_contiguous(t):
     """fp16, contiguous copy of a (possibly permuted) fp32 view in ONE copy kernel (cast + layout change) - `.contiguous().half()` is two"""
     return torch.empty(t.shape, dtype=torch.float16, device=t.device).copy_(t)

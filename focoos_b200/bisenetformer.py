@@ -16,14 +16,14 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field, fields
-from typing import Dict, List, Optional
+from typing import List, Optional
 
 import torch
 import torch.nn as nn
 
 from . import ops
-from .fai_detr import _bn_fold, _Conv, _CriterionStub, _Linear
-from .fai_mf import MaskFormerModelOutput, MFEngine, PredictionHeads, _AttnLayer, _ConvBN, _FFNLayer
+from .fai_detr import _bn_fold, _Conv, _CriterionStub, _packed_layers
+from .fai_mf import MaskFormerModelOutput, MFEngine, PredictionHeads, _AttnLayer, _ConvBN, _FFNLayer, _SegmentationModel
 from .ports import ModelOutput
 
 
@@ -186,16 +186,9 @@ class BisenetFormerHead(nn.Module):
 
 
 class BisenetEngine(MFEngine):
-    def __init__(self, sd: Dict[str, torch.Tensor], cfg: BisenetFormerConfig, device, precision: str = "fp16", algo: int = ops.ALGO_AUTO):
-        self.cfg, self.device, self.precision, self.algo = cfg, torch.device(device), precision, algo
-        assert precision in ("fp32", "fp16", "fp32_tc")
-        self.dt = torch.float16 if precision == "fp16" else torch.float32
-        self._host_w3 = {} if precision == "fp32_tc" else None  # fp32 storage, three fp16 tensor-core products per conv / linear (fai_detr._split3_weights)
+    def _pack(self, sd):
+        cfg = self.cfg
         self.nhead, self.d = 8, cfg.transformer_predictor_hidden_dim
-        self._consts = {}
-        # pack on the HOST (BN folding, re-parameterisation, concatenations are a few hundred tiny tensor ops: as device launches they were ~700 `at::`
-        # kernels in front of the first forward); only the packed tensors travel to the device
-        sd = {k: v.detach().to("cpu") for k, v in sd.items()}
         bb = "pixel_decoder.backbone.features"
         w = sd[bb + ".0.conv.weight"].float()
         s, b = _bn_fold(sd, bb + ".0.bn")
@@ -233,7 +226,10 @@ class BisenetEngine(MFEngine):
         self.ffm_c2 = _Conv(self._to(sd[ffm + ".conv2.weight"].float().permute(0, 2, 3, 1)), None, None, 1, 0, ops.ACT_SIGMOID)
         self.conv_out = self._convx(sd, "pixel_decoder.conv_out", 1)
         self._pack_decoder(sd, 2)
-        self._finish_pack()
+
+    def _pair_layers(self):
+        """the decoder linears (whether an STDC block runs in the pair format depends on its shapes: _pair_block_ok)"""
+        return list(_packed_layers([self.dec, self.mask_mlp]))
 
     def _convx(self, sd, p, stride):
         w = sd[p + ".conv.weight"].float()
@@ -287,7 +283,7 @@ class BisenetEngine(MFEngine):
 
     def _pair_block_ok(self, blk, H, W) -> bool:
         """conv2d_pair takes the block: every conv has its weight triple; a 32-channel 3x3 input needs the halo mode (rows of at least 64 pixels, Cout <= 64)"""
-        if blk["stride"] != 1 or not self.pair_capable():
+        if blk["stride"] != 1 or self.precision != "fp32_tc":
             return False
         for cv in blk["convs"]:
             cin, cout, k = cv.w.shape[3], cv.w.shape[0], cv.w.shape[1]
@@ -343,52 +339,17 @@ class BisenetEngine(MFEngine):
         return self._run_decoder([f32, f16], mask_features, B, H, W, taps)
 
 
-class BisenetFormer(nn.Module):
+class BisenetFormer(_SegmentationModel):
     """Drop-in for the reference `BisenetFormer(BaseModelNN)` (bisenetformer/modelling.py:534)."""
 
-    lazy_masks = False  # True: forward() returns fai_mf.LazyMasks (low-resolution logits) instead of the upsampled [B,Q,H,W] probabilities
+    engine_cls = BisenetEngine
 
     def __init__(self, config: BisenetFormerConfig, precision: str = "fp16"):
-        super().__init__()
-        self.config = c = config
+        super().__init__(config, precision)
+        c = config
         self.pixel_decoder = BiseNet(STDC(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim)
         self.head = BisenetFormerHead(TransformerDecoder(c.pixel_decoder_out_dim, c.transformer_predictor_out_dim, c.num_classes, c.transformer_predictor_hidden_dim,
                                                          c.num_queries, 8, c.transformer_predictor_dim_feedforward, c.transformer_predictor_dec_layers), c.num_classes)
         self.register_buffer("pixel_mean", torch.tensor(c.pixel_mean, dtype=torch.float32).view(-1, 1, 1), False)
         self.register_buffer("pixel_std", torch.tensor(c.pixel_std, dtype=torch.float32).view(-1, 1, 1), False)
-        self.num_classes, self.precision, self.algo, self._engine = c.num_classes, precision, ops.ALGO_AUTO, None
         self.eval()
-
-    device = property(lambda self: self.pixel_mean.device)
-    dtype = property(lambda self: self.pixel_mean.dtype)
-
-    def load_state_dict(self, state_dict, strict: bool = False, assign: bool = False):
-        if "model" in state_dict and isinstance(state_dict["model"], dict):
-            state_dict = state_dict["model"]
-        own = self.state_dict()
-        filtered = {k: v for k, v in state_dict.items() if k in own and tuple(own[k].shape) == tuple(v.shape)}
-        res = super().load_state_dict(filtered, strict=False)
-        self._engine = None
-        if strict and (res.missing_keys or len(filtered) != len(state_dict)):
-            raise RuntimeError(f"load_state_dict(strict): missing {res.missing_keys[:5]} / dropped {len(state_dict) - len(filtered)}")
-        return res
-
-    def _apply(self, fn, *a, **k):
-        self._engine = None
-        return super()._apply(fn, *a, **k)
-
-    def engine(self) -> BisenetEngine:
-        e = self._engine
-        if e is None or e.device != self.device or e.precision != self.precision or e.algo != self.algo:
-            self._engine = BisenetEngine(self.state_dict(), self.config, self.device, self.precision, self.algo)
-        return self._engine
-
-    def forward(self, images: torch.Tensor, targets: list = [], taps: Optional[dict] = None) -> MaskFormerModelOutput:
-        if self.training or (targets is not None and len(targets) > 0):
-            raise NotImplementedError("focoos_b200: losses / fine-tuning are not part of the inference hot path")
-        if ops._backend is None and not images.is_cuda:
-            raise RuntimeError("focoos_b200.BisenetFormer runs on CUDA (sm_90a) only — no CPU fallback")
-        eng = self.engine()
-        eng.lazy_masks = bool(getattr(self, "lazy_masks", False))
-        probs, masks = eng.forward(images if images.dtype == torch.uint8 else images.to(torch.float32), taps)
-        return MaskFormerModelOutput(masks=masks, logits=probs, loss=None)

@@ -406,12 +406,6 @@ using namespace fb200;
 
 extern "C" const char* fb200_last_error(void) { return fb200::g_err; }
 extern "C" int fb200_version(void) { return 100; }
-extern "C" int fb200_device_supports_tcgen05(void) {
-  int dev = 0, major = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return FB200_ERR_CUDA;
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return FB200_ERR_CUDA;
-  return major == 9 ? 1 : 0;
-}
 
 static int stem_launch(const void* img, bool u8, int B, int H, int W, const float* w, const float* scale, const float* bias, const float* mean3,
                        const float* std3, int act, void* out, int out_dtype, int Cout, void* stream) {

@@ -22,7 +22,7 @@ from __future__ import annotations
 
 import math
 from collections import OrderedDict
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional
 
 import torch
 import torch.nn as nn
@@ -233,8 +233,7 @@ def _split3_weights(w):
 
 def _split3_ok(x, w3, act, algo):
     a = (act & 15)
-    return (w3 is not None and algo != ops.ALGO_SIMT and x.dtype == torch.float32 and (x.is_cuda or ops._backend is not None) and a not in (ops.ACT_GELU, 4)
-            and (x.numel() // x.shape[-1]) >= 64)
+    return w3 is not None and algo != ops.ALGO_SIMT and x.dtype == torch.float32 and a not in (ops.ACT_GELU, 4) and (x.numel() // x.shape[-1]) >= 64
 
 
 class _Conv:
@@ -273,33 +272,25 @@ class _Linear:
                 self.w3 = _split3_weights(self.w)
 
     def __call__(self, x, act=ops.ACT_NONE, residual=None, out_dtype=None, out=None, algo=ops.ALGO_AUTO):
-        if (act & 15) == ops.ACT_GELU and residual is None and _split3_ok(x, self.w3, ops.ACT_NONE, algo) and (out_dtype in (None, torch.float32)):
-            # exact-erf GELU (AIFI FFN) in the fp32-accurate mode: the tensor-core product without activation, then GELU in place (the GELU epilogue instantiation
-            # is fp16-only; without this the layer fell back to the CUDA-core fp32 GEMM: 256 us vs ~30)
-            from . import autograd_ops  # noqa: F401  (binds fb200_add_act)
-            y = self(x, act=ops.ACT_NONE, out_dtype=out_dtype, out=out, algo=algo)
-            ops._be().add_act(y, None, None, ops.ACT_GELU, y)
-            return y
         if _split3_ok(x, self.w3, act, algo) and (out_dtype in (None, torch.float32)):
             return ops.linear(ops.split_pair(x), self.w3, self.bias, act=act, residual=residual, out_dtype=torch.float32, out=out, algo=ops.ALGO_TCGEN05_SPLIT3)
         return ops.linear(x, self.w, self.bias, act=act, residual=residual, out_dtype=out_dtype, out=out, algo=algo)
 
 
-def _enable_split3(obj, seen=None, host_w3=None):
-    """walk an engine's packed layers (attributes / lists / dicts / tuples) and attach the split-precision weight triples
-    (`host_w3`: triples already split on the host at pack time, keyed by id() of the packed device weight)"""
+def _packed_layers(obj, seen=None):
+    """every packed layer (_Conv / _Linear) reachable from obj through dicts / lists / tuples, once each"""
     seen = set() if seen is None else seen
     if id(obj) in seen:
         return
     seen.add(id(obj))
     if isinstance(obj, (_Conv, _Linear)):
-        obj.enable_split3(host_w3)
+        yield obj
     elif isinstance(obj, dict):
         for v in obj.values():
-            _enable_split3(v, seen, host_w3)
+            yield from _packed_layers(v, seen)
     elif isinstance(obj, (list, tuple)):
         for v in obj:
-            _enable_split3(v, seen, host_w3)
+            yield from _packed_layers(v, seen)
 
 
 def _bn_fold(sd, p, eps=1e-5):
@@ -308,26 +299,33 @@ def _bn_fold(sd, p, eps=1e-5):
 
 
 class DetrEngine:
-    """Packs a FAIDetr state_dict for one (device, precision) and runs the fused forward."""
+    """Packs a state_dict for one (device, precision) and runs the fused forward.  The engines of the other families subclass it and implement `_pack`.
 
-    _host_w3 = None  # set per instance in fp32_tc mode (see _to)
+    precision "fp16" / "fp32": activations in that dtype; `algo` goes to every conv / linear (ALGO_SIMT: the CUDA-core kernels).
+    precision "fp32_tc": the pair flow - fp32 storage, every conv / linear of the flow three fp16 tensor-core products on activations kept as fp16 [hi | lo]
+    planes between them (`_pc` / `_plin`); it runs only with the default algorithm choice."""
 
-    def __init__(self, sd: Dict[str, torch.Tensor], cfg: DETRConfig, device, precision: str = "fp16", algo: int = ops.ALGO_AUTO):
+    def __init__(self, sd: Dict[str, torch.Tensor], cfg, device, precision: str = "fp16", algo: int = ops.ALGO_AUTO):
         assert precision in ("fp32", "fp16", "fp32_tc")
+        if precision == "fp32_tc" and algo != ops.ALGO_AUTO:
+            raise ValueError(f"focoos_b200: precision 'fp32_tc' runs the tensor-core pair flow and takes no other algorithm (got algo={algo})")
         self.cfg, self.device, self.precision, self.algo = cfg, torch.device(device), precision, algo
         self.dt = torch.float16 if precision == "fp16" else torch.float32
-        self.depth = cfg.backbone_config.depth
-        self.nhead = cfg.transformer_predictor_nhead
-        self.d = cfg.transformer_predictor_hidden_dim
-        self._consts: Dict[Tuple[int, int], dict] = {}
+        self._consts = {}  # per-resolution constants (_constants, MFEngine._pos)
         self._host_w3 = {} if precision == "fp32_tc" else None  # id(packed device weight) -> [W_hi|W_lo|W_hi] split on the host in _to()
         # pack on the HOST (BN folding, re-parameterisation, concatenations are a few hundred tiny tensor ops: as device launches they were ~700 `at::`
         # kernels in front of the first forward); only the packed tensors travel to the device
         sd = {k: v.detach().to("cpu") for k, v in sd.items()}
         self._pack(sd)
-        if precision == "fp32_tc":  # fp32 storage everywhere; convs/linears = three fp16 tensor-core products (fp32-accurate)
-            _enable_split3(vars(self), host_w3=self._host_w3)
+        if precision == "fp32_tc":
+            for layer in _packed_layers(vars(self)):
+                layer.enable_split3(self._host_w3)
+            assert all(layer.w3 is not None for layer in self._pair_layers()), "fp32_tc: a layer of the pair flow has no [W_hi|W_lo|W_hi] weight triple"
         self._host_w3 = None
+
+    def _pair_layers(self):
+        """the packed layers the fp32_tc flow runs on their weight triples: all but query_pos_head.layers.0 (K = 4), which stays fp32"""
+        return [layer for layer in _packed_layers(vars(self)) if layer is not self.qpos[0]]
 
     # ---- packing -------------------------------------------------------------------------------
     def _to(self, t, dtype=None):
@@ -408,6 +406,8 @@ class DetrEngine:
         return feats
 
     def _pack(self, sd):
+        cfg = self.cfg
+        self.depth, self.nhead, self.d = cfg.backbone_config.depth, cfg.transformer_predictor_nhead, cfg.transformer_predictor_hidden_dim
         self._pack_backbone(sd)
         pd = "pixel_decoder"
         self.enc_in = [self._seq_conv_bn(sd, f"{pd}.input_proj.{i}.0", f"{pd}.input_proj.{i}.1") for i in range(3)]
@@ -480,7 +480,7 @@ class DetrEngine:
         B, L, d = x.shape
         qk = blk["qk"](ops.add(x, pos), algo=self.algo)
         v = blk["v"](x, algo=self.algo)
-        a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, 1.0 / math.sqrt(d // self.nhead), split=self.precision == "fp32_tc")
+        a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, 1.0 / math.sqrt(d // self.nhead))
         y = blk["out"](a, residual=x, algo=self.algo)
         return ops.layernorm(y, *blk["n_attn"])
 
@@ -538,10 +538,6 @@ class DetrEngine:
             last = i == len(reps) - 1
             x = self._pc(r, x, residual=y12.slice(C, 2 * C) if last else None, act=(ops.ACT_SILU | 16) if last else None, out=out if last else None)
         return x
-
-    def pair_capable(self) -> bool:
-        """the pair-native fp32_tc data flow is available (default algorithm choice, a tensor-core (sm_90) device or the CPU test backend)"""
-        return self.precision == "fp32_tc" and self.algo == ops.ALGO_AUTO and (ops._backend is not None or ops.supports_tcgen05_cached())
 
     def _run_backbone_pair(self, images):
         """ResNet-vd in the pair format -> [res2, res3, res4, res5] as Pairs (nn/backbone/resnet.py:252-266); shared by every model family with this backbone"""
@@ -614,7 +610,7 @@ class DetrEngine:
             # DETRProcessor resizes to im_size; the encoder buffers, anchors and positional constants are laid out for 1/8 and 1/16 maps of exactly 4x and
             # 2x the 1/32 map, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
             raise ValueError(f"focoos_b200: input size {H}x{W} is not a multiple of 32; resize/pad the image (e.g. ModelInfo.im_size) before the model")
-        if self.pair_capable():
+        if self.precision == "fp32_tc":
             mem_pair, shapes, K = self._forward_pair_trunk(images, taps)
             value_all = self._plin(self.value_all, mem_pair)
             t = self._plin(self.enc_output, mem_pair)
@@ -667,13 +663,13 @@ class DetrEngine:
         return self._forward_head(t, value_all, memory, shapes, K, B, S, taps)
 
     def _forward_head(self, t, value_all, memory, shapes, K, B, S, taps):
-        """query selection + decoder + head on the encoder memory (every flow but the pair-native fp32_tc one, which runs _forward_head_pair)"""
+        """query selection + decoder + head on the encoder memory of the fp16 / fp32 flow (fp32_tc runs _forward_head_pair)"""
         cfg, dt, A, d = self.cfg, self.dt, self.algo, self.d
         dev = t.device
         t = ops.row_select(t, K["valid"], self.enc_output.bias)
         output_memory = ops.layernorm(t, *self.enc_output_ln)
         ncls = cfg.num_classes
-        if self.precision == "fp16" and A == ops.ALGO_AUTO and ops.supports_tcgen05_cached():
+        if self.precision == "fp16" and A == ops.ALGO_AUTO:
             # only the per-anchor maximum is ever used in eval (modelling.py:1210-1214): the [B,S,365] fp32 logits (395 MB at bs=32) are never materialised
             scores = ops.linear_rowmax(output_memory, self.enc_score.w, self.enc_score.bias)
         else:
@@ -760,50 +756,18 @@ def cfg_points(cfg) -> int:
     return 4  # num_decoder_points (modelling.py:1039)
 
 
-class FAIDetr(nn.Module):
-    """Drop-in for the reference `FAIDetr(BaseModelNN)` (modelling.py:1273): same constructor argument, same
-    state_dict, `forward(images[, targets]) -> DETRModelOutput`, `.device` / `.dtype` from `pixel_mean`."""
+class _EngineModel(nn.Module):
+    """The nn.Module side of every model family: parameters under the reference's state_dict keys, `.device` / `.dtype` from `pixel_mean`, and
+    the `engine_cls` engine packed from the parameters for the current (device, precision, algo) on first use, dropped whenever they may change."""
 
-    def __init__(self, config: DETRConfig, precision: str = "fp16"):
+    engine_cls: type
+
+    def __init__(self, config, precision: str = "fp16"):
         super().__init__()
-        self.config = config
-        c = config
-        self.pixel_decoder = Encoder(ResNet(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_nhead,
-                                     c.pixel_decoder_dim_feedforward, c.pixel_decoder_num_encoder_layers)
-        self.head = DETRHead(TransformerPredictor(c.pixel_decoder_out_dim, c.num_classes, c.transformer_predictor_hidden_dim, c.num_queries,
-                                                  c.transformer_predictor_nhead, c.transformer_predictor_dec_layers,
-                                                  c.transformer_predictor_dim_feedforward), c.num_classes)
-        self.register_buffer("pixel_mean", torch.tensor(c.pixel_mean, dtype=torch.float32).view(-1, 1, 1), False)
-        self.register_buffer("pixel_std", torch.tensor(c.pixel_std, dtype=torch.float32).view(-1, 1, 1), False)
-        self.num_classes = c.num_classes
-        self.precision = precision
-        self.algo = ops.ALGO_AUTO
-        self._engine: Optional[DetrEngine] = None
-        self.train_precision = None  # training arithmetic: None (follow `precision`), "fp32", "fp32_tc" or "amp" (see train_graph)
-        self.sync_bn = False    # training: BatchNorm statistics over all data-parallel ranks (torch.nn.SyncBatchNorm, trainer/trainer.py:334); set by the trainer
-        self.freeze_bn = False  # training: every BatchNorm as FrozenBatchNorm2d (TrainerArgs.freeze_bn, trainer/trainer.py:330)
-        from .train_step import freeze_backbone_at, freeze_backbone_norm
-        freeze_backbone_at(self, getattr(c.backbone_config, "freeze_at", -1), getattr(c.backbone_config, "num_stages", 4))  # resnet.py:221-224
-        if getattr(c.backbone_config, "freeze_norm", False):  # resnet.py:226 (the registry configs ship freeze_norm=false)
-            freeze_backbone_norm(self)
-        self.eval()
+        self.config, self.num_classes, self.precision, self.algo, self._engine = config, config.num_classes, precision, ops.ALGO_AUTO, None
 
-    @property
-    def device(self):
-        return self.pixel_mean.device
-
-    @property
-    def dtype(self):
-        return self.pixel_mean.dtype
-
-    def train(self, mode: bool = True):
-        self._engine = None  # packed (BN-folded, re-parameterised) weights are rebuilt from the parameters at the next eval forward
-        return super().train(mode)
-
-    def set_precision(self, precision: str, algo: int = ops.ALGO_AUTO):
-        assert precision in ("fp32", "fp16", "fp32_tc")
-        self.precision, self.algo, self._engine = precision, algo, None
-        return self
+    device = property(lambda self: self.pixel_mean.device)
+    dtype = property(lambda self: self.pixel_mean.dtype)
 
     def load_state_dict(self, state_dict, strict: bool = False, assign: bool = False):
         """Shape-tolerant non-strict load like BaseModelNN.load_state_dict (models/base_model.py:98-143); accepts
@@ -821,6 +785,46 @@ class FAIDetr(nn.Module):
     def _apply(self, fn, *a, **k):
         self._engine = None
         return super()._apply(fn, *a, **k)
+
+    def engine(self):
+        e = self._engine
+        if e is None or e.device != self.device or e.precision != self.precision or e.algo != self.algo:
+            self._engine = self.engine_cls(self.state_dict(), self.config, self.device, self.precision, self.algo)
+        return self._engine
+
+    def _check_device(self, images):
+        if ops._backend is None and not images.is_cuda:
+            raise RuntimeError(f"focoos_b200.{type(self).__name__} runs on CUDA (sm_90a) only — no CPU fallback; move the model and inputs to the GPU")
+
+
+class FAIDetr(_EngineModel):
+    """Drop-in for the reference `FAIDetr(BaseModelNN)` (modelling.py:1273): same constructor argument, same
+    state_dict, `forward(images[, targets]) -> DETRModelOutput`."""
+
+    engine_cls = DetrEngine
+
+    def __init__(self, config: DETRConfig, precision: str = "fp16"):
+        super().__init__(config, precision)
+        c = config
+        self.pixel_decoder = Encoder(ResNet(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_nhead,
+                                     c.pixel_decoder_dim_feedforward, c.pixel_decoder_num_encoder_layers)
+        self.head = DETRHead(TransformerPredictor(c.pixel_decoder_out_dim, c.num_classes, c.transformer_predictor_hidden_dim, c.num_queries,
+                                                  c.transformer_predictor_nhead, c.transformer_predictor_dec_layers,
+                                                  c.transformer_predictor_dim_feedforward), c.num_classes)
+        self.register_buffer("pixel_mean", torch.tensor(c.pixel_mean, dtype=torch.float32).view(-1, 1, 1), False)
+        self.register_buffer("pixel_std", torch.tensor(c.pixel_std, dtype=torch.float32).view(-1, 1, 1), False)
+        self.train_precision = None  # training arithmetic: None (follow `precision`), "fp32", "fp32_tc" or "amp" (see train_graph)
+        self.sync_bn = False    # training: BatchNorm statistics over all data-parallel ranks (torch.nn.SyncBatchNorm, trainer/trainer.py:334); set by the trainer
+        self.freeze_bn = False  # training: every BatchNorm as FrozenBatchNorm2d (TrainerArgs.freeze_bn, trainer/trainer.py:330)
+        from .train_step import freeze_backbone_at, freeze_backbone_norm
+        freeze_backbone_at(self, getattr(c.backbone_config, "freeze_at", -1), getattr(c.backbone_config, "num_stages", 4))  # resnet.py:221-224
+        if getattr(c.backbone_config, "freeze_norm", False):  # resnet.py:226 (the registry configs ship freeze_norm=false)
+            freeze_backbone_norm(self)
+        self.eval()
+
+    def train(self, mode: bool = True):
+        self._engine = None  # packed (BN-folded, re-parameterised) weights are rebuilt from the parameters at the next eval forward
+        return super().train(mode)
 
     def train_graph(self):
         """training-mode forward built from the autograd ops (fai_detr_train.py); fp32 storage, tensor-core split products by default"""
@@ -846,14 +850,8 @@ class FAIDetr(nn.Module):
                 deep_supervision=c.criterion_deep_supervision)
         return self._criterion
 
-    def engine(self) -> DetrEngine:
-        if self._engine is None or self._engine.device != self.device or self._engine.precision != self.precision or self._engine.algo != self.algo:
-            self._engine = DetrEngine(self.state_dict(), self.config, self.device, self.precision, self.algo)
-        return self._engine
-
     def forward(self, images: torch.Tensor, targets: list = [], taps: Optional[dict] = None) -> DETRModelOutput:
-        if ops._backend is None and not images.is_cuda:
-            raise RuntimeError("focoos_b200.FAIDetr runs on CUDA (sm_90a) only — no CPU fallback; move the model and inputs to the GPU")
+        self._check_device(images)
         if self.training:  # modelling.py:1354-1356: losses only, empty logits/boxes
             assert targets is not None and len(targets) > 0, "targets should not be None or empty - training mode"
             outputs = self.train_graph().forward(images)

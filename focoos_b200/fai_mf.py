@@ -20,13 +20,13 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field, fields
-from typing import Dict, List, Optional
+from typing import List, Optional
 
 import torch
 import torch.nn as nn
 
 from . import ops
-from .fai_detr import _split3_weights, MLP, DetrEngine, ResNet, _bn_fold, _Conv, _CriterionStub, _enable_split3, _Linear
+from .fai_detr import _split3_weights, MLP, DetrEngine, ResNet, _bn_fold, _Conv, _CriterionStub, _EngineModel, _Linear, _packed_layers
 from .ports import ModelOutput, ResnetConfig
 
 
@@ -214,17 +214,9 @@ class MFEngine(DetrEngine):
 
     lazy_masks = False  # True: return LazyMasks instead of the materialised [B,Q,H,W] probabilities
 
-    def __init__(self, sd: Dict[str, torch.Tensor], cfg: MaskFormerConfig, device, precision: str = "fp16", algo: int = ops.ALGO_AUTO):
-        self.cfg, self.device, self.precision, self.algo = cfg, torch.device(device), precision, algo
-        assert precision in ("fp32", "fp16", "fp32_tc")
-        self.dt = torch.float16 if precision == "fp16" else torch.float32
-        self._host_w3 = {} if precision == "fp32_tc" else None  # fp32 storage, three fp16 tensor-core products per conv / linear (fai_detr._split3_weights)
-        self.depth = cfg.backbone_config.depth
-        self.nhead, self.d = 8, cfg.transformer_predictor_hidden_dim
-        self._consts = {}
-        # pack on the HOST (BN folding, re-parameterisation, concatenations are a few hundred tiny tensor ops: as device launches they were ~700 `at::`
-        # kernels in front of the first forward); only the packed tensors travel to the device
-        sd = {k: v.detach().to("cpu") for k, v in sd.items()}
+    def _pack(self, sd):
+        cfg = self.cfg
+        self.depth, self.nhead, self.d = cfg.backbone_config.depth, 8, cfg.transformer_predictor_hidden_dim
         self._pack_backbone(sd)
         pd = "pixel_decoder"
         self.pd_in = self._conv_bias(sd, pd + ".input_proj", 0)
@@ -234,12 +226,10 @@ class MFEngine(DetrEngine):
         self.adapter = {i: self._conv_bn(sd, f"{pd}.adapter_{i}", 0, ops.ACT_NONE) for i in (1, 2, 3)}
         self.mask_features = self._conv_bias(sd, pd + ".mask_features", 1)
         self._pack_decoder(sd, 3)
-        self._finish_pack()
 
-    def _finish_pack(self):
-        if self.precision == "fp32_tc":
-            _enable_split3(vars(self), host_w3=self._host_w3)
-        self._host_w3 = None
+    def _pair_layers(self):
+        """the backbone, the pixel-decoder convs that read its pairs, the 1/4-resolution chain into mask_features, and the decoder linears"""
+        return list(_packed_layers([self.stem2, self.stem3, self.stages, self.pd_in, self.adapter, self.layer[1], self.mask_features, self.dec, self.mask_mlp]))
 
     def _pack_decoder(self, sd, num_levels):
         """head.predictor.* of the masked transformer decoder (same key names in fai_mf and bisenetformer)."""
@@ -279,12 +269,13 @@ class MFEngine(DetrEngine):
             self._consts[key] = self._to(position_embedding_sine_normalized(h, w, self.d // 2))
         return self._consts[key]
 
-    def _heads(self, out, mask_features, mf_pair, fused, size, want_class):
+    def _heads(self, out, mask_features, size, want_class):
         """PredictionHeads.forward (:69-112) -> (class logits fp32 or None, mask logits NHWC [B,h4,w4,Qp], (mask, allowed) or None).
-        mf_pair: mask_features as fp16 [hi | lo] planes (fp32_tc) or None; fused: the fused row glue of the fp32_tc decoder (see _run_decoder)."""
+        mask_features: a Pair under fp32_tc (see _run_decoder)."""
         A, dt = self.algo, self.dt
         B, Q, d = out.shape
-        if fused:  # fp32_tc: LayerNorm writes the pair operand of the mask MLP, whose hidden layers stay in the pair format
+        pair = self.precision == "fp32_tc"
+        if pair:  # LayerNorm writes the pair operand of the mask MLP, whose hidden layers stay in the pair format
             dn, dnp, _ = ops.layernorm_ex(out, *self.head_norm, want_f32=want_class)
             cls = self.classifier(dn, out_dtype=torch.float32, algo=ops.ALGO_SIMT) if want_class else None
             me = self._plin(self.mask_mlp[2], self._plin(self.mask_mlp[1], self._plin(self.mask_mlp[0], dnp, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True))
@@ -296,10 +287,10 @@ class MFEngine(DetrEngine):
         Qp = (Q + 7) // 8 * 8
         masks = torch.zeros((B, h4, w4, Qp), dtype=dt, device=out.device)
         # einsum("bqc,bchw->bqhw"): a [h4*w4, C] x [C, Q] GEMM per image whose "weights" (the mask embeddings) differ per image - ONE launch
-        if mf_pair is not None:
-            # fp32_tc: the same GEMM as three fp16 tensor-core products - mask_features split ONCE per forward (_run_decoder), the per-image embeddings as
-            # [W_hi | W_lo | W_hi] triples.  (On the CUDA-core fp32 kernel this product was a third of the parity-mode step: 16.9 of 50.4 ms at bs=16 800x800.)
-            ops.conv2d_per_image(mf_pair, _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=masks[..., :Q], algo=ops.ALGO_TCGEN05_SPLIT3)
+        if pair:
+            # the same GEMM as three fp16 tensor-core products on the mask_features pair and the per-image embeddings as [W_hi | W_lo | W_hi] triples.
+            # (On the CUDA-core fp32 kernel this product was a third of the parity-mode step: 16.9 of 50.4 ms at bs=16 800x800.)
+            ops.conv2d_per_image(mask_features.buf, _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=masks[..., :Q], algo=ops.ALGO_TCGEN05_SPLIT3)
         else:
             ops.conv2d_per_image(mask_features, me.reshape(B, Q, 1, 1, C), out=masks[..., :Q], algo=A)
         attn = None
@@ -317,9 +308,9 @@ class MFEngine(DetrEngine):
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
         # any H x W, like the reference (its processor does not resize): odd maps from the stride-2 convs and ceil-mode pools run on the same kernels
-        pair = self.pair_capable() and all(getattr(c, "w3", None) is not None for c in [self.pd_in] + [self.adapter[i] for i in (1, 2, 3)])
+        pair = self.precision == "fp32_tc"
         if pair:
-            # fp32_tc: the backbone keeps its activations as fp16 [hi | lo] planes between convs (no split pass in front of every conv, DetrEngine._run_backbone_pair);
+            # the backbone keeps its activations as fp16 [hi | lo] planes between convs (no split pass in front of every conv, DetrEngine._run_backbone_pair);
             # the four pixel-decoder convs that consume res2..res5 read the pairs and write the fp32 tensors the transformer / FPN arithmetic below works on
             res2, res3, res4, res5 = self._run_backbone_pair(images)
             in_conv = lambda conv, f: self._pc(conv, f, out_pair=False)  # noqa: E731
@@ -336,7 +327,7 @@ class MFEngine(DetrEngine):
         for blk in self.enc:  # pre-norm encoder layer (nn/layers/transformer.py:583-601 with normalize_before)
             s2 = ops.layernorm(src, *blk["n_attn"])
             qk = blk["qk"](ops.add(s2, pos), algo=A)
-            a = ops.attention(qk[..., :d], qk[..., d:], blk["v"](s2, algo=A), nh, scale, split=self.precision == "fp32_tc")
+            a = ops.attention(qk[..., :d], qk[..., d:], blk["v"](s2, algo=A), nh, scale, split=pair)
             src = blk["out"](a, residual=src, algo=A)
             s2 = ops.layernorm(src, *blk["n_ffn"])
             src = blk["l2"](blk["l1"](s2, act=ops.ACT_RELU, algo=A), residual=src, algo=A)
@@ -345,15 +336,14 @@ class MFEngine(DetrEngine):
         ms = [y]
         # fp32_tc: the 1/4-resolution layer feeds only the mask_features conv, whose output is only ever read as a tensor-core operand (the per-image mask product):
         # both stay in the pair format - no fp32 copy of the two largest activations of the pixel decoder, no split pass over them
-        chain = pair and getattr(self.layer[1], "w3", None) is not None and getattr(self.mask_features, "w3", None) is not None
         for idx, f in ((3, res4), (2, res3), (1, res2)):
             u = ops.upsample_nearest_add(y, in_conv(self.adapter[idx], f))
-            y = self._pc(self.layer[idx], u) if (chain and idx == 1) else self.layer[idx](u, algo=A)
+            y = self._pc(self.layer[idx], u) if (pair and idx == 1) else self.layer[idx](u, algo=A)
             if len(ms) < 3:
                 ms.append(y)
-        mask_features = self._pc(self.mask_features, y) if chain else self.mask_features(y, algo=A)
+        mask_features = self._pc(self.mask_features, y) if pair else self.mask_features(y, algo=A)
         if taps is not None:
-            taps.update(res5=res5.float() if pair else res5, enc_memory=src.reshape(B, h, w, d), mask_features=mask_features.float() if chain else mask_features, multi_scale=ms)
+            taps.update(res5=res5.float(), enc_memory=src.reshape(B, h, w, d), mask_features=mask_features.float(), multi_scale=ms)
         return self._run_decoder(ms, mask_features, B, H, W, taps)
 
     def _run_decoder(self, ms, mask_features, B, H, W, taps=None):
@@ -363,12 +353,10 @@ class MFEngine(DetrEngine):
         d, nh = self.d, self.nhead
         scale = 1.0 / math.sqrt(d // nh)
         nl = len(ms)
-        mf_pair = None
-        if isinstance(mask_features, ops.Pair):  # written as a pair by its conv (MFEngine.forward)
-            mf_pair = mask_features.buf
-        elif (self.precision == "fp32_tc" and A == ops.ALGO_AUTO and mask_features.dtype == torch.float32 and mask_features.shape[-1] % 64 == 0
-                and (ops._backend is not None or ops.supports_tcgen05_cached())):
-            mf_pair = ops.split_pair(mask_features)  # consumed by every _heads call of this forward
+        pair = self.precision == "fp32_tc"
+        if pair:  # every _heads call reads mask_features as a Pair: MaskFormer's conv writes one, BisenetFormer's fp32 output is split once here
+            assert mask_features.shape[-1] % 64 == 0, mask_features.shape
+            mask_features = ops.to_pair(mask_features)
         srcs, kpos, sizes = [], [], []
         for i in range(nl):
             hh, ww = ms[i].shape[1], ms[i].shape[2]
@@ -376,25 +364,20 @@ class MFEngine(DetrEngine):
             srcs.append(s)
             kpos.append(ops.add(s, self._pos(hh, ww)))
             sizes.append((hh, ww))
-        # fp32_tc: masked cross-attention on the tensor cores (fb200_attention_masked_split); the per-level key / value inputs are split ONCE (they are the same for the
-        # three layers of a level) and the K / V projections run pair -> pair
-        split_attn = self.precision == "fp32_tc" and A == ops.ALGO_AUTO
-        pair_kv = split_attn and self.pair_capable() and all(b_["ck"].w3 is not None and b_["cv"].w3 is not None for b_ in self.dec)
-        if pair_kv:
-            kpos_p, srcs_p = [ops.to_pair(t) for t in kpos], [ops.to_pair(t) for t in srcs]
         Q = cfg.num_queries
         out = self.query_feat.unsqueeze(0).expand(B, Q, d).contiguous()
         qpos = self.query_embed
-        # fused row glue (csrc/head_fused.cu, the kernels of the fai-detr head): every LayerNorm writes the pair operand(s) of the linears behind it - LN(x) and
-        # LN(x) + query_pos in one launch - and the FFN / mask-MLP hidden layers stay in the pair format: no add / split launches between two tensor-core linears
-        lins = [b_[k] for b_ in self.dec for k in ("cq", "cout", "sqk", "sv", "sout", "l1", "l2")] + list(self.mask_mlp)
-        fused = bool(pair_kv and all(getattr(l_, "w3", None) is not None for l_ in lins))
-        _, masks, attn = self._heads(out, mask_features, mf_pair, fused, sizes[0], False)
         L = len(self.dec)
         cls = None
-        for i, blk in enumerate(self.dec):
-            lvl = i % nl
-            if fused:
+        if pair:
+            # masked cross-attention on the tensor cores (fb200_attention_masked_split): the per-level key / value inputs are split ONCE (they are the same for
+            # the layers of a level) and the K / V projections run pair -> pair.  Fused row glue (csrc/head_fused.cu, the kernels of the fai-detr head): every
+            # LayerNorm writes the pair operand(s) of the linears behind it - LN(x) and LN(x) + query_pos in one launch - and the FFN / mask-MLP hidden layers
+            # stay in the pair format: no add / split launches between two tensor-core linears
+            kpos_p, srcs_p = [ops.to_pair(t) for t in kpos], [ops.to_pair(t) for t in srcs]
+            _, masks, attn = self._heads(out, mask_features, sizes[0], False)
+            for i, blk in enumerate(self.dec):
+                lvl = i % nl
                 _, _, tq = ops.layernorm_ex(out, *blk["cn"], pos=qpos, want_f32=False, want_pair=False, want_pair_pos=True)
                 q = self._plin(blk["cq"], tq)
                 kk, vv = self._plin(blk["ck"], kpos_p[lvl], out_pair=True), self._plin(blk["cv"], srcs_p[lvl], out_pair=True)
@@ -407,28 +390,27 @@ class MFEngine(DetrEngine):
                 _, t2p, _ = ops.layernorm_ex(out, *blk["fn"], want_f32=False)
                 out = self._plin(blk["l2"], self._plin(blk["l1"], t2p, act=ops.ACT_RELU, out_pair=True), residual=out)
                 last = i == L - 1
-                cls, masks, attn = self._heads(out, mask_features, mf_pair, fused, None if last else sizes[(i + 1) % nl], last)
+                cls, masks, attn = self._heads(out, mask_features, None if last else sizes[(i + 1) % nl], last)
                 if taps is not None:
                     taps[f"dec{i}_out"] = out
-                continue
-            t2 = ops.layernorm(out, *blk["cn"])
-            q = blk["cq"](ops.add(t2, qpos), algo=A)
-            if pair_kv:  # K / V projections write the fp16 [hi | lo] pairs the attention kernel stages with plain 16-byte copies
-                kk, vv = self._plin(blk["ck"], kpos_p[lvl], out_pair=True), self._plin(blk["cv"], srcs_p[lvl], out_pair=True)
-            else:
-                kk, vv = blk["ck"](kpos[lvl], algo=A), blk["cv"](srcs[lvl], algo=A)
-            a = ops.attention_masked(q, kk, vv, attn[0], attn[1], nh, scale, split=split_attn)
-            out = blk["cout"](a, residual=out, algo=A)
-            t2 = ops.layernorm(out, *blk["sn"])
-            qk = blk["sqk"](ops.add(t2, qpos), algo=A)
-            a = ops.attention(qk[..., :d], qk[..., d:], blk["sv"](t2, algo=A), nh, scale, split=self.precision == "fp32_tc")
-            out = blk["sout"](a, residual=out, algo=A)
-            t2 = ops.layernorm(out, *blk["fn"])
-            out = blk["l2"](blk["l1"](t2, act=ops.ACT_RELU, algo=A), residual=out, algo=A)
-            last = i == L - 1
-            cls, masks, attn = self._heads(out, mask_features, mf_pair, fused, None if last else sizes[(i + 1) % nl], last)
-            if taps is not None:
-                taps[f"dec{i}_out"] = out
+        else:
+            _, masks, attn = self._heads(out, mask_features, sizes[0], False)
+            for i, blk in enumerate(self.dec):
+                lvl = i % nl
+                t2 = ops.layernorm(out, *blk["cn"])
+                q = blk["cq"](ops.add(t2, qpos), algo=A)
+                a = ops.attention_masked(q, blk["ck"](kpos[lvl], algo=A), blk["cv"](srcs[lvl], algo=A), attn[0], attn[1], nh, scale)
+                out = blk["cout"](a, residual=out, algo=A)
+                t2 = ops.layernorm(out, *blk["sn"])
+                qk = blk["sqk"](ops.add(t2, qpos), algo=A)
+                a = ops.attention(qk[..., :d], qk[..., d:], blk["sv"](t2, algo=A), nh, scale)
+                out = blk["sout"](a, residual=out, algo=A)
+                t2 = ops.layernorm(out, *blk["fn"])
+                out = blk["l2"](blk["l1"](t2, act=ops.ACT_RELU, algo=A), residual=out, algo=A)
+                last = i == L - 1
+                cls, masks, attn = self._heads(out, mask_features, None if last else sizes[(i + 1) % nl], last)
+                if taps is not None:
+                    taps[f"dec{i}_out"] = out
         if taps is not None:
             taps.update(pred_logits=cls, pred_masks=masks)  # masks: NHWC [B,h4,w4,Qp] pre-sigmoid logits
         probs = ops.softmax_drop_last(cls)
@@ -436,14 +418,29 @@ class MFEngine(DetrEngine):
         return probs, (lazy if self.lazy_masks else lazy.materialize())
 
 
-class FAIMaskFormer(nn.Module):
-    """Drop-in for the reference `FAIMaskFormer(BaseModelNN)` (fai_mf/modelling.py:633)."""
+class _SegmentationModel(_EngineModel):
+    """What FAIMaskFormer and BisenetFormer share: inference through the engine, masks returned as LazyMasks when `lazy_masks` is set."""
 
     lazy_masks = False  # True: forward() returns fai_mf.LazyMasks (low-resolution logits) instead of the upsampled [B,Q,H,W] probabilities
 
+    def forward(self, images: torch.Tensor, targets: list = [], taps: Optional[dict] = None) -> MaskFormerModelOutput:
+        if self.training or (targets is not None and len(targets) > 0):
+            raise NotImplementedError("focoos_b200: losses / fine-tuning are not part of the inference hot path")
+        self._check_device(images)
+        eng = self.engine()
+        eng.lazy_masks = bool(getattr(self, "lazy_masks", False))
+        probs, masks = eng.forward(images if images.dtype == torch.uint8 else images.to(torch.float32), taps)
+        return MaskFormerModelOutput(masks=masks, logits=probs, loss=None)
+
+
+class FAIMaskFormer(_SegmentationModel):
+    """Drop-in for the reference `FAIMaskFormer(BaseModelNN)` (fai_mf/modelling.py:633)."""
+
+    engine_cls = MFEngine
+
     def __init__(self, config: MaskFormerConfig, precision: str = "fp16"):
-        super().__init__()
-        self.config = c = config
+        super().__init__(config, precision)
+        c = config
         if c.postprocessing_type not in ("semantic", "instance"):
             raise ValueError(f"Invalid postprocessing type: {c.postprocessing_type}. Must be one of: ['semantic', 'instance']")
         self.pixel_decoder = TransformerFPN(ResNet(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_transformer_layers,
@@ -453,39 +450,4 @@ class FAIMaskFormer(nn.Module):
                                                                       c.transformer_predictor_dim_feedforward, c.transformer_predictor_dec_layers), c.num_classes)
         self.register_buffer("pixel_mean", torch.tensor(c.pixel_mean, dtype=torch.float32).view(-1, 1, 1), False)
         self.register_buffer("pixel_std", torch.tensor(c.pixel_std, dtype=torch.float32).view(-1, 1, 1), False)
-        self.num_classes, self.precision, self.algo, self._engine = c.num_classes, precision, ops.ALGO_AUTO, None
         self.eval()
-
-    device = property(lambda self: self.pixel_mean.device)
-    dtype = property(lambda self: self.pixel_mean.dtype)
-
-    def load_state_dict(self, state_dict, strict: bool = False, assign: bool = False):
-        if "model" in state_dict and isinstance(state_dict["model"], dict):
-            state_dict = state_dict["model"]
-        own = self.state_dict()
-        filtered = {k: v for k, v in state_dict.items() if k in own and tuple(own[k].shape) == tuple(v.shape)}
-        res = super().load_state_dict(filtered, strict=False)
-        self._engine = None
-        if strict and (res.missing_keys or len(filtered) != len(state_dict)):
-            raise RuntimeError(f"load_state_dict(strict): missing {res.missing_keys[:5]} / dropped {len(state_dict) - len(filtered)}")
-        return res
-
-    def _apply(self, fn, *a, **k):
-        self._engine = None
-        return super()._apply(fn, *a, **k)
-
-    def engine(self) -> MFEngine:
-        e = self._engine
-        if e is None or e.device != self.device or e.precision != self.precision or e.algo != self.algo:
-            self._engine = MFEngine(self.state_dict(), self.config, self.device, self.precision, self.algo)
-        return self._engine
-
-    def forward(self, images: torch.Tensor, targets: list = [], taps: Optional[dict] = None) -> MaskFormerModelOutput:
-        if self.training or (targets is not None and len(targets) > 0):
-            raise NotImplementedError("focoos_b200: losses / fine-tuning are not part of the inference hot path")
-        if ops._backend is None and not images.is_cuda:
-            raise RuntimeError("focoos_b200.FAIMaskFormer runs on CUDA (sm_90a) only — no CPU fallback")
-        eng = self.engine()
-        eng.lazy_masks = bool(getattr(self, "lazy_masks", False))
-        probs, masks = eng.forward(images if images.dtype == torch.uint8 else images.to(torch.float32), taps)
-        return MaskFormerModelOutput(masks=masks, logits=probs, loss=None)

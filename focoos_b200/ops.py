@@ -667,23 +667,6 @@ def _be():
     return _cuda_backend
 
 
-def supports_tcgen05() -> bool:
-    return load_library().fb200_device_supports_tcgen05() == 1
-
-
-_tc_ok = None
-
-
-def supports_tcgen05_cached() -> bool:
-    """tensor-core path usable (real sm_90 device; False under the tests' CPU backend hook)"""
-    global _tc_ok
-    if _backend is not None:
-        return False
-    if _tc_ok is None:
-        _tc_ok = supports_tcgen05()
-    return _tc_ok
-
-
 # ------------------------------------------------------------------------------------------------
 # public tensor-level API
 # ------------------------------------------------------------------------------------------------

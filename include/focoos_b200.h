@@ -43,8 +43,6 @@ typedef enum { FB200_ALGO_AUTO = 0, FB200_ALGO_SIMT = 1, FB200_ALGO_TCGEN05 = 2,
 
 const char* fb200_last_error(void);
 int fb200_version(void);
-/* 1 if the current device is sm_90 (the wgmma tensor-core path, FB200_ALGO_TCGEN05*, is usable), 0 otherwise, <0 on error. */
-int fb200_device_supports_tcgen05(void);
 
 /* ---- a2: ResNet-vd stem, first conv fused with the input normalisation ------------------------
  * Replaces `(images - pixel_mean) / pixel_std` (models/fai_detr/modelling.py:1349) followed by

@@ -43,6 +43,23 @@ def seeded_sd(seed=0, name="fai_detr_l_obj365"):
     return seeded_state_dict(manifest_template(name), seed)
 
 
+class ConvCalls:
+    """ops backend wrapper that records the weight operand of every conv2d / conv2d_pair call (which flow a layer took)"""
+
+    def __init__(self, be):
+        self.be, self.w = be, {"conv2d": [], "conv2d_pair": []}
+
+    def __getattr__(self, name):
+        fn = getattr(self.be, name)
+        if name not in self.w:
+            return fn
+
+        def call(*a):
+            self.w[name].append(a[1])
+            return fn(*a)
+        return call
+
+
 def align_by_key(key_a: np.ndarray, key_b: np.ndarray) -> np.ndarray:
     """perm such that key_b[perm] == key_a (both are permutations of the same unique set)."""
     assert sorted(key_a.tolist()) == sorted(key_b.tolist()), "query SETS differ"

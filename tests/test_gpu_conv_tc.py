@@ -37,10 +37,6 @@ def run_case(B, H, W, Cin, Cout, k, stride, act=0, use_res=False, use_scale=True
     assert err <= tolerance * scale, f"tensor-core conv B{B} {H}x{W} {Cin}->{Cout} k{k} s{stride}: max|d|={err:.3e} (scale {scale:.2e}); frac bad={(float(((a-b).abs()>tolerance*scale).float().mean())):.4f}"
 
 
-def test_tc_supported_flag():
-    assert ops.supports_tcgen05()
-
-
 @pytest.mark.parametrize("M,K,N", [(128, 64, 64), (256, 128, 128), (1000, 256, 256), (300, 256, 288), (777, 1024, 256), (128, 256, 512), (9600, 256, 1536)])
 def test_linear_flat(M, K, N):
     run_case(1, 1, M, K, N, 1, 1, seed=M + K + N)

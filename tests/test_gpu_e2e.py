@@ -167,17 +167,22 @@ def test_batch_invariance_and_full_size(sd):
     assert torch.equal(flat, s)
 
 
-def test_fp32_tc_meets_the_parity_bars(sd):
+def test_fp32_tc_runs_the_pair_flow_and_meets_the_parity_bars(sd):
     """precision="fp32_tc" (split-precision tensor-core convs/linears, activations as fp16 [hi|lo] pairs between convs): same bars as the fp32 SIMT mode."""
     g = load_golden("detr_l_obj365_b2_640")
     m = _model(sd, "fp32_tc")
-    assert m.engine().pair_capable()
     proc = DETRProcessor(m.config, image_size=640)
     imgs = synth_images(1, [(640, 640)] * 2)
     x, _ = proc.preprocess(imgs, device=m.device)
     taps = {}
-    out = m(x, taps=taps)
-    torch.cuda.synchronize()
+    trace = ops.enable_trace()
+    try:
+        out = m(x, taps=taps)
+        torch.cuda.synchronize()
+    finally:
+        ops.enable_trace(False)
+    symbols = [e[0] for e in trace]
+    assert "fb200_conv2d_pair" in symbols and "fb200_conv2d" not in symbols, "every conv / linear of the fp32_tc flow runs as conv2d_pair"
     for t in ("res3", "res4", "res5"):
         v = taps[t].permute(0, 3, 1, 2).float().cpu()
         sl = v[:, :: max(1, v.shape[1] // 8)][:, :8, :: max(1, v.shape[2] // 20), :: max(1, v.shape[3] // 20)].numpy()

@@ -10,7 +10,7 @@ from focoos_b200 import FAIDetr, DETRConfig, DETRProcessor, ops
 from focoos_b200.ports import DETRModelOutput
 from oracle.gen_golden import synth_images
 from oracle.ops_ref import RefBackend
-from tests.parity_utils import compare_queries, load_golden, manifest_template, seeded_sd
+from tests.parity_utils import ConvCalls, compare_queries, load_golden, manifest_template, seeded_sd
 
 
 @pytest.fixture()
@@ -32,6 +32,13 @@ def test_no_cpu_fallback():
     m = FAIDetr(DETRConfig())
     with pytest.raises(RuntimeError):
         m(torch.zeros(1, 3, 64, 64))
+
+
+def test_fp32_tc_takes_only_the_default_algorithm():
+    m = FAIDetr(DETRConfig(), precision="fp32_tc")
+    m.algo = ops.ALGO_SIMT
+    with pytest.raises(ValueError):
+        m.engine()
 
 
 def test_fused_graph_matches_golden(ref_backend):
@@ -73,7 +80,7 @@ def test_processor_ragged_sizes(ref_backend):
         assert sorted(tuple(x.bbox) for x in d.detections) == sorted(map(tuple, g["det_boxes"][i, :n].tolist()))
 
 
-def test_fp32_tc_pair_graph_with_fused_glue_matches_golden(ref_backend):
+def test_fp32_tc_runs_only_pair_convs_and_matches_golden(ref_backend):
     """precision="fp32_tc" host orchestration (pair-format trunk, fused row glue of csrc/head_fused.cu in the AIFI / selection / decoder chains) through the CPU
     operator references: same golden bars as the fp32 graph, and the same selected queries, outputs and taps as the fp32 graph under the same references.
     Near-tied selection scores may come out in another order, so the queries are compared as sets and the per-query rows matched by encoder anchor."""
@@ -85,9 +92,14 @@ def test_fp32_tc_pair_graph_with_fused_glue_matches_golden(ref_backend):
     for precision in ("fp32_tc", "fp32"):
         m = FAIDetr(DETRConfig(), precision=precision)
         m.load_state_dict(seeded_sd(0), strict=True)
-        assert m.engine().pair_capable() == (precision == "fp32_tc")
+        ops._backend = calls = ConvCalls(ops._backend)
         taps = {}
         runs[precision] = (m(x, taps=taps), taps)
+        ops._backend = calls.be
+        if precision == "fp32_tc":  # the pair flow runs every conv and linear through conv2d_pair: none goes to conv2d
+            assert not calls.w["conv2d"] and calls.w["conv2d_pair"]
+        else:
+            assert calls.w["conv2d"] and not calls.w["conv2d_pair"]
     (a, ta), (b, tb) = runs["fp32_tc"], runs["fp32"]
     ds, db = compare_queries(g["scores"], g["boxes"], g["enc_topk_ind"], a.logits.numpy(), a.boxes.numpy(), ta["topk_ind"].numpy())
     assert ds < 2e-4 and db < 2e-4, (ds, db)

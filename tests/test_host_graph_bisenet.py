@@ -12,7 +12,7 @@ from focoos_b200.processor import MaskFormerProcessor
 from focoos_b200.utils.seeded_weights import seeded_state_dict
 from oracle.gen_golden import state_dict_digest, synth_images
 from oracle.ops_ref import RefBackend
-from tests.parity_utils import GOLDEN, load_golden, manifest_template
+from tests.parity_utils import GOLDEN, ConvCalls, load_golden, manifest_template
 
 
 @pytest.fixture()
@@ -68,21 +68,25 @@ def test_bisenet_fused_graph_matches_golden(ref_backend):
     assert torch.equal(lazy_out.masks.materialize(), out.masks)
 
 
-def test_bisenet_pair_native_blocks_host_logic(ref_backend):
+def test_bisenet_pair_blocks_run_as_pair_convs(ref_backend):
     """precision="fp32_tc": the stride-1 CatBottlenecks run in the pair format (concat buffer = channel slices of one pair buffer), the stride-2 blocks and the
     context path read the pairs through fp32-output convs - host bookkeeping on the CPU references, same results as the fp32 graph up to the pair rounding."""
     g = load_golden("bisenetformer_l_ade_b2_256x384")
     m = BisenetFormer(BisenetFormerConfig(), precision="fp32_tc")
     m.load_state_dict(seeded_state_dict(manifest_template("bisenetformer_l_ade"), 0), strict=True)
     eng = m.engine()
-    assert eng.pair_capable()
     H, W = (int(v) for v in g["sizes"][0])
     taken = [eng._pair_block_ok(blk, H // (8 << si), W // (8 << si)) for si, stage in enumerate(eng.blocks) for blk in stage]
     assert sum(taken) >= 6 and not any(t for t, blk in zip(taken, [b for st in eng.blocks for b in st]) if blk["stride"] == 2)
     imgs = synth_images(4, [tuple(s) for s in g["sizes"].tolist()])
     x = torch.stack([torch.from_numpy(im).permute(2, 0, 1).float() for im in imgs])
     taps = {}
+    ops._backend = calls = ConvCalls(ops._backend)
     out = m(x, taps=taps)
+    pair_convs = [c for t, blk in zip(taken, [b for st in eng.blocks for b in st]) if t for c in blk["convs"]]
+    paired = {id(w) for w in calls.w["conv2d_pair"]}
+    assert all(id(c.w3) in paired for c in pair_convs)
+    assert not any(c.w is w or c.w3 is w for c in pair_convs for w in calls.w["conv2d"])
     assert np.abs(taps["cp32"].permute(0, 3, 1, 2)[:, ::16].numpy() - g["cp32_tap"]).max() <= 1e-4 * np.abs(g["cp32_tap"]).max()
     assert np.abs(out.logits.numpy() - g["logits"]).max() <= 1e-3
     assert np.abs(out.masks[:, ::10, ::4, ::4].numpy() - g["masks_q10_s4"]).max() <= 1e-3

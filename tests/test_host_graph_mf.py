@@ -13,7 +13,7 @@ from focoos_b200.processor import MaskFormerProcessor
 from focoos_b200.utils.seeded_weights import seeded_state_dict
 from oracle.gen_golden import state_dict_digest, synth_images
 from oracle.ops_ref import RefBackend
-from tests.parity_utils import GOLDEN, load_golden, manifest_template
+from tests.parity_utils import GOLDEN, ConvCalls, load_golden, manifest_template
 
 
 @pytest.fixture()
@@ -73,16 +73,21 @@ def test_mf_fused_graph_matches_golden(ref_backend):
         assert np.allclose([d.conf for d in a_.detections], [d.conf for d in b_.detections], rtol=1e-6)
 
 
-def test_mf_pair_native_backbone_host_logic(ref_backend):
+def test_mf_pair_backbone_runs_as_pair_convs(ref_backend):
     """precision="fp32_tc": the ResNet backbone runs in the pair format (fp16 hi/lo planes between convs, DetrEngine._run_backbone_pair) and the four pixel-decoder
     convs read the pairs - host-side bookkeeping on the CPU references: same outputs as the fp32 graph up to the pair rounding (2^-22 relative per activation)."""
     g = load_golden("mf_l_coco_ins_b2_320x416")
     m = FAIMaskFormer(MaskFormerConfig(), precision="fp32_tc")
     m.load_state_dict(_sd(), strict=True)
-    assert m.engine().pair_capable()
     imgs = synth_images(3, [tuple(s) for s in g["sizes"].tolist()])
     x = torch.stack([torch.from_numpy(im).permute(2, 0, 1).float() for im in imgs])
     taps = {}
+    ops._backend = calls = ConvCalls(ops._backend)
     out = m(x, taps=taps)
+    eng = m.engine()
+    backbone = [eng.stem2, eng.stem3] + [blk[k] for st in eng.stages for blk in st for k in ("a", "b", "c", "short") if blk[k] is not None]
+    paired = {id(w) for w in calls.w["conv2d_pair"]}
+    assert all(id(c.w3) in paired for c in backbone + [eng.pd_in, *eng.adapter.values(), eng.layer[1], eng.mask_features])
+    assert not any(c.w is w or c.w3 is w for c in backbone for w in calls.w["conv2d"])
     assert np.abs(out.logits.numpy() - g["logits"]).max() <= 1e-3
     assert np.abs(out.masks[:, ::10, ::4, ::4].numpy() - g["masks_q10_s4"]).max() <= 2e-3
