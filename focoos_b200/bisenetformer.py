@@ -22,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .fai_detr import _bn_fold, _Conv, _CriterionStub, _packed_layers
+from .fai_detr import _bn_fold, _channels, _Conv, _CriterionStub, _packed_layers, _unpair
 from .fai_mf import MaskFormerModelOutput, MFEngine, PredictionHeads, _AttnLayer, _ConvBN, _FFNLayer, _SegmentationModel
 from .ports import ModelOutput
 
@@ -239,51 +239,33 @@ class BisenetEngine(MFEngine):
     def _gate(self, conv, vec):
         """tiny [B,C] GEMM(s) of the channel-attention gates, SIMT path (M = batch size)."""
         B, C = vec.shape
-        return conv(vec.reshape(B, 1, 1, C), algo=ops.ALGO_SIMT).reshape(B, -1)
+        return self._conv(conv, vec.reshape(B, 1, 1, C), algo=ops.ALGO_SIMT).reshape(B, -1)
 
-    def _cat_bottleneck(self, x, blk, first_in_pair=False):
-        A, dt = self.algo, self.dt
+    def _cat_bottleneck(self, x, blk):
+        """CatBottleneck, concat-free: each conv writes its channel slice of the block's output buffer, which the next conv reads in place.  A block that
+        _pair_block_ok takes keeps the buffer as a Pair (no split pass inside the block); a stride-2 block's first conv reads a Pair input and writes fp32."""
         c = blk["convs"]
         half = c[0].w.shape[0]
-        Cout = half * 2
         B, H, W, _ = x.shape
-        if first_in_pair and blk["stride"] != 2:  # a stride-1 block the pair path does not take: back to fp32 first
-            x, first_in_pair = x.float(), False
         if blk["stride"] == 2:
-            out1 = self._pc(c[0], x, out_pair=False) if first_in_pair else c[0](x, algo=A)
-            buf = torch.empty((B, (H - 1) // 2 + 1, (W - 1) // 2 + 1, Cout), dtype=dt, device=x.device)
+            out1 = self._conv(c[0], x)
+            buf = torch.empty((B, (H - 1) // 2 + 1, (W - 1) // 2 + 1, 2 * half), dtype=self.dt, device=x.device)
             ops.avgpool3x3s2(out1, out=buf[..., :half])
             src = ops.dwconv3x3s2(out1, *blk["avd"])
         else:
-            buf = torch.empty((B, H, W, Cout), dtype=dt, device=x.device)
-            c[0](x, out=buf[..., :half], algo=A)
-            src = buf[..., :half]
+            shape = (B, H, W, 2 * half)
+            buf = ops.Pair.empty(shape, x.device) if self._pair_block_ok(blk, H, W) else torch.empty(shape, dtype=self.dt, device=x.device)
+            src = self._conv(c[0], x, out=_channels(buf, 0, half))
         o = half
         for i in (1, 2, 3):
             w = c[i].w.shape[0]
-            c[i](src, out=buf[..., o:o + w], algo=A)
-            src = buf[..., o:o + w]
-            o += w
-        return buf
-
-    def _cat_bottleneck_pair(self, x, blk):
-        """stride-1 CatBottleneck in the pair format (fp32_tc): the four convs read and write fp16 [hi | lo] planes - each one's output is a channel slice of the block's
-        concat buffer and the next one's input - so no split pass runs inside the block.  x: Pair or fp32 tensor (split once) -> Pair"""
-        c = blk["convs"]
-        half = c[0].w.shape[0]
-        B, H, W, _ = x.shape
-        buf = ops.Pair.empty((B, H, W, 2 * half), x.device)
-        src = self._pc(c[0], x, out=buf.slice(0, half))
-        o = half
-        for i in (1, 2, 3):
-            w = c[i].w.shape[0]
-            src = self._pc(c[i], src, out=buf.slice(o, o + w))
+            src = self._conv(c[i], src, out=_channels(buf, o, o + w))
             o += w
         return buf
 
     def _pair_block_ok(self, blk, H, W) -> bool:
         """conv2d_pair takes the block: every conv has its weight triple; a 32-channel 3x3 input needs the halo mode (rows of at least 64 pixels, Cout <= 64)"""
-        if blk["stride"] != 1 or self.precision != "fp32_tc":
+        if blk["stride"] != 1 or not self.pair:
             return False
         for cv in blk["convs"]:
             cin, cout, k = cv.w.shape[3], cv.w.shape[0], cv.w.shape[1]
@@ -295,47 +277,39 @@ class BisenetEngine(MFEngine):
 
     @torch.no_grad()
     def forward(self, images: torch.Tensor, taps: Optional[dict] = None):
-        cfg, dt, A = self.cfg, self.dt, self.algo
+        cfg = self.cfg
         if images.dtype == torch.uint8:
             B, H, W, _ = images.shape
         else:
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
         # any H x W, like the reference (its processor does not resize): odd maps from the stride-2 convs and pools run on the same kernels
-        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, dt)
-        x = self.stem2(x, algo=A)  # res2
+        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, self.dt)
+        x = self._conv(self.stem2, x)  # res2
         feats = []
-        P = ops.Pair
-        as_f32 = lambda t: t.float() if isinstance(t, P) else t  # noqa: E731  (a torch op: only ever applied to the small 1/32-resolution map below)
         for stage in self.blocks:
             for blk in stage:
-                if self._pair_block_ok(blk, x.shape[1], x.shape[2]):
-                    x = self._cat_bottleneck_pair(x, blk)
-                elif isinstance(x, P):  # a stride-2 block after pair-native ones: its first conv reads the pair and writes fp32, the rest runs as before
-                    x = self._cat_bottleneck(x, blk, first_in_pair=True)
-                else:
-                    x = self._cat_bottleneck(x, blk)
+                x = self._cat_bottleneck(x, blk)
             feats.append(x)
         res3, res4, res5 = feats
-        res5 = as_f32(res5)  # global average pool + ARM gates work on fp32 (33 M elements at bs=64 1024x512)
-        pin = lambda conv, f, **kw: (self._pc(conv, f, out_pair=False, **kw) if isinstance(f, P) else conv(f, algo=A, **kw))  # noqa: E731
-        # context path
+        res5 = _unpair(res5)  # global average pool + ARM gates work on fp32 (33 M elements at bs=64 1024x512)
+        # context path; the convs that read res4 / res3 take a Pair to fp32 themselves
         avg = self._gate(self.conv_avg, ops.global_avgpool(res5))
         a = self.arm["arm32"]
-        f = a["conv"](a["proj"](res5, algo=A), algo=A)
+        f = self._conv(a["conv"], self._conv(a["proj"], res5))
         f32 = ops.channel_scale(f, self._gate(a["att"], ops.global_avgpool(f)), addvec=avg)
-        up = self.head32(ops.resize_bilinear(f32, (res4.shape[1], res4.shape[2])), algo=A)
+        up = self._conv(self.head32, ops.resize_bilinear(f32, (res4.shape[1], res4.shape[2])))
         a = self.arm["arm16"]
-        f = a["conv"](pin(a["proj"], res4), algo=A)
+        f = self._conv(a["conv"], self._conv(a["proj"], res4))
         f16 = ops.channel_scale(f, self._gate(a["att"], ops.global_avgpool(f)), addt=up)
-        f8 = self.head16(ops.resize_bilinear(f16, (res3.shape[1], res3.shape[2])), algo=A)
+        f8 = self._conv(self.head16, ops.resize_bilinear(f16, (res3.shape[1], res3.shape[2])))
         # feature fusion
-        feat = self.ffm_blk(pin(self.ffm_p1, res3, residual=self.ffm_p2(f8, algo=A)), algo=A)
+        feat = self._conv(self.ffm_blk, self._conv(self.ffm_p1, res3, residual=self._conv(self.ffm_p2, f8)))
         att = self._gate(self.ffm_c2, self._gate(self.ffm_c1, ops.global_avgpool(feat)))
         fuse = ops.channel_scale(feat, att, self_add=True)
-        mask_features = self.conv_out(fuse, algo=A)
+        mask_features = self._conv(self.conv_out, fuse)
         if taps is not None:
-            taps.update(res3=as_f32(res3), res4=as_f32(res4), res5=res5, cp32=f32, cp16=f16, cp8=f8, mask_features=mask_features)
+            taps.update(res3=_unpair(res3), res4=_unpair(res4), res5=res5, cp32=f32, cp16=f16, cp8=f8, mask_features=mask_features)
         return self._run_decoder([f32, f16], mask_features, B, H, W, taps)
 
 

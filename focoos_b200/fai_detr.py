@@ -231,50 +231,36 @@ def _split3_weights(w):
     return torch.cat([hi, lo, hi], dim=-1).contiguous()
 
 
-def _split3_ok(x, w3, act, algo):
-    a = (act & 15)
-    return w3 is not None and algo != ops.ALGO_SIMT and x.dtype == torch.float32 and a not in (ops.ACT_GELU, 4) and (x.numel() // x.shape[-1]) >= 64
-
-
 class _Conv:
-    """Packed conv/linear: weight [Cout,KH,KW,Cin] in activation dtype, fp32 scale/bias (folded BN).
-    `w3` (precision="fp32_tc"): the [W_hi|W_lo|W_hi] fp16 triple for the split-precision tensor-core path on fp32 activations."""
+    """Packed conv: weight [Cout,KH,KW,Cin] in activation dtype, fp32 scale/bias (folded BN).
+    `w3` (precision="fp32_tc"): the [W_hi|W_lo|W_hi] fp16 triple of the pair flow's tensor-core products.  Run by DetrEngine._conv."""
 
     __slots__ = ("w", "scale", "bias", "stride", "pad", "act", "w3")
 
     def __init__(self, w, scale, bias, stride=1, pad=0, act=ops.ACT_NONE):
         self.w, self.scale, self.bias, self.stride, self.pad, self.act, self.w3 = w, scale, bias, stride, pad, act, None
 
-    def enable_split3(self, host_w3=None):
-        if self.w.dtype == torch.float32 and self.w.shape[-1] % 32 == 0:
-            self.w3 = host_w3.get(id(self.w)) if host_w3 else None
-            if self.w3 is None:
-                self.w3 = _split3_weights(self.w)
-
-    def __call__(self, x, residual=None, out=None, out_dtype=None, act=None, algo=ops.ALGO_AUTO):
-        act = self.act if act is None else act
-        if _split3_ok(x, self.w3, act, algo) and (out_dtype in (None, torch.float32)):
-            return ops.conv2d(ops.split_pair(x), self.w3, self.scale, self.bias, stride=self.stride, pad=self.pad, act=act, residual=residual, out=out,
-                              out_dtype=torch.float32, algo=ops.ALGO_TCGEN05_SPLIT3)
-        return ops.conv2d(x, self.w, self.scale, self.bias, stride=self.stride, pad=self.pad, act=act, residual=residual, out=out, out_dtype=out_dtype, algo=algo)
-
 
 class _Linear:
+    """Packed linear: weight [N,K] in activation dtype, fp32 bias, `w3` as in _Conv.  Run by DetrEngine._linear."""
+
     __slots__ = ("w", "bias", "w3")
 
     def __init__(self, w, bias):
         self.w, self.bias, self.w3 = w, bias, None
 
-    def enable_split3(self, host_w3=None):
-        if self.w.dtype == torch.float32 and self.w.shape[-1] % 32 == 0:
-            self.w3 = host_w3.get(id(self.w)) if host_w3 else None
-            if self.w3 is None:
-                self.w3 = _split3_weights(self.w)
 
-    def __call__(self, x, act=ops.ACT_NONE, residual=None, out_dtype=None, out=None, algo=ops.ALGO_AUTO):
-        if _split3_ok(x, self.w3, act, algo) and (out_dtype in (None, torch.float32)):
-            return ops.linear(ops.split_pair(x), self.w3, self.bias, act=act, residual=residual, out_dtype=torch.float32, out=out, algo=ops.ALGO_TCGEN05_SPLIT3)
-        return ops.linear(x, self.w, self.bias, act=act, residual=residual, out_dtype=out_dtype, out=out, algo=algo)
+def _unpair(t):
+    """a Pair as its fp32 values (a torch op: taps and the small 1/32 map of BisenetFormer's context path), any tensor as it is"""
+    return t.float() if isinstance(t, ops.Pair) else t
+
+
+def _channels(t, a, b):
+    """channels [a, b) of an NHWC activation buffer (a tensor view or a Pair slice): concat-free blocks write their branches into them"""
+    return t.slice(a, b) if isinstance(t, ops.Pair) else t[..., a:b]
+
+
+_PAIR_MIN_ROWS = 64  # fp32_tc: an fp32 operand with fewer rows (MaskFormer's 1/32 encoder below ~256x256 input) stays on the CUDA-core fp32 kernel
 
 
 def _packed_layers(obj, seen=None):
@@ -303,23 +289,27 @@ class DetrEngine:
 
     precision "fp16" / "fp32": activations in that dtype; `algo` goes to every conv / linear (ALGO_SIMT: the CUDA-core kernels).
     precision "fp32_tc": the pair flow - fp32 storage, every conv / linear of the flow three fp16 tensor-core products on activations kept as fp16 [hi | lo]
-    planes between them (`_pc` / `_plin`); it runs only with the default algorithm choice."""
+    planes between them; it runs only with the default algorithm choice.  `_conv` / `_linear` pick the kernel of every layer."""
 
     def __init__(self, sd: Dict[str, torch.Tensor], cfg, device, precision: str = "fp16", algo: int = ops.ALGO_AUTO):
         assert precision in ("fp32", "fp16", "fp32_tc")
         if precision == "fp32_tc" and algo != ops.ALGO_AUTO:
             raise ValueError(f"focoos_b200: precision 'fp32_tc' runs the tensor-core pair flow and takes no other algorithm (got algo={algo})")
         self.cfg, self.device, self.precision, self.algo = cfg, torch.device(device), precision, algo
+        self.pair = precision == "fp32_tc"
         self.dt = torch.float16 if precision == "fp16" else torch.float32
         self._consts = {}  # per-resolution constants (_constants, MFEngine._pos)
-        self._host_w3 = {} if precision == "fp32_tc" else None  # id(packed device weight) -> [W_hi|W_lo|W_hi] split on the host in _to()
+        self._host_w3 = {} if self.pair else None  # id(packed device weight) -> [W_hi|W_lo|W_hi] split on the host in _to()
         # pack on the HOST (BN folding, re-parameterisation, concatenations are a few hundred tiny tensor ops: as device launches they were ~700 `at::`
         # kernels in front of the first forward); only the packed tensors travel to the device
         sd = {k: v.detach().to("cpu") for k, v in sd.items()}
         self._pack(sd)
-        if precision == "fp32_tc":
+        if self.pair:
             for layer in _packed_layers(vars(self)):
-                layer.enable_split3(self._host_w3)
+                if layer.w.dtype == torch.float32 and layer.w.shape[-1] % 32 == 0:
+                    layer.w3 = self._host_w3.get(id(layer.w))
+                    if layer.w3 is None:
+                        layer.w3 = _split3_weights(layer.w)
             assert all(layer.w3 is not None for layer in self._pair_layers()), "fp32_tc: a layer of the pair flow has no [W_hi|W_lo|W_hi] weight triple"
         self._host_w3 = None
 
@@ -391,19 +381,55 @@ class DetrEngine:
             self.stages.append(blocks)
 
     def _run_backbone(self, images):
-        """-> [res2, res3, res4, res5] NHWC (nn/backbone/resnet.py:252-266)."""
-        cfg, dt, A = self.cfg, self.dt, self.algo
-        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, dt)
-        x = self.stem3(self.stem2(x, algo=A), algo=A)
+        """-> [res2, res3, res4, res5] NHWC (nn/backbone/resnet.py:252-266): Pairs under fp32_tc (shared by every model family with this backbone)."""
+        cfg = self.cfg
+        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, self.dt, out_pair=self.pair)
+        x = self._conv(self.stem3, self._conv(self.stem2, x, out_pair=True), out_pair=True)
         x = ops.maxpool3x3s2(x)
         feats = []
         for blocks in self.stages:
             for blk in blocks:
-                y = blk["b"](blk["a"](x, algo=A), algo=A)
-                short = x if blk["short"] is None else blk["short"](ops.avgpool2x2(x) if blk["stride"] == 2 else x, algo=A)
-                x = blk["c"](y, residual=short, algo=A)
+                y = self._conv(blk["b"], self._conv(blk["a"], x, out_pair=True), out_pair=True)
+                short = x if blk["short"] is None else self._conv(blk["short"], ops.avgpool2x2(x) if blk["stride"] == 2 else x, out_pair=True)
+                x = self._conv(blk["c"], y, residual=short, out_pair=True)
             feats.append(x)
         return feats
+
+    # ---- the layer call: the one place that picks a conv / linear kernel from the precision and the operand's format ---------------------------------
+    def _on_pairs(self, layer, x, algo, out_pair):
+        """fp32_tc: whether the layer runs as three fp16 tensor-core products on the pair planes of x (conv2d_pair) rather than on the fp32 CUDA cores.
+        A Pair operand or a Pair result can only take the products.  An fp32 operand with an fp32 result stays on the CUDA cores when the call asks for
+        ALGO_SIMT (the [B,C] gates, the MaskFormer classifier), when the layer has no weight triple, or when it has fewer than _PAIR_MIN_ROWS rows."""
+        if not self.pair:
+            return False
+        if isinstance(x, ops.Pair) or out_pair:
+            return True
+        return algo != ops.ALGO_SIMT and layer.w3 is not None and x.numel() // x.shape[-1] >= _PAIR_MIN_ROWS
+
+    def _conv(self, conv, x, *, act=None, residual=None, out=None, out_dtype=None, algo=None, out_pair=False):
+        """one packed conv.  fp16 / fp32: ops.conv2d on the storage weight with `algo` (default self.algo).  fp32_tc (see _on_pairs): ops.conv2d_pair on
+        the weight triple - x a Pair or split into one - whose result is a Pair with out_pair=True or a Pair `out`, else fp32.  The storage flow ignores
+        out_pair.  The residual has the result's format."""
+        act = conv.act if act is None else act
+        algo = self.algo if algo is None else algo
+        if self._on_pairs(conv, x, algo, out_pair or isinstance(out, ops.Pair)):
+            assert act & 15 not in (ops.ACT_GELU, ops.ACT_SIGMOID), "no layer of the pair flow has a GELU / sigmoid epilogue"
+            return ops.conv2d_pair(ops.to_pair(x), conv.w3, conv.scale, conv.bias, stride=conv.stride, pad=conv.pad, act=act, residual=residual, out=out,
+                                   out_pair=out_pair)
+        return ops.conv2d(x, conv.w, conv.scale, conv.bias, stride=conv.stride, pad=conv.pad, act=act, residual=residual, out=out, out_dtype=out_dtype, algo=algo)
+
+    def _linear(self, lin, x, *, act=ops.ACT_NONE, residual=None, out=None, out_dtype=None, algo=None, out_pair=False):
+        """one packed linear on tokens [..., K]: ops.linear, or under fp32_tc ops.linear_pair, chosen as in _conv.  `out` may be a column slice of a wider
+        fp32 buffer."""
+        algo = self.algo if algo is None else algo
+        if self._on_pairs(lin, x, algo, out_pair):
+            assert act & 15 not in (ops.ACT_GELU, ops.ACT_SIGMOID), "no layer of the pair flow has a GELU / sigmoid epilogue"
+            return ops.linear_pair(ops.to_pair(x), lin.w3, lin.bias, act=act, residual=residual, out=out, out_pair=out_pair)
+        return ops.linear(x, lin.w, lin.bias, act=act, residual=residual, out=out, out_dtype=out_dtype, algo=algo)
+
+    def _empty(self, shape, device):
+        """an activation buffer of the flow: a Pair under fp32_tc, else a tensor in the storage dtype"""
+        return ops.Pair.empty(shape, device) if self.pair else torch.empty(shape, dtype=self.dt, device=device)
 
     def _pack(self, sd):
         cfg = self.cfg
@@ -468,49 +494,26 @@ class DetrEngine:
     def _csp_run(self, packed, cat, out=None):
         both, reps = packed
         C = both.w.shape[0] // 2
-        y12 = both(cat, algo=self.algo)
-        x = y12[..., :C]
+        y12 = self._conv(both, cat, out_pair=True)
+        x = _channels(y12, 0, C)
         for i, r in enumerate(reps):
             last = i == len(reps) - 1
-            x = r(x, residual=y12[..., C:] if last else None, act=(ops.ACT_SILU | 16) if last else None, out=out if last else None, algo=self.algo)
+            x = self._conv(r, x, residual=_channels(y12, C, 2 * C) if last else None, act=(ops.ACT_SILU | 16) if last else None, out=out if last else None,
+                           out_pair=True)
         return x
 
     def _mha(self, blk, x, pos):
         """post-norm self-attention block: LN(x + out_proj(attn(q=k=x+pos, v=x)))."""
         B, L, d = x.shape
-        qk = blk["qk"](ops.add(x, pos), algo=self.algo)
-        v = blk["v"](x, algo=self.algo)
+        qk = self._linear(blk["qk"], ops.add(x, pos))
+        v = self._linear(blk["v"], x)
         a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, 1.0 / math.sqrt(d // self.nhead))
-        y = blk["out"](a, residual=x, algo=self.algo)
+        y = self._linear(blk["out"], a, residual=x)
         return ops.layernorm(y, *blk["n_attn"])
 
     def _ffn(self, blk, x, act):
-        f = blk["l2"](blk["l1"](x, act=act, algo=self.algo), residual=x, algo=self.algo)
+        f = self._linear(blk["l2"], self._linear(blk["l1"], x, act=act), residual=x)
         return ops.layernorm(f, *blk["n_ffn"])
-
-    # ---- pair-native fp32_tc path: conv activations stay in the fp16 [hi | lo] pair format between convs (written by the conv epilogue), so the split kernel
-    # only runs where a non-conv operator (LayerNorm, attention, selection) produced fp32 --------------------------------------------------------------
-    def _pc(self, conv, x, residual=None, out=None, out_pair=True, act=None):
-        """packed _Conv on a pair-format input (an fp32 tensor is split first) -> Pair, or fp32 tensor with out_pair=False"""
-        return ops.conv2d_pair(ops.to_pair(x), conv.w3, conv.scale, conv.bias, stride=conv.stride, pad=conv.pad, act=conv.act if act is None else act,
-                               residual=residual, out=out, out_pair=out_pair)
-
-    def _plin(self, lin, xp: "ops.Pair", act=ops.ACT_NONE, residual=None, out_pair=False, out=None):
-        """packed _Linear on pair-format tokens [B,S,K] -> fp32 [B,S,N] (+ fp32 residual), or a Pair [B,S,N] with out_pair=True.
-        `out`: an fp32 [B,S,>=N] buffer whose first N columns receive the result (row pitch = its last dimension)"""
-        buf = xp.buf
-        assert buf.is_contiguous() and xp.c0 == 0 and xp.C == xp.Ctot
-        lead = buf.shape[:-1]
-        x4 = ops.Pair(buf.reshape(1, 1, -1, buf.shape[-1]))
-        N = lin.w3.shape[0]
-        w4 = lin.w3.reshape(N, 1, 1, lin.w3.shape[-1])
-        if out_pair:
-            y = ops.conv2d_pair(x4, w4, None, lin.bias, act=act, out_pair=True)
-            return ops.Pair(y.buf.reshape(*lead, 2 * N))
-        r4 = None if residual is None else residual.reshape(1, 1, -1, N)
-        o4 = None if out is None else out.reshape(1, 1, -1, out.shape[-1])[..., :N]
-        y = ops.conv2d_pair(x4, w4, None, lin.bias, act=act, residual=r4, out=o4, out_pair=False)
-        return y.reshape(*lead, N) if out is None else out[..., :N]
 
     # fused row glue (csrc/head_fused.cu): LayerNorm / positional add / GELU / gather / mask kernels write the pair operand of the next tensor-core linear themselves
     # (and attention / deformable attention write pair rows), so no split_f32_pair / add / row_select launch remains in the AIFI, selection and decoder chains
@@ -518,88 +521,69 @@ class DetrEngine:
         """AIFI encoder layer (nn/layers/transformer.py:583-601, post-norm, GELU) on fp32 tokens [B,L,d] -> (fp32 tokens, their Pair)"""
         blk, d = self.aifi, src.shape[-1]
         sp, spp = ops.split_pair_ex(src, pos=pos, want_pair=True, want_pair_pos=True)
-        qk = self._plin(blk["qk"], spp)
-        v = self._plin(blk["v"], sp)
+        qk = self._linear(blk["qk"], spp)
+        v = self._linear(blk["v"], sp)
         a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, 1.0 / math.sqrt(d // self.nhead), split=True, out_pair=True)
-        y = self._plin(blk["out"], a, residual=src)
+        y = self._linear(blk["out"], a, residual=src)
         x1, x1p, _ = ops.layernorm_ex(y, *blk["n_attn"])
-        h = self._plin(blk["l1"], x1p)
+        h = self._linear(blk["l1"], x1p)
         hp, _ = ops.split_pair_ex(h, act=ops.ACT_GELU)
-        y = self._plin(blk["l2"], hp, residual=x1)
+        y = self._linear(blk["l2"], hp, residual=x1)
         x2, x2p, _ = ops.layernorm_ex(y, *blk["n_ffn"])
         return x2, x2p
 
-    def _csp_run_pair(self, packed, cat, out=None):
-        both, reps = packed
-        C = both.w.shape[0] // 2
-        y12 = self._pc(both, cat)
-        x = y12.slice(0, C)
-        for i, r in enumerate(reps):
-            last = i == len(reps) - 1
-            x = self._pc(r, x, residual=y12.slice(C, 2 * C) if last else None, act=(ops.ACT_SILU | 16) if last else None, out=out if last else None)
-        return x
-
-    def _run_backbone_pair(self, images):
-        """ResNet-vd in the pair format -> [res2, res3, res4, res5] as Pairs (nn/backbone/resnet.py:252-266); shared by every model family with this backbone"""
+    def _trunk(self, images, taps):
+        """backbone + hybrid encoder + decoder input projection -> (memory [B,S,d] - a Pair under fp32_tc, else in the storage dtype -, shapes, constants)"""
         cfg = self.cfg
-        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, out_pair=True)
-        x = self._pc(self.stem3, self._pc(self.stem2, x))
-        x = ops.pair_maxpool3x3s2(x)
-        feats = []
-        for blocks in self.stages:
-            for blk in blocks:
-                y = self._pc(blk["b"], self._pc(blk["a"], x))
-                short = x if blk["short"] is None else self._pc(blk["short"], ops.pair_avgpool2x2(x) if blk["stride"] == 2 else x)
-                x = self._pc(blk["c"], y, residual=short)
-            feats.append(x)
-        return feats
-
-    def _forward_pair_trunk(self, images, taps):
-        """backbone + hybrid encoder + decoder input projection in the pair format -> (memory Pair [B,S,d], shapes, constants)"""
-        cfg = self.cfg
-        P = ops.Pair
-        feats = self._run_backbone_pair(images)
-        res3, res4, res5 = feats[1], feats[2], feats[3]
+        _, res3, res4, res5 = self._run_backbone(images)
         B, h32, w32, _ = res5.shape
         K = self._constants(h32, w32)
         C = cfg.pixel_decoder_feat_dim
         dev = images.device
-        cat1 = P.empty((B, h32 * 2, w32 * 2, 2 * C), dev)  # [up(lat0) | proj(res4)]
-        cat2 = P.empty((B, h32 * 4, w32 * 4, 2 * C), dev)  # [up(lat1) | proj(res3)]
-        cat3 = P.empty((B, h32 * 2, w32 * 2, 2 * C), dev)  # [down(fpn1) | lat1]
-        cat4 = P.empty((B, h32, w32, 2 * C), dev)          # [down(pan0) | lat0]
-        self._pc(self.enc_in[0], res3, out=cat2.slice(C, 2 * C))
-        self._pc(self.enc_in[1], res4, out=cat1.slice(C, 2 * C))
-        p5 = self._pc(self.enc_in[2], res5, out_pair=False)          # fp32 tokens for the AIFI block (LayerNorm / attention work on fp32)
-        src, src_p = self._aifi_pair(p5.reshape(B, h32 * w32, C), K["pos"])
+        cat1 = self._empty((B, h32 * 2, w32 * 2, 2 * C), dev)  # [up(lat0) | proj(res4)]
+        cat2 = self._empty((B, h32 * 4, w32 * 4, 2 * C), dev)  # [up(lat1) | proj(res3)]
+        cat3 = self._empty((B, h32 * 2, w32 * 2, 2 * C), dev)  # [down(fpn1) | lat1]
+        cat4 = self._empty((B, h32, w32, 2 * C), dev)          # [down(pan0) | lat0]
+        self._conv(self.enc_in[0], res3, out=_channels(cat2, C, 2 * C))
+        self._conv(self.enc_in[1], res4, out=_channels(cat1, C, 2 * C))
+        src = self._conv(self.enc_in[2], res5).reshape(B, h32 * w32, C)  # tokens for the AIFI block: fp32 in the pair flow (LayerNorm / attention work on fp32)
+        # AIFI (modelling.py:315-324)
+        if self.pair:
+            src, src_p = self._aifi_pair(src, K["pos"])
+        else:
+            src = self._ffn(self.aifi, self._mha(self.aifi, src, K["pos"]), ops.ACT_GELU)
         p5 = src.reshape(B, h32, w32, C)
-        lat0 = self._pc(self.lateral[0], P(src_p.buf.reshape(B, h32, w32, 2 * C)), out=cat4.slice(C, 2 * C))
-        ops.pair_resize_bilinear(lat0, (h32 * 2, w32 * 2), out=cat1.slice(0, C))
-        fpn0 = self._csp_run_pair(self.fpn[0], cat1)
-        lat1 = self._pc(self.lateral[1], fpn0, out=cat3.slice(C, 2 * C))
-        ops.pair_resize_bilinear(lat1, (h32 * 4, w32 * 4), out=cat2.slice(0, C))
-        fpn1 = self._csp_run_pair(self.fpn[1], cat2)
-        self._pc(self.down[0], ops.pair_resize_bilinear(fpn1, (h32 * 2, w32 * 2)), out=cat3.slice(0, C))
-        pan0 = self._csp_run_pair(self.pan[0], cat3)
-        self._pc(self.down[1], ops.pair_resize_bilinear(pan0, (h32, w32)), out=cat4.slice(0, C))
-        pan1 = self._csp_run_pair(self.pan[1], cat4)
-        enc_outs = [pan1, pan0, fpn1]
+        lat_in = ops.Pair(src_p.buf.reshape(B, h32, w32, 2 * C)) if self.pair else p5  # the pair flow's conv reads the pair its LayerNorm wrote
+        # top-down FPN (modelling.py:328-336)
+        lat0 = self._conv(self.lateral[0], lat_in, out=_channels(cat4, C, 2 * C))
+        ops.resize_bilinear(lat0, (h32 * 2, w32 * 2), out=_channels(cat1, 0, C))
+        fpn0 = self._csp_run(self.fpn[0], cat1)
+        lat1 = self._conv(self.lateral[1], fpn0, out=_channels(cat3, C, 2 * C))
+        ops.resize_bilinear(lat1, (h32 * 4, w32 * 4), out=_channels(cat2, 0, C))
+        fpn1 = self._csp_run(self.fpn[1], cat2)
+        # bottom-up PAN (modelling.py:338-345)
+        self._conv(self.down[0], ops.resize_bilinear(fpn1, (h32 * 2, w32 * 2)), out=_channels(cat3, 0, C))
+        pan0 = self._csp_run(self.pan[0], cat3)
+        self._conv(self.down[1], ops.resize_bilinear(pan0, (h32, w32)), out=_channels(cat4, 0, C))
+        pan1 = self._csp_run(self.pan[1], cat4)
+        enc_outs = [pan1, pan0, fpn1]  # outs[::-1] (modelling.py:347): 1/32, 1/16, 1/8
         if taps is not None:
-            taps.update(res3=res3.float(), res4=res4.float(), res5=res5.float(), aifi=p5, fpn0=fpn0.float(), fpn1=fpn1.float(), pan0=pan0.float(), pan1=pan1.float())
+            taps.update(res3=_unpair(res3), res4=_unpair(res4), res5=_unpair(res5), aifi=p5, fpn0=_unpair(fpn0), fpn1=_unpair(fpn1), pan0=_unpair(pan0),
+                        pan1=_unpair(pan1))
+        # predictor: memory [B, S, d] (modelling.py:1145-1167), each level written in place
         shapes = K["shapes"]
-        S = sum(h * w for h, w in shapes)
-        d = self.d
-        membuf = torch.empty((B, S, 2 * d), dtype=torch.float16, device=dev)
+        memory = self._empty((B, sum(h * w for h, w in shapes), self.d), dev)
+        buf = memory.buf if self.pair else memory
         start = 0
         for i, (f, (h, w)) in enumerate(zip(enc_outs, shapes)):
-            self._pc(self.dec_in[i], f, out=P(membuf[:, start:start + h * w].unflatten(1, (h, w))))
+            lvl = buf[:, start:start + h * w].unflatten(1, (h, w))
+            self._conv(self.dec_in[i], f, out=ops.Pair(lvl) if self.pair else lvl)
             start += h * w
-        return P(membuf), shapes, K
+        return memory, shapes, K
 
     @torch.no_grad()
     def forward(self, images: torch.Tensor, taps: Optional[dict] = None):
         """images [B,3,H,W] fp32 0..255 (H,W multiples of 32) -> (scores [B,Q,C] fp32, boxes xyxy [B,Q,4] fp32)."""
-        cfg, dt, A = self.cfg, self.dt, self.algo
         if images.dtype == torch.uint8:  # [B,H,W,3] decoded images straight into the stem kernel
             assert images.dim() == 4 and images.shape[3] == 3
             B, H, W, _ = images.shape
@@ -610,57 +594,12 @@ class DetrEngine:
             # DETRProcessor resizes to im_size; the encoder buffers, anchors and positional constants are laid out for 1/8 and 1/16 maps of exactly 4x and
             # 2x the 1/32 map, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
             raise ValueError(f"focoos_b200: input size {H}x{W} is not a multiple of 32; resize/pad the image (e.g. ModelInfo.im_size) before the model")
-        if self.precision == "fp32_tc":
-            mem_pair, shapes, K = self._forward_pair_trunk(images, taps)
-            value_all = self._plin(self.value_all, mem_pair)
-            t = self._plin(self.enc_output, mem_pair)
-            return self._forward_head_pair(t, value_all, shapes, K, B, mem_pair.buf.shape[1], taps, mem_pair)
-        feats = self._run_backbone(images)
-        res3, res4, res5 = feats[1], feats[2], feats[3]
-        h32, w32 = res5.shape[1], res5.shape[2]
-        K = self._constants(h32, w32)
-        C = cfg.pixel_decoder_feat_dim
-        dev = images.device
-        cat1 = torch.empty((B, h32 * 2, w32 * 2, 2 * C), dtype=dt, device=dev)  # [up(lat0) | proj(res4)]
-        cat2 = torch.empty((B, h32 * 4, w32 * 4, 2 * C), dtype=dt, device=dev)  # [up(lat1) | proj(res3)]
-        cat3 = torch.empty((B, h32 * 2, w32 * 2, 2 * C), dtype=dt, device=dev)  # [down(fpn1) | lat1]
-        cat4 = torch.empty((B, h32, w32, 2 * C), dtype=dt, device=dev)          # [down(pan0) | lat0]
-        self.enc_in[0](res3, out=cat2[..., C:], algo=A)
-        self.enc_in[1](res4, out=cat1[..., C:], algo=A)
-        p5 = self.enc_in[2](res5, algo=A)
-        # AIFI (modelling.py:315-324)
-        src = p5.reshape(B, h32 * w32, C)
-        src = self._mha(self.aifi, src, K["pos"])
-        src = self._ffn(self.aifi, src, ops.ACT_GELU)
-        p5 = src.reshape(B, h32, w32, C)
-        # top-down FPN (modelling.py:328-336)
-        lat0 = self.lateral[0](p5, out=cat4[..., C:], algo=A)
-        ops.resize_bilinear(lat0, (h32 * 2, w32 * 2), out=cat1[..., :C])
-        fpn0 = self._csp_run(self.fpn[0], cat1)
-        lat1 = self.lateral[1](fpn0, out=cat3[..., C:], algo=A)
-        ops.resize_bilinear(lat1, (h32 * 4, w32 * 4), out=cat2[..., :C])
-        fpn1 = self._csp_run(self.fpn[1], cat2)
-        # bottom-up PAN (modelling.py:338-345)
-        self.down[0](ops.resize_bilinear(fpn1, (h32 * 2, w32 * 2)), out=cat3[..., :C], algo=A)
-        pan0 = self._csp_run(self.pan[0], cat3)
-        self.down[1](ops.resize_bilinear(pan0, (h32, w32)), out=cat4[..., :C], algo=A)
-        pan1 = self._csp_run(self.pan[1], cat4)
-        enc_outs = [pan1, pan0, fpn1]  # outs[::-1] (modelling.py:347): 1/32, 1/16, 1/8
-        if taps is not None:
-            taps.update(res3=res3, res4=res4, res5=res5, aifi=p5, fpn0=fpn0, fpn1=fpn1, pan0=pan0, pan1=pan1)
-        # predictor: memory [B, S, d] (modelling.py:1145-1167), each level written in place
-        shapes = K["shapes"]
-        S = sum(h * w for h, w in shapes)
-        d = self.d
-        memory = torch.empty((B, S, d), dtype=dt, device=dev)
-        start = 0
-        for i, (f, (h, w)) in enumerate(zip(enc_outs, shapes)):
-            self.dec_in[i](f, out=memory[:, start:start + h * w].unflatten(1, (h, w)), algo=A)
-            start += h * w
-        value_all = self.value_all(memory, algo=A)  # [B,S,6*d], layer i uses columns [i*d,(i+1)*d)
+        memory, shapes, K = self._trunk(images, taps)
+        value_all = self._linear(self.value_all, memory)  # [B,S,6*d], layer i uses columns [i*d,(i+1)*d)
         # query selection (modelling.py:1191-1232)
-        t = self.enc_output(memory, algo=A)
-        return self._forward_head(t, value_all, memory, shapes, K, B, S, taps)
+        t = self._linear(self.enc_output, memory)
+        head = self._forward_head_pair if self.pair else self._forward_head
+        return head(t, value_all, memory, shapes, K, B, memory.shape[1], taps)
 
     def _forward_head(self, t, value_all, memory, shapes, K, B, S, taps):
         """query selection + decoder + head on the encoder memory of the fp16 / fp32 flow (fp32_tc runs _forward_head_pair)"""
@@ -674,37 +613,38 @@ class DetrEngine:
             scores = ops.linear_rowmax(output_memory, self.enc_score.w, self.enc_score.bias)
         else:
             cls_buf = torch.empty((B, S, (ncls + 7) // 8 * 8), dtype=torch.float32, device=dev)
-            self.enc_score(output_memory, out=cls_buf[..., :ncls], algo=A)
+            self._linear(self.enc_score, output_memory, out=cls_buf[..., :ncls])
             scores = ops.rowmax(cls_buf[..., :ncls])
         _, topk_ind = ops.topk(scores, cfg.num_queries)
         tgt = ops.gather_rows(output_memory, topk_ind)
-        bb = self.enc_bbox[2](self.enc_bbox[1](self.enc_bbox[0](tgt, act=ops.ACT_RELU, algo=A), act=ops.ACT_RELU, algo=A), out_dtype=torch.float32, algo=A)
+        bb = self._linear(self.enc_bbox[2], self._linear(self.enc_bbox[1], self._linear(self.enc_bbox[0], tgt, act=ops.ACT_RELU), act=ops.ACT_RELU),
+                          out_dtype=torch.float32)
         ref_unact = ops.box_add_anchors(bb, K["anchors"], topk_ind)
         ref = ops.box_sigmoid(ref_unact)
         if taps is not None:
             taps.update(memory=memory, enc_scores=scores, topk_ind=topk_ind, target=tgt, ref_unact=ref_unact)
         # decoder (modelling.py:969-1020, eval: logits only from the last layer)
         for i, blk in enumerate(self.dec):
-            pos = self.qpos[1](self.qpos[0](ref, act=ops.ACT_RELU, out_dtype=dt, algo=ops.ALGO_SIMT), algo=A)
+            pos = self._linear(self.qpos[1], self._linear(self.qpos[0], ref, act=ops.ACT_RELU, out_dtype=dt, algo=ops.ALGO_SIMT))
             tgt = self._mha(blk, tgt, pos)
-            oa = blk["oa"](ops.add(tgt, pos), out_dtype=torch.float32, algo=A)
+            oa = self._linear(blk["oa"], ops.add(tgt, pos), out_dtype=torch.float32)
             c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, cfg_points(cfg), self.nhead, out_dtype=dt)
-            tgt = ops.layernorm(blk["cross_out"](c, residual=tgt, algo=A), *blk["n_cross"])
+            tgt = ops.layernorm(self._linear(blk["cross_out"], c, residual=tgt), *blk["n_cross"])
             tgt = self._ffn(blk, tgt, ops.ACT_RELU)
-            delta = blk["bbox"][2](blk["bbox"][1](blk["bbox"][0](tgt, act=ops.ACT_RELU, algo=A), act=ops.ACT_RELU, algo=A), out_dtype=torch.float32, algo=A)
+            bbox = blk["bbox"]
+            delta = self._linear(bbox[2], self._linear(bbox[1], self._linear(bbox[0], tgt, act=ops.ACT_RELU), act=ops.ACT_RELU), out_dtype=torch.float32)
             ref = ops.box_refine(delta, ref)
             if taps is not None:
                 taps[f"dec{i}_out"] = tgt
                 taps[f"dec{i}_ref"] = ref
-        logits = self.dec_score(tgt, out_dtype=torch.float32, algo=ops.ALGO_SIMT)  # [B,Q,C] contiguous
+        logits = self._linear(self.dec_score, tgt, out_dtype=torch.float32, algo=ops.ALGO_SIMT)  # [B,Q,C] contiguous
         if taps is not None:
             taps.update(pred_logits=logits, pred_boxes_cxcywh=ref)
         return ops.box_sigmoid(logits), ops.box_cxcywh_to_xyxy(ref)
 
-
-    def _forward_head_pair(self, t, value_all, shapes, K, B, S, taps, mem_pair):
+    def _forward_head_pair(self, t, value_all, memory, shapes, K, B, S, taps):
         """query selection + decoder + head of the fp32-accurate mode with the fused row glue: the same operators and arithmetic as _forward_head, ~18 launches per
-        decoder layer instead of 31.  t = enc_output.0(memory) BEFORE the valid-mask fill (modelling.py:1202-1207)."""
+        decoder layer instead of 31.  t = enc_output.0(memory) BEFORE the valid-mask fill (modelling.py:1202-1207); memory: the Pair."""
         cfg, d = self.cfg, self.d
         nq, ncls = cfg.num_queries, cfg.num_classes
         ln_w, ln_b = self.enc_output_ln
@@ -713,32 +653,32 @@ class DetrEngine:
         scores = ops.linear_rowmax_pair(om_pair, self.enc_score.w3, self.enc_score.bias)
         _, topk_ind = ops.topk(scores, nq)
         tgt, tgt_p, _ = ops.layernorm_ex(t, ln_w, ln_b, gather=topk_ind, valid=K["valid"], fill=self.enc_output.bias)
-        h = self._plin(self.enc_bbox[1], self._plin(self.enc_bbox[0], tgt_p, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True)
-        bb = self._plin(self.enc_bbox[2], h)
+        h = self._linear(self.enc_bbox[1], self._linear(self.enc_bbox[0], tgt_p, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True)
+        bb = self._linear(self.enc_bbox[2], h)
         ref_unact = ops.box_add_anchors(bb, K["anchors"], topk_ind)
         ref = ops.box_sigmoid(ref_unact)
         if taps is not None:
-            taps.update(memory=mem_pair.float(), enc_scores=scores, topk_ind=topk_ind, target=tgt, ref_unact=ref_unact)
+            taps.update(memory=memory.float(), enc_scores=scores, topk_ind=topk_ind, target=tgt, ref_unact=ref_unact)
         q0w, q0b = self.qpos[0].w, self.qpos[0].bias   # query_pos_head layer 0: fp32 [2d, 4]
         _, qp = ops.box_refine_qpos(None, ref, q0w, q0b)
         scale = 1.0 / math.sqrt(d // self.nhead)
         L = len(self.dec)
         for i, blk in enumerate(self.dec):
-            pos = self._plin(self.qpos[1], qp)
+            pos = self._linear(self.qpos[1], qp)
             _, tpp = ops.split_pair_ex(tgt, pos=pos, want_pair=False, want_pair_pos=True)
-            qk = self._plin(blk["qk"], tpp)
-            v = self._plin(blk["v"], tgt_p)
+            qk = self._linear(blk["qk"], tpp)
+            v = self._linear(blk["v"], tgt_p)
             a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, scale, split=True, out_pair=True)
-            y = self._plin(blk["out"], a, residual=tgt)
+            y = self._linear(blk["out"], a, residual=tgt)
             tgt, _, tpp = ops.layernorm_ex(y, *blk["n_attn"], pos=pos, want_pair=False, want_pair_pos=True)
-            oa = self._plin(blk["oa"], tpp)
+            oa = self._linear(blk["oa"], tpp)
             c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, cfg_points(cfg), self.nhead, out_pair=True)
-            y = self._plin(blk["cross_out"], c, residual=tgt)
+            y = self._linear(blk["cross_out"], c, residual=tgt)
             tgt, tgt_p, _ = ops.layernorm_ex(y, *blk["n_cross"])
-            y = self._plin(blk["l2"], self._plin(blk["l1"], tgt_p, act=ops.ACT_RELU, out_pair=True), residual=tgt)
+            y = self._linear(blk["l2"], self._linear(blk["l1"], tgt_p, act=ops.ACT_RELU, out_pair=True), residual=tgt)
             tgt, tgt_p, _ = ops.layernorm_ex(y, *blk["n_ffn"])
-            h = self._plin(blk["bbox"][1], self._plin(blk["bbox"][0], tgt_p, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True)
-            delta = self._plin(blk["bbox"][2], h)
+            h = self._linear(blk["bbox"][1], self._linear(blk["bbox"][0], tgt_p, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True)
+            delta = self._linear(blk["bbox"][2], h)
             last = i == L - 1
             ref, qp = ops.box_refine_qpos(delta, ref, None if last else q0w, None if last else q0b)
             if taps is not None:
@@ -746,7 +686,7 @@ class DetrEngine:
                 taps[f"dec{i}_ref"] = ref
         # class logits on the tensor cores into a 16-byte-padded row (TMA store pitch), then sigmoid into the dense [B,Q,C] scores
         lbuf = torch.empty((B, nq, (ncls + 3) // 4 * 4), dtype=torch.float32, device=t.device)
-        logits = self._plin(self.dec_score, tgt_p, out=lbuf)
+        logits = self._linear(self.dec_score, tgt_p, out=lbuf[..., :ncls])
         if taps is not None:
             taps.update(pred_logits=logits, pred_boxes_cxcywh=ref)
         return ops.sigmoid_rows(logits), ops.box_cxcywh_to_xyxy(ref)

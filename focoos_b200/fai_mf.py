@@ -274,20 +274,18 @@ class MFEngine(DetrEngine):
         mask_features: a Pair under fp32_tc (see _run_decoder)."""
         A, dt = self.algo, self.dt
         B, Q, d = out.shape
-        pair = self.precision == "fp32_tc"
-        if pair:  # LayerNorm writes the pair operand of the mask MLP, whose hidden layers stay in the pair format
+        if self.pair:  # LayerNorm writes the pair operand of the mask MLP, whose hidden layers stay in the pair format
             dn, dnp, _ = ops.layernorm_ex(out, *self.head_norm, want_f32=want_class)
-            cls = self.classifier(dn, out_dtype=torch.float32, algo=ops.ALGO_SIMT) if want_class else None
-            me = self._plin(self.mask_mlp[2], self._plin(self.mask_mlp[1], self._plin(self.mask_mlp[0], dnp, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True))
         else:
-            dn = ops.layernorm(out, *self.head_norm)
-            cls = self.classifier(dn, out_dtype=torch.float32, algo=ops.ALGO_SIMT) if want_class else None
-            me = self.mask_mlp[2](self.mask_mlp[1](self.mask_mlp[0](dn, act=ops.ACT_RELU, algo=A), act=ops.ACT_RELU, algo=A), algo=A)  # [B,Q,256]
+            dn = dnp = ops.layernorm(out, *self.head_norm)
+        cls = self._linear(self.classifier, dn, out_dtype=torch.float32, algo=ops.ALGO_SIMT) if want_class else None
+        mlp = self.mask_mlp
+        me = self._linear(mlp[2], self._linear(mlp[1], self._linear(mlp[0], dnp, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True))  # [B,Q,256]
         _, h4, w4, C = mask_features.shape
         Qp = (Q + 7) // 8 * 8
         masks = torch.zeros((B, h4, w4, Qp), dtype=dt, device=out.device)
         # einsum("bqc,bchw->bqhw"): a [h4*w4, C] x [C, Q] GEMM per image whose "weights" (the mask embeddings) differ per image - ONE launch
-        if pair:
+        if self.pair:
             # the same GEMM as three fp16 tensor-core products on the mask_features pair and the per-image embeddings as [W_hi | W_lo | W_hi] triples.
             # (On the CUDA-core fp32 kernel this product was a third of the parity-mode step: 16.9 of 50.4 ms at bs=16 800x800.)
             ops.conv2d_per_image(mask_features.buf, _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=masks[..., :Q], algo=ops.ALGO_TCGEN05_SPLIT3)
@@ -301,47 +299,40 @@ class MFEngine(DetrEngine):
 
     @torch.no_grad()
     def forward(self, images: torch.Tensor, taps: Optional[dict] = None):
-        cfg, dt, A = self.cfg, self.dt, self.algo
         if images.dtype == torch.uint8:
             B, H, W, _ = images.shape
         else:
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
         # any H x W, like the reference (its processor does not resize): odd maps from the stride-2 convs and ceil-mode pools run on the same kernels
-        pair = self.precision == "fp32_tc"
-        if pair:
-            # the backbone keeps its activations as fp16 [hi | lo] planes between convs (no split pass in front of every conv, DetrEngine._run_backbone_pair);
-            # the four pixel-decoder convs that consume res2..res5 read the pairs and write the fp32 tensors the transformer / FPN arithmetic below works on
-            res2, res3, res4, res5 = self._run_backbone_pair(images)
-            in_conv = lambda conv, f: self._pc(conv, f, out_pair=False)  # noqa: E731
-        else:
-            res2, res3, res4, res5 = self._run_backbone(images)
-            in_conv = lambda conv, f: conv(f, algo=A)  # noqa: E731
+        # fp32_tc: the backbone keeps its activations as fp16 [hi | lo] planes between convs (no split pass in front of every conv); the four pixel-decoder
+        # convs that consume res2..res5 read the pairs and write the fp32 tensors the transformer / FPN arithmetic below works on
+        res2, res3, res4, res5 = self._run_backbone(images)
         d, nh = self.d, self.nhead
         scale = 1.0 / math.sqrt(d // nh)
         # ---- pixel decoder (TransformerFPN.forward_features)
-        x = in_conv(self.pd_in, res5)
+        x = self._conv(self.pd_in, res5)
         h, w = x.shape[1], x.shape[2]
         pos = self._pos(h, w)
         src = x.reshape(B, h * w, d)
         for blk in self.enc:  # pre-norm encoder layer (nn/layers/transformer.py:583-601 with normalize_before)
             s2 = ops.layernorm(src, *blk["n_attn"])
-            qk = blk["qk"](ops.add(s2, pos), algo=A)
-            a = ops.attention(qk[..., :d], qk[..., d:], blk["v"](s2, algo=A), nh, scale, split=pair)
-            src = blk["out"](a, residual=src, algo=A)
+            qk = self._linear(blk["qk"], ops.add(s2, pos))
+            a = ops.attention(qk[..., :d], qk[..., d:], self._linear(blk["v"], s2), nh, scale, split=self.pair)
+            src = self._linear(blk["out"], a, residual=src)
             s2 = ops.layernorm(src, *blk["n_ffn"])
-            src = blk["l2"](blk["l1"](s2, act=ops.ACT_RELU, algo=A), residual=src, algo=A)
+            src = self._linear(blk["l2"], self._linear(blk["l1"], s2, act=ops.ACT_RELU), residual=src)
         src = ops.layernorm(src, *self.enc_norm)
-        y = self.layer[4](src.reshape(B, h, w, d), algo=A)
+        y = self._conv(self.layer[4], src.reshape(B, h, w, d))
         ms = [y]
         # fp32_tc: the 1/4-resolution layer feeds only the mask_features conv, whose output is only ever read as a tensor-core operand (the per-image mask product):
         # both stay in the pair format - no fp32 copy of the two largest activations of the pixel decoder, no split pass over them
         for idx, f in ((3, res4), (2, res3), (1, res2)):
-            u = ops.upsample_nearest_add(y, in_conv(self.adapter[idx], f))
-            y = self._pc(self.layer[idx], u) if (pair and idx == 1) else self.layer[idx](u, algo=A)
+            u = ops.upsample_nearest_add(y, self._conv(self.adapter[idx], f))
+            y = self._conv(self.layer[idx], u, out_pair=idx == 1)
             if len(ms) < 3:
                 ms.append(y)
-        mask_features = self._pc(self.mask_features, y) if pair else self.mask_features(y, algo=A)
+        mask_features = self._conv(self.mask_features, y, out_pair=True)
         if taps is not None:
             taps.update(res5=res5.float(), enc_memory=src.reshape(B, h, w, d), mask_features=mask_features.float(), multi_scale=ms)
         return self._run_decoder(ms, mask_features, B, H, W, taps)
@@ -349,18 +340,17 @@ class MFEngine(DetrEngine):
     def _run_decoder(self, ms, mask_features, B, H, W, taps=None):
         """MultiScaleMaskedTransformerDecoder.forward (fai_mf/modelling.py:467-550) + head + final upsample; `ms` = the decoder's
         feature levels (3 for fai_mf, 2 for bisenetformer)."""
-        cfg, A = self.cfg, self.algo
+        cfg = self.cfg
         d, nh = self.d, self.nhead
         scale = 1.0 / math.sqrt(d // nh)
         nl = len(ms)
-        pair = self.precision == "fp32_tc"
-        if pair:  # every _heads call reads mask_features as a Pair: MaskFormer's conv writes one, BisenetFormer's fp32 output is split once here
+        if self.pair:  # every _heads call reads mask_features as a Pair: MaskFormer's conv writes one, BisenetFormer's fp32 output is split once here
             assert mask_features.shape[-1] % 64 == 0, mask_features.shape
             mask_features = ops.to_pair(mask_features)
         srcs, kpos, sizes = [], [], []
         for i in range(nl):
             hh, ww = ms[i].shape[1], ms[i].shape[2]
-            s = self.dec_in[i](ms[i], algo=A).reshape(B, hh * ww, d)
+            s = self._conv(self.dec_in[i], ms[i]).reshape(B, hh * ww, d)
             srcs.append(s)
             kpos.append(ops.add(s, self._pos(hh, ww)))
             sizes.append((hh, ww))
@@ -369,48 +359,41 @@ class MFEngine(DetrEngine):
         qpos = self.query_embed
         L = len(self.dec)
         cls = None
-        if pair:
+        if self.pair:
             # masked cross-attention on the tensor cores (fb200_attention_masked_split): the per-level key / value inputs are split ONCE (they are the same for
             # the layers of a level) and the K / V projections run pair -> pair.  Fused row glue (csrc/head_fused.cu, the kernels of the fai-detr head): every
             # LayerNorm writes the pair operand(s) of the linears behind it - LN(x) and LN(x) + query_pos in one launch - and the FFN / mask-MLP hidden layers
             # stay in the pair format: no add / split launches between two tensor-core linears
             kpos_p, srcs_p = [ops.to_pair(t) for t in kpos], [ops.to_pair(t) for t in srcs]
-            _, masks, attn = self._heads(out, mask_features, sizes[0], False)
-            for i, blk in enumerate(self.dec):
-                lvl = i % nl
+        _, masks, attn = self._heads(out, mask_features, sizes[0], False)
+        for i, blk in enumerate(self.dec):
+            lvl = i % nl
+            if self.pair:
                 _, _, tq = ops.layernorm_ex(out, *blk["cn"], pos=qpos, want_f32=False, want_pair=False, want_pair_pos=True)
-                q = self._plin(blk["cq"], tq)
-                kk, vv = self._plin(blk["ck"], kpos_p[lvl], out_pair=True), self._plin(blk["cv"], srcs_p[lvl], out_pair=True)
+                q = self._linear(blk["cq"], tq)
+                kk, vv = self._linear(blk["ck"], kpos_p[lvl], out_pair=True), self._linear(blk["cv"], srcs_p[lvl], out_pair=True)
                 a = ops.attention_masked(q, kk, vv, attn[0], attn[1], nh, scale, split=True)
-                out = self._plin(blk["cout"], ops.to_pair(a), residual=out)
+                out = self._linear(blk["cout"], ops.to_pair(a), residual=out)
                 _, t2p, t2pp = ops.layernorm_ex(out, *blk["sn"], pos=qpos, want_f32=False, want_pair=True, want_pair_pos=True)
-                qk = self._plin(blk["sqk"], t2pp)
-                a = ops.attention(qk[..., :d], qk[..., d:], self._plin(blk["sv"], t2p), nh, scale, split=True, out_pair=True)
-                out = self._plin(blk["sout"], a, residual=out)
-                _, t2p, _ = ops.layernorm_ex(out, *blk["fn"], want_f32=False)
-                out = self._plin(blk["l2"], self._plin(blk["l1"], t2p, act=ops.ACT_RELU, out_pair=True), residual=out)
-                last = i == L - 1
-                cls, masks, attn = self._heads(out, mask_features, None if last else sizes[(i + 1) % nl], last)
-                if taps is not None:
-                    taps[f"dec{i}_out"] = out
-        else:
-            _, masks, attn = self._heads(out, mask_features, sizes[0], False)
-            for i, blk in enumerate(self.dec):
-                lvl = i % nl
+                qk = self._linear(blk["sqk"], t2pp)
+                a = ops.attention(qk[..., :d], qk[..., d:], self._linear(blk["sv"], t2p), nh, scale, split=True, out_pair=True)
+                out = self._linear(blk["sout"], a, residual=out)
+                _, ffn_in, _ = ops.layernorm_ex(out, *blk["fn"], want_f32=False)
+            else:
                 t2 = ops.layernorm(out, *blk["cn"])
-                q = blk["cq"](ops.add(t2, qpos), algo=A)
-                a = ops.attention_masked(q, blk["ck"](kpos[lvl], algo=A), blk["cv"](srcs[lvl], algo=A), attn[0], attn[1], nh, scale)
-                out = blk["cout"](a, residual=out, algo=A)
+                q = self._linear(blk["cq"], ops.add(t2, qpos))
+                a = ops.attention_masked(q, self._linear(blk["ck"], kpos[lvl]), self._linear(blk["cv"], srcs[lvl]), attn[0], attn[1], nh, scale)
+                out = self._linear(blk["cout"], a, residual=out)
                 t2 = ops.layernorm(out, *blk["sn"])
-                qk = blk["sqk"](ops.add(t2, qpos), algo=A)
-                a = ops.attention(qk[..., :d], qk[..., d:], blk["sv"](t2, algo=A), nh, scale)
-                out = blk["sout"](a, residual=out, algo=A)
-                t2 = ops.layernorm(out, *blk["fn"])
-                out = blk["l2"](blk["l1"](t2, act=ops.ACT_RELU, algo=A), residual=out, algo=A)
-                last = i == L - 1
-                cls, masks, attn = self._heads(out, mask_features, None if last else sizes[(i + 1) % nl], last)
-                if taps is not None:
-                    taps[f"dec{i}_out"] = out
+                qk = self._linear(blk["sqk"], ops.add(t2, qpos))
+                a = ops.attention(qk[..., :d], qk[..., d:], self._linear(blk["sv"], t2), nh, scale)
+                out = self._linear(blk["sout"], a, residual=out)
+                ffn_in = ops.layernorm(out, *blk["fn"])
+            out = self._linear(blk["l2"], self._linear(blk["l1"], ffn_in, act=ops.ACT_RELU, out_pair=True), residual=out)
+            last = i == L - 1
+            cls, masks, attn = self._heads(out, mask_features, None if last else sizes[(i + 1) % nl], last)
+            if taps is not None:
+                taps[f"dec{i}_out"] = out
         if taps is not None:
             taps.update(pred_logits=cls, pred_masks=masks)  # masks: NHWC [B,h4,w4,Qp] pre-sigmoid logits
         probs = ops.softmax_drop_last(cls)

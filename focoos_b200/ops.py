@@ -783,68 +783,75 @@ def image_resize(images, size: Tuple[int, int]):
     return out
 
 
-def pair_maxpool3x3s2(x: Pair) -> Pair:
-    B, H, W, C = x.shape
-    out = Pair.empty((B, (H - 1) // 2 + 1, (W - 1) // 2 + 1, C), x.device)
-    _be().pair_pool(0, x, out)
-    return out
-
-
-def pair_avgpool2x2(x: Pair) -> Pair:
-    B, H, W, C = x.shape
-    out = Pair.empty((B, (H + 1) // 2, (W + 1) // 2, C), x.device)
-    _be().pair_pool(1, x, out)
-    return out
-
-
-def pair_resize_bilinear(x: Pair, size: Tuple[int, int], out: Optional[Pair] = None) -> Pair:
-    B, H, W, C = x.shape
-    if out is None:
-        out = Pair.empty((B, size[0], size[1], C), x.device)
-    assert tuple(out.shape) == (B, size[0], size[1], C)
-    _be().pair_pool(2, x, out)
-    return out
-
-
 def linear(x, w, bias=None, *, act=ACT_NONE, residual=None, out=None, out_dtype=None, algo=ALGO_AUTO):
     """y = act(x @ w.T + bias (+ residual)); x [..., K] (rows may be pitched), w [N, K]."""
     lead = x.shape[:-1]
-    K = x.shape[-1]
     N = w.shape[0]
-    x4 = x.reshape(1, 1, -1, K) if x.is_contiguous() else _as4(x)
-    r4 = None if residual is None else (residual.reshape(1, 1, -1, N) if residual.is_contiguous() else _as4(residual))
-    o4 = None if out is None else (out.reshape(1, 1, -1, N) if out.is_contiguous() else _as4(out))
-    y = conv2d(x4, w.reshape(N, 1, 1, w.shape[-1]), None, bias, act=act, residual=r4, out=o4, out_dtype=out_dtype, algo=algo)
+    y = conv2d(_as4(x), w.reshape(N, 1, 1, w.shape[-1]), None, bias, act=act, residual=None if residual is None else _as4(residual),
+               out=None if out is None else _as4(out), out_dtype=out_dtype, algo=algo)
     return out if out is not None else y.reshape(*lead, N)
 
 
+def linear_pair(x: Pair, w3, bias=None, *, act=ACT_NONE, residual=None, out=None, out_pair: bool = False):
+    """linear on dense pair-format rows x [..., K] with the weight triple w3 [N, 3K] (conv2d_pair on the rows as one [1,1,M,K] image) -> fp32 [..., N], or a
+    Pair with out_pair=True.  `out` may be a column slice [..., :N] of a wider fp32 buffer (its row pitch is kept)."""
+    buf = x.buf
+    assert buf.is_contiguous() and x.c0 == 0 and x.C == x.Ctot
+    lead = buf.shape[:-1]
+    N = w3.shape[0]
+    y = conv2d_pair(Pair(buf.reshape(1, 1, -1, buf.shape[-1])), w3.reshape(N, 1, 1, w3.shape[-1]), None, bias, act=act,
+                    residual=None if residual is None else _as4(residual), out=None if out is None else _as4(out), out_pair=out_pair)
+    if out is not None:
+        return out
+    return Pair(y.buf.reshape(*lead, 2 * N)) if out_pair else y.reshape(*lead, N)
+
+
 def _as4(t):
-    """[..., L, C] pitched view -> [1,1,M,C] view (requires uniform pitch, checked by _pitch)."""
+    """[..., L, C] rows, dense or with a uniform pitch (checked by _pitch) -> [1,1,M,C] view."""
+    if t.is_contiguous():
+        return t.reshape(1, 1, -1, t.shape[-1])
     p = _pitch(t)
     M = t.numel() // t.shape[-1]
     return t.as_strided((1, 1, M, t.shape[-1]), (M * p, M * p, p, 1), t.storage_offset())
 
 
+def _empty_like_format(x, shape):
+    """an output of x's format: a Pair for a Pair, else a tensor of x's dtype"""
+    return Pair.empty(shape, x.device) if isinstance(x, Pair) else torch.empty(shape, dtype=x.dtype, device=x.device)
+
+
 def maxpool3x3s2(x):
+    """3x3/s2/p1 max pool of an NHWC tensor or a Pair (same format out)"""
     B, H, W, C = x.shape
-    out = torch.empty((B, (H - 1) // 2 + 1, (W - 1) // 2 + 1, C), dtype=x.dtype, device=x.device)
-    _be().maxpool3x3s2(x.contiguous(), out)
+    out = _empty_like_format(x, (B, (H - 1) // 2 + 1, (W - 1) // 2 + 1, C))
+    if isinstance(x, Pair):
+        _be().pair_pool(0, x, out)
+    else:
+        _be().maxpool3x3s2(x.contiguous(), out)
     return out
 
 
 def avgpool2x2(x):
+    """2x2/s2 ceil-mode average pool of an NHWC tensor or a Pair (same format out)"""
     B, H, W, C = x.shape
-    out = torch.empty((B, (H + 1) // 2, (W + 1) // 2, C), dtype=x.dtype, device=x.device)
-    _be().avgpool2x2(x.contiguous(), out)
+    out = _empty_like_format(x, (B, (H + 1) // 2, (W + 1) // 2, C))
+    if isinstance(x, Pair):
+        _be().pair_pool(1, x, out)
+    else:
+        _be().avgpool2x2(x.contiguous(), out)
     return out
 
 
 def resize_bilinear(x, size: Tuple[int, int], out=None):
+    """bilinear resize (align_corners=False) of an NHWC tensor or a Pair; `out` (same format as x) may be a channel slice of a wider buffer"""
     B, H, W, C = x.shape
     if out is None:
-        out = torch.empty((B, size[0], size[1], C), dtype=x.dtype, device=x.device)
-    assert tuple(out.shape) == (B, size[0], size[1], C)
-    _be().resize_bilinear(x, out)
+        out = _empty_like_format(x, (B, size[0], size[1], C))
+    assert tuple(out.shape) == (B, size[0], size[1], C) and isinstance(out, Pair) == isinstance(x, Pair)
+    if isinstance(x, Pair):
+        _be().pair_pool(2, x, out)
+    else:
+        _be().resize_bilinear(x, out)
     return out
 
 

@@ -7,6 +7,7 @@ zero-extended to even size, and the engines are checked to launch the same conv 
 import json
 import math
 import os
+import time
 
 import numpy as np
 import pytest
@@ -134,6 +135,7 @@ def _conv_kernel_sequence(m, x):
     m(x)
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        time.sleep(0.2)  # kernels launched right as a session starts have been seen missing from its trace: start the work 0.2 s in
         m(x)
         torch.cuda.synchronize()
     ev = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA), key=lambda e: e.time_range.start)
@@ -171,7 +173,7 @@ def test_stem_from_uint8_on_odd_images():
 
 
 @pytest.mark.parametrize("H,W", [(179, 242), (45, 61), (23, 31), (90, 121), (5, 7), (1, 1)])
-def test_pools_on_odd_maps_vs_fp64(H, W):
+def test_tensor_and_pair_pools_on_odd_maps_vs_fp64(H, W):
     x = rnd((2, H, W, 64), torch.float32, H + W, 3.0)
     x64 = nchw(x.double())
     xg = x.to(DEV)
@@ -182,11 +184,11 @@ def test_pools_on_odd_maps_vs_fp64(H, W):
     dw = F.conv2d(x64, w9c.double().t().reshape(64, 1, 3, 3), None, 2, 1, 1, 64) * sc.double().view(1, -1, 1, 1) + bi.double().view(1, -1, 1, 1)
     close(ops.dwconv3x3s2(xg, w9c.to(DEV), sc.to(DEV), bi.to(DEV)), nhwc(dw), 1e-5, "dwconv3x3s2")
     xp = ops.Pair(ops.split_pair(xg))
-    close(ops.pair_maxpool3x3s2(xp).float(), nhwc(F.max_pool2d(x64, 3, 2, 1)), 3e-6, "pair pool mode 0")
-    close(ops.pair_avgpool2x2(xp).float(), nhwc(F.avg_pool2d(x64, 2, 2, 0, ceil_mode=True)), 3e-6, "pair pool mode 1")
+    close(ops.maxpool3x3s2(xp).float(), nhwc(F.max_pool2d(x64, 3, 2, 1)), 3e-6, "pair pool mode 0")
+    close(ops.avgpool2x2(xp).float(), nhwc(F.avg_pool2d(x64, 2, 2, 0, ceil_mode=True)), 3e-6, "pair pool mode 1")
     size = (2 * H + 1, 2 * W - 1)
     ref = nhwc(F.interpolate(x64, size=size, mode="bilinear", align_corners=False))
-    close(ops.pair_resize_bilinear(xp, size).float(), ref, 3e-6 + resize_tol(x64, size) / max(1.0, float(ref.abs().max())), "pair pool mode 2")
+    close(ops.resize_bilinear(xp, size).float(), ref, 3e-6 + resize_tol(x64, size) / max(1.0, float(ref.abs().max())), "pair pool mode 2")
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16])

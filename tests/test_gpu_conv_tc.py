@@ -224,15 +224,16 @@ def test_conv2d_pair_channel_slices_of_a_wider_pair_buffer():
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
-def test_pair_pool_matches_the_fp32_operator(mode):
+def test_pools_on_pairs_match_the_fp32_operator(mode):
     x = rnd((2, 37, 50, 64), torch.float32, 21, 3.0)
     xp = _pair_from(x)
     if mode == 0:
-        got, ref = ops.pair_maxpool3x3s2(xp), torch.nn.functional.max_pool2d(x.permute(0, 3, 1, 2), 3, 2, 1)
+        got, ref = ops.maxpool3x3s2(xp), torch.nn.functional.max_pool2d(x.permute(0, 3, 1, 2), 3, 2, 1)
     elif mode == 1:
-        got, ref = ops.pair_avgpool2x2(xp), torch.nn.functional.avg_pool2d(x.permute(0, 3, 1, 2), 2, 2, 0, ceil_mode=True)
+        got, ref = ops.avgpool2x2(xp), torch.nn.functional.avg_pool2d(x.permute(0, 3, 1, 2), 2, 2, 0, ceil_mode=True)
     else:
-        got, ref = ops.pair_resize_bilinear(xp, (74, 100)), torch.nn.functional.interpolate(x.permute(0, 3, 1, 2), size=(74, 100), mode="bilinear", align_corners=False)
+        got, ref = ops.resize_bilinear(xp, (74, 100)), torch.nn.functional.interpolate(x.permute(0, 3, 1, 2), size=(74, 100), mode="bilinear", align_corners=False)
+    assert isinstance(got, ops.Pair)
     assert float((got.float().cpu() - ref.permute(0, 2, 3, 1)).abs().max()) <= 3e-6 * 12
 
 

@@ -74,7 +74,7 @@ def test_mf_fused_graph_matches_golden(ref_backend):
 
 
 def test_mf_pair_backbone_runs_as_pair_convs(ref_backend):
-    """precision="fp32_tc": the ResNet backbone runs in the pair format (fp16 hi/lo planes between convs, DetrEngine._run_backbone_pair) and the four pixel-decoder
+    """precision="fp32_tc": the ResNet backbone runs in the pair format (fp16 hi/lo planes between convs, DetrEngine._run_backbone) and the four pixel-decoder
     convs read the pairs - host-side bookkeeping on the CPU references: same outputs as the fp32 graph up to the pair rounding (2^-22 relative per activation)."""
     g = load_golden("mf_l_coco_ins_b2_320x416")
     m = FAIMaskFormer(MaskFormerConfig(), precision="fp32_tc")

@@ -56,13 +56,13 @@ with torch.no_grad():
     state = {}
 
     def trunk():
-        state["mem"], state["shapes"], state["K"] = eng._forward_pair_trunk(x, None)
+        state["mem"], state["shapes"], state["K"] = eng._trunk(x, None)
 
     def head():
         mem, shapes, K = state["mem"], state["shapes"], state["K"]
-        value_all = eng._plin(eng.value_all, mem)
-        t = eng._plin(eng.enc_output, mem)
-        return eng._forward_head_pair(t, value_all, shapes, K, B, mem.buf.shape[1], None, mem)
+        value_all = eng._linear(eng.value_all, mem)
+        t = eng._linear(eng.enc_output, mem)
+        return eng._forward_head_pair(t, value_all, mem, shapes, K, B, mem.shape[1], None)
 
     l0 = ops.launch_count()
     trunk()
