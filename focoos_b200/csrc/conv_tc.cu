@@ -451,6 +451,168 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   if (ct == 0) tma_store_wait_all();
 }
 
+// ---------------------------------------------------------------------------------------------- small-channel 3x3 fused-split kernel
+// 3x3 / stride 1 / pad 1 fp32-accurate convs with 32 input channels and 32 or 64 output channels (the ResNet-vd stem's conv1_2 and conv1_3).  The
+// general kernel streams A_hi, A_lo, W_hi, W_lo through its ring once per filter tap.  Here BLOCK_N = Cout and the whole [W_hi | W_lo] (9 taps x 2 x
+// Cout x 64 B: 36 or 72 KiB) is loaded into shared memory once, at kernel start, and an output tile takes ONE ring entry: three kw-shifted boxes of
+// SC_BW x (SC_BH + 2) input pixels per plane.  Tap (kh, kw) is box kw from pixel row kh * SC_BW on, a 128-row operand whose start is a multiple of the
+// 512-byte repeat of the 64-byte swizzle, so the usual descriptors address it.  That is 3 x 160 instead of 9 x 128 A rows per tile and no weights in the
+// stream.  Products run in the general kernel's order (tap, 16-channel step, then hi x W_hi, hi x W_lo, lo x W_hi) with N = Cout, so the outputs are the
+// same bits.  Same warp roles and epilogue (folded BN, activation, fp32 or pair output through TMA stores) without residual or row-max.
+constexpr int SC_BW = 16, SC_BH = 8;                 // output tile: 16 x 8 pixels = BLOCK_M rows
+constexpr int SC_BOX_ROWS = SC_BW * (SC_BH + 2);     // one kw-shifted input box
+constexpr int SC_BOX_BYTES = SC_BOX_ROWS * 64;       // 32 channels of fp16: 64-byte rows, 64-byte swizzle
+constexpr int SC_STAGE_BYTES = 2 * 3 * SC_BOX_BYTES;  // hi and lo planes x three kw shifts: 60 KiB
+constexpr int SC_STAGES = 2;
+template <int BLOCK_N> __host__ __device__ constexpr int sc_w_bytes() { return 9 * 2 * BLOCK_N * 64; }
+template <int BLOCK_N> constexpr int sc_smem_bytes() {
+  return sc_w_bytes<BLOCK_N>() + SC_STAGES * SC_STAGE_BYTES + 2 * STAGING_BYTES + (2 * SC_STAGES + 1) * 8 + 1024 /*align slack*/;
+}
+
+template <int BLOCK_N, typename TOut>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+conv_tc_smallc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                      const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_d2, const KParams p) {
+  constexpr bool PAIR = is_pair<TOut>::value;
+  constexpr int W_BYTES = sc_w_bytes<BLOCK_N>();
+  constexpr int W_TAP = 2 * BLOCK_N * 64;  // [W_hi | W_lo] of one tap
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_w = smem;
+  uint8_t* smem_a = smem_w + W_BYTES;
+  uint8_t* staging = smem_a + SC_STAGES * SC_STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + 2 * STAGING_BYTES);
+  uint64_t* empty_bar = full_bar + SC_STAGES;
+  uint64_t* w_bar = empty_bar + SC_STAGES;
+  constexpr int CHUNK_COLS = 32;  // pair and fp32 staging rows alike
+  constexpr int NCHUNKS = BLOCK_N / CHUNK_COLS;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_d) : "memory");
+    for (int i = 0; i < SC_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], CONSUMER_WARPS); }
+    mbar_init(w_bar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  const int tiles_per_img = p.tiles_w * p.tiles_h;
+  struct TileXY { int img, h0, w0; };
+  auto tile_of = [&](int t) {  // BLOCK_N = Cout: one N tile
+    TileXY r;
+    r.img = t / tiles_per_img;
+    const int rem = t - r.img * tiles_per_img;
+    r.h0 = (rem / p.tiles_w) * SC_BH;
+    r.w0 = (rem % p.tiles_w) * SC_BW;
+    return r;
+  };
+
+  if (warp < 4) {
+    // ===================================================================== TMA producer
+    if (threadIdx.x != 0) return;
+    mbar_arrive_expect_tx(w_bar, (uint32_t)W_BYTES);
+    for (int tap = 0; tap < 9; ++tap) {  // weights packed [W_hi | W_lo | W_hi] per tap
+      tma_load_2d(&tmap_b, w_bar, smem_w + tap * W_TAP, tap * 3 * p.w_seg, 0);
+      tma_load_2d(&tmap_b, w_bar, smem_w + tap * W_TAP + W_TAP / 2, tap * 3 * p.w_seg + p.w_seg, 0);
+    }
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+      const TileXY tc = tile_of(t);
+      mbar_wait(&empty_bar[stage], phase ^ 1);
+      mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)SC_STAGE_BYTES);
+      uint8_t* dst = smem_a + stage * SC_STAGE_BYTES;
+      for (int kw = 0; kw < 3; ++kw) {  // box kw: input pixels (h0 - 1 .. h0 + SC_BH, w0 + kw - 1 ..); the TMA unit zero-fills the padding
+        tma_load_4d(&tmap_a, &full_bar[stage], dst + kw * SC_BOX_BYTES, 0, tc.w0 + kw - 1, tc.h0 - 1, tc.img);
+        tma_load_4d(&tmap_a, &full_bar[stage], dst + (3 + kw) * SC_BOX_BYTES, p.lo_off, tc.w0 + kw - 1, tc.h0 - 1, tc.img);
+      }
+      if (++stage == SC_STAGES) { stage = 0; phase ^= 1; }
+    }
+    return;
+  }
+
+  // ===================================================================== consumers: wgmma over the nine taps of one patch + epilogue
+  const int ct = threadIdx.x - 128;
+  const int g = ct >> 7;
+  const int r0 = g * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  float acc[BLOCK_N / 2];
+  float sc[BLOCK_N / 4], bi[BLOCK_N / 4];  // folded BN of this thread's columns, the same for every tile
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int n = 8 * j + cq + e;
+      sc[2 * j + e] = p.scale ? __ldg(p.scale + n) : 1.f;
+      bi[2 * j + e] = p.bias ? __ldg(p.bias + n) : 0.f;
+    }
+  mbar_wait(w_bar, 0);
+  const uint32_t sw = smem_u32(smem_w);
+  int stage = 0;
+  uint32_t phase = 0, chunk_ctr = 0;
+  for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+    const TileXY tc = tile_of(t);
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem_a + stage * SC_STAGE_BYTES) + (uint32_t)(g * 64 * 64);
+    wgmma_fence();
+#pragma unroll
+    for (int tap = 0; tap < 9; ++tap) {
+      const int kh = tap / 3, kw = tap - 3 * (tap / 3);
+      const uint32_t a_tap = sa + (uint32_t)(kw * SC_BOX_BYTES + kh * SC_BW * 64);
+      const uint64_t da = make_smem_desc<32>(a_tap), da_lo = make_smem_desc<32>(a_tap + 3 * SC_BOX_BYTES);
+      const uint64_t db = make_smem_desc<32>(sw + tap * W_TAP), db_lo = make_smem_desc<32>(sw + tap * W_TAP + W_TAP / 2);
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const uint64_t ko = (uint64_t)(k * 2);
+        Wgmma<BLOCK_N, 0>::mma(acc, da + ko, db + ko, (tap > 0 || k > 0) ? 1u : 0u);
+        Wgmma<BLOCK_N, 0>::mma(acc, da + ko, db_lo + ko, 1u);
+        Wgmma<BLOCK_N, 0>::mma(acc, da_lo + ko, db + ko, 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);  // the producer refills this entry with a later tile's patch while the epilogue runs
+    if (++stage == SC_STAGES) { stage = 0; phase ^= 1; }
+
+#pragma unroll
+    for (int ch = 0; ch < NCHUNKS; ++ch) {
+      uint8_t* stg = staging + (chunk_ctr & 1) * STAGING_BYTES;
+      if (ct == 0) tma_store_wait_read<1>();  // the TMA store that last used this staging buffer has finished reading it
+      consumer_bar();
+#pragma unroll
+      for (int jj = 0; jj < CHUNK_COLS / 8; ++jj) {
+        const int j = ch * (CHUNK_COLS / 8) + jj;
+        const int lc = 8 * jj + cq;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          const float v0 = act1<false>(fmaf(acc[4 * j + 2 * h], sc[2 * j], bi[2 * j]), p.act);
+          const float v1 = act1<false>(fmaf(acc[4 * j + 2 * h + 1], sc[2 * j + 1], bi[2 * j + 1]), p.act);
+          if constexpr (PAIR) {  // two 64-byte-row planes, 64-byte swizzle
+            const int off = row * 64 + ((((lc >> 3) ^ ((row >> 1) & 3)) << 4) | ((lc & 7) * 2));
+            const __half2 hi = __floats2half2_rn(v0, v1);
+            const float2 hf = __half22float2(hi);
+            *reinterpret_cast<__half2*>(stg + off) = hi;
+            *reinterpret_cast<__half2*>(stg + STAGING_BYTES / 2 + off) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+          } else {
+            const int off = row * 128 + ((((lc >> 2) ^ (row & 7)) << 4) | ((lc & 3) * 4));
+            *reinterpret_cast<float2*>(stg + off) = make_float2(v0, v1);
+          }
+        }
+      }
+      fence_proxy_async();
+      consumer_bar();
+      if (ct == 0) {
+        tma_store_4d(&tmap_d, stg, ch * CHUNK_COLS, tc.w0, tc.h0, tc.img);
+        if constexpr (PAIR) tma_store_4d(&tmap_d2, stg + STAGING_BYTES / 2, ch * CHUNK_COLS, tc.w0, tc.h0, tc.img);
+        tma_store_commit();
+      }
+      ++chunk_ctr;
+    }
+  }
+  if (ct == 0) tma_store_wait_all();
+}
+
 // ---------------------------------------------------------------------------------------------- host
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -531,6 +693,75 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
   return FB200_OK;
 }
 
+template <int BLOCK_N, typename TOut>
+static int launch_smallc(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& td2, const KParams& kp, cudaStream_t st) {
+  auto kern = conv_tc_smallc_kernel<BLOCK_N, TOut>;
+  constexpr int smem = sc_smem_bytes<BLOCK_N>();
+  static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) { set_error("conv_tc: cudaFuncSetAttribute(%d B) failed: %s", smem, cudaGetErrorString(e)); return FB200_ERR_CUDA; }
+    configured = true;
+  }
+  const int64_t cap = num_sms();
+  const unsigned grid = (unsigned)(kp.total_tiles < cap ? kp.total_tiles : cap);
+  kern<<<grid, NUM_THREADS, smem, st>>>(ta, tb, td, td2, kp);
+  FB_CHECK_LAUNCH("conv_tc_smallc_kernel");
+  return FB200_OK;
+}
+
+// fused-split 3x3 / stride 1 / pad 1, Cin = 32, Cout = 32 or 64, no residual, fp32 or pair output
+static bool smallc_fits(const ConvParams& p) {
+  return p.split3 && p.Cin == 3 * 32 && (p.Cout == 32 || p.Cout == 64) && p.KH == 3 && p.KW == 3 && p.stride == 1 && p.pad == 1 &&
+         !p.res && !p.rowmax && p.w_bs == 0 && (p.out_dtype == FB200_F32 || p.out_dtype == FB200_F16PAIR);
+}
+
+static int conv2d_tc_smallc(const ConvParams& p, cudaStream_t st) {
+  KParams kp{};
+  kp.scale = p.scale; kp.bias = p.bias; kp.act = p.act; kp.Cout = p.Cout;
+  kp.lo_off = p.x_lo_off ? (int)p.x_lo_off : 32;
+  kp.w_seg = 32;
+  kp.tiles_w = (p.Wo + SC_BW - 1) / SC_BW; kp.tiles_h = (p.Ho + SC_BH - 1) / SC_BH; kp.Ho = p.Ho; kp.Wo = p.Wo;
+  const int64_t total = (int64_t)p.B * kp.tiles_w * kp.tiles_h;
+  if (total > 0x7fffffffLL) { set_error("conv_tc: too many tiles (%lld)", (long long)total); return FB200_ERR_UNSUPPORTED; }
+  kp.total_tiles = (int)total;
+  CUtensorMap ta, tb, td, td2;
+  const uint64_t P = (uint64_t)p.x_pitch;
+  {
+    const uint64_t dims[4] = {(uint64_t)kp.lo_off + 32, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.B};
+    const uint64_t str[4] = {1, P, P * p.W, P * p.W * p.H};
+    const uint32_t box[4] = {32, SC_BW, SC_BH + 2, 1};
+    int rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "A(patch)", CU_TENSOR_MAP_SWIZZLE_64B);
+    if (rc) return rc;
+  }
+  {
+    const uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.Cout};
+    const uint64_t str[2] = {1, (uint64_t)p.K};
+    const uint32_t box[2] = {32, (uint32_t)p.Cout};
+    int rc = encode(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2, const_cast<void*>(p.w), dims, str, box, "W", CU_TENSOR_MAP_SWIZZLE_64B);
+    if (rc) return rc;
+  }
+  const bool outp = p.out_dtype == FB200_F16PAIR;
+  {
+    const uint64_t OP = (uint64_t)p.out_pitch;
+    const uint64_t dims[4] = {(uint64_t)p.Cout, (uint64_t)p.Wo, (uint64_t)p.Ho, (uint64_t)p.B};
+    const uint64_t str[4] = {1, OP, OP * p.Wo, (uint64_t)p.out_bs};
+    const uint32_t box[4] = {32, SC_BW, SC_BH, 1};
+    int rc;
+    if (outp) {  // two fp16 planes, 32-channel boxes with 64-byte swizzle
+      rc = encode(&td, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, p.out, dims, str, box, "D(hi)", CU_TENSOR_MAP_SWIZZLE_64B);
+      if (!rc) rc = encode(&td2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, static_cast<__half*>(p.out) + p.out_lo_off, dims, str, box, "D(lo)", CU_TENSOR_MAP_SWIZZLE_64B);
+    } else {
+      rc = encode(&td, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 4, p.out, dims, str, box, "D");
+      td2 = td;
+    }
+    if (rc) return rc;
+  }
+  if (p.Cout == 32) return outp ? launch_smallc<32, PairOut>(ta, tb, td, td2, kp, st) : launch_smallc<32, float>(ta, tb, td, td2, kp, st);
+  return outp ? launch_smallc<64, PairOut>(ta, tb, td, td2, kp, st) : launch_smallc<64, float>(ta, tb, td, td2, kp, st);
+}
+
 }  // namespace tc
 
 bool conv2d_tc_supported(const ConvParams& p, int x_dtype, int out_dtype) {
@@ -565,6 +796,7 @@ bool conv2d_tc_supported(const ConvParams& p, int x_dtype, int out_dtype) {
 
 int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   using namespace tc;
+  if (smallc_fits(p)) return conv2d_tc_smallc(p, st);  // fp32-accurate 3x3 with 32 input channels: resident weights, one input patch per tile
   KParams kp;
   kp.scale = p.scale; kp.bias = p.bias; kp.res = p.res; kp.act = p.act; kp.Cout = p.Cout;
   kp.KH = p.KH; kp.KW = p.KW; kp.pad = p.pad;
