@@ -557,7 +557,8 @@ static int conv2d_impl(const void* x, int x_dtype, int B, int H, int W, int Cin,
   p.w_bs = w_bs;
   const bool tc_ok = conv2d_tc_supported(p, x_dtype, out_dtype);
   if (algo == FB200_ALGO_TCGEN05 && !tc_ok) {
-    set_error("conv2d: tensor-core path does not support this shape/dtype (Cin=%d Cout=%d k=%dx%d s=%d dtype=%d/%d)", Cin, Cout, KH, KW, stride, x_dtype, out_dtype);
+    set_error("conv2d: tensor-core path does not support this shape/dtype (Cin=%d Cout=%d k=%dx%d s=%d dtype=%d/%d); split-precision convs write fp32 or the fp16 pair", Cin,
+              Cout, KH, KW, stride, x_dtype, out_dtype);
     return FB200_ERR_UNSUPPORTED;
   }
   if ((algo == FB200_ALGO_AUTO && tc_ok) || algo == FB200_ALGO_TCGEN05) return conv2d_tc(p, st);

@@ -30,6 +30,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace fb200 {
@@ -51,8 +52,9 @@ template <> struct is_pair<PairOut> { static constexpr bool value = true; };
 struct KParams {
   const float* scale; const float* bias; const void* res;
   int act, Cout;
-  int KH, KW, pad, cchunks;        // cchunks = Cin / BLOCK_K (segmented split-precision: 3C / BLOCK_K; fused split: C / BLOCK_K)
-  int seg_chunks, lo_off;          // split-precision: chunks per K segment (C/BLOCK_K, 0 = off) and channel offset of the A operand's lo half (C unless the input is a channel slice of a wider pair buffer)
+  int KH, KW, pad, cchunks;        // cchunks = C / BLOCK_K, C = channels of the input (split-precision: of one of its [hi | lo] planes)
+  int w_batched;                   // 1: weights differ per image (3-D weight map, third coordinate = image)
+  int lo_off;                      // split-precision: channel offset of the A operand's lo half (C unless the input is a channel slice of a wider pair buffer)
   int w_seg;                       // split-precision: channels per weight segment ([W_hi | W_lo | W_hi] per tap)
   int BW, BH, tiles_w, tiles_h;    // output tile rectangle and tile counts per image
   int Ho, Wo;                      // output spatial size (validity of rows)
@@ -61,63 +63,9 @@ struct KParams {
   int num_k_blocks;
   int n_tiles, total_tiles;        // N tiles per M tile; total = m_tiles * n_tiles
   float* rowmax;                   // not null: row-max-only epilogue (query selection scores), nothing is stored
-  int w_batched;                   // 1: weights differ per image (3-D weight map, third coordinate = image)
 };
 
-// ---------------------------------------------------------------------------------------------- PTX
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done = 0;
-  uint32_t spins = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (done) break;
-    if (++spins > (1u << 26)) __trap();  // a descriptor / phase bug must not hang the GPU
-  }
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-__device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_5d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // K-major swizzled shared-memory matrix descriptor (sm_90 format: layout type at bits 62-63, 1 = SWIZZLE_128B, 2 = SWIZZLE_64B)
 template <int BLOCK_K>
@@ -144,6 +92,66 @@ __device__ __forceinline__ float act1(float v, int act) {
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
   if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
   else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
+}
+
+// ---------------------------------------------------------------------------------------------- epilogue pieces of both kernels
+// A consumer thread's place in the 128-row accumulator tile (fragment layout: wgmma.cuh)
+struct AccThread {
+  int ct;  // consumer thread 0..255; thread 0 issues the TMA stores
+  int g;   // warp-group: tile rows 64g .. 64g + 63
+  int r0;  // accumulator rows r0 and r0 + 8 of this thread
+  int cq;  // first of the two adjacent accumulator columns
+};
+__device__ __forceinline__ AccThread acc_thread() {
+  const int ct = threadIdx.x - 128, lane = threadIdx.x & 31;
+  return {ct, ct >> 7, (ct >> 7) * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2), 2 * (lane & 3)};
+}
+
+// Byte offset of (row, lc = column inside the chunk) in a swizzled staging tile - the layout a TMA store reads and a residual box lands in: the 16-byte piece
+// index XOR the row phase.  A pair has two planes of 64-byte rows (64-byte swizzle), the same offset in each; fp16 and fp32 have 128-byte rows.
+template <typename TOut>
+__device__ __forceinline__ int staging_offset(int row, int lc) {
+  if constexpr (is_pair<TOut>::value) return row * 64 + ((((lc >> 3) ^ ((row >> 1) & 3)) << 4) | ((lc & 7) * 2));
+  else if constexpr (sizeof(TOut) == 2) return row * 128 + ((((lc >> 3) ^ (row & 7)) << 4) | ((lc & 7) * 2));
+  else return row * 128 + ((((lc >> 2) ^ (row & 7)) << 4) | ((lc & 3) * 4));
+}
+
+// the adjacent columns (v0, v1) -> the staging tile at `off`; a pair is split again: hi = fp16(v), lo = fp16(v - hi) on the second plane
+template <typename TOut>
+__device__ __forceinline__ void staging_store(uint8_t* stg, int off, float v0, float v1) {
+  if constexpr (is_pair<TOut>::value) {
+    const __half2 hi = __floats2half2_rn(v0, v1);
+    const float2 hf = __half22float2(hi);
+    *reinterpret_cast<__half2*>(stg + off) = hi;
+    *reinterpret_cast<__half2*>(stg + STAGING_BYTES / 2 + off) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+  } else if constexpr (sizeof(TOut) == 2) {
+    *reinterpret_cast<__half2*>(stg + off) = __floats2half2_rn(v0, v1);
+  } else {
+    *reinterpret_cast<float2*>(stg + off) = make_float2(v0, v1);
+  }
+}
+
+// The consumers write a staging buffer between staging_open and staging_close.  open: thread 0 waits until the TMA store that last used the buffer
+// (NSTG chunks ago) has finished READING it and runs `then` (what else it must start once the buffer is free), then the consumers meet.
+template <int NSTG, typename F>
+__device__ __forceinline__ void staging_open(int ct, F&& then) {
+  if (ct == 0) {
+    tma_store_wait_read<NSTG - 1>();
+    then();
+  }
+  consumer_bar();
+}
+// close: every consumer's writes are made visible to the TMA unit, the consumers meet, and thread 0 stores the chunk at channel n of the tile at
+// (w0, h0, img) - both planes of a pair - as one bulk group; the TMA unit clips ragged tiles and Cout tails
+template <typename TOut>
+__device__ __forceinline__ void staging_close(int ct, const uint8_t* stg, const CUtensorMap* tmap_d, const CUtensorMap* tmap_d2, int n, int w0, int h0, int img) {
+  fence_proxy_async();
+  consumer_bar();
+  if (ct == 0) {
+    tma_store_4d(tmap_d, stg, n, w0, h0, img);
+    if constexpr (is_pair<TOut>::value) tma_store_4d(tmap_d2, stg + STAGING_BYTES / 2, n, w0, h0, img);
+    tma_store_commit();
+  }
 }
 
 // FS ("fused split", fp32-accurate mode): one ring stage holds the hi AND lo halves of both operands of a channel chunk - A_hi, A_lo, B_hi, B_lo are loaded ONCE
@@ -218,13 +226,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     // ===================================================================== TMA producer
     if (threadIdx.x != 0) return;
     const uint32_t a_bytes = (uint32_t)(p.BW * p.BH * BLOCK_K * 2);
-    // channel coordinate of K-chunk cc.  Segmented split-precision mode (fp32-accurate products from fp16 tensor cores, fp16 output): the stored tensor is
-    // [hi(C) | lo(C)] and K runs over three segments  hi x W_hi,  hi x W_lo,  lo x W_hi  (weights packed [W_hi | W_lo | W_hi]).
-    auto a_chan = [&](int cc) -> int {
-      if (p.seg_chunks == 0) return cc * BLOCK_K;
-      const int seg = cc / p.seg_chunks, within = cc - seg * p.seg_chunks;
-      return (seg == 2 ? p.lo_off : 0) + within * BLOCK_K;
-    };
     auto load_a = [&](uint64_t* bar, void* dst, int c, int kh, int kw, int h0, int w0, int img) {
       if (!p.stride2) {
         tma_load_4d(&tmap_a, bar, dst, c, w0 + kw - p.pad, h0 + kh - p.pad, img);
@@ -252,7 +253,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         const int kh = tap / p.KW, kw = tap - kh * p.KW;
         uint8_t* dst_a = smem_a + stage * A_STAGE_BYTES;
         uint8_t* dst_b = smem_b + stage * B_STAGE_BYTES;
-        if constexpr (FS) {  // k-block = (tap, channel chunk): A_hi, A_lo, W_hi, W_lo once each
+        if constexpr (FS) {  // the stored input is [hi(C) | lo(C)]; k-block = (tap, channel chunk): A_hi, A_lo, W_hi, W_lo once each
           const int k_hi = tap * 3 * p.w_seg + cc * BLOCK_K, k_lo = k_hi + p.w_seg;  // weights packed [W_hi | W_lo | W_hi] per tap
           mbar_arrive_expect_tx(&full_bar[stage], 2u * a_bytes + (uint32_t)B_STAGE_BYTES);
           load_a(&full_bar[stage], dst_a, cc * BLOCK_K, kh, kw, tc.h0, tc.w0, tc.img);
@@ -261,7 +262,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           load_b(&full_bar[stage], dst_b + B_HALF, k_lo, tc.n0, tc.img);
         } else {
           mbar_arrive_expect_tx(&full_bar[stage], a_bytes + (uint32_t)B_STAGE_BYTES);
-          load_a(&full_bar[stage], dst_a, a_chan(cc), kh, kw, tc.h0, tc.w0, tc.img);
+          load_a(&full_bar[stage], dst_a, cc * BLOCK_K, kh, kw, tc.h0, tc.w0, tc.img);
           load_b(&full_bar[stage], dst_b, kb * BLOCK_K, tc.n0, tc.img);
         }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -287,10 +288,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   }
 
   // ===================================================================== consumers: wgmma main loop + epilogue
-  const int ct = threadIdx.x - 128;           // 0..255
-  const int g = ct >> 7;                      // warp-group: tile rows 64g .. 64g + 63
-  const int r0 = g * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2);  // accumulator rows r0 and r0 + 8 of this thread
-  const int cq = 2 * (lane & 3);              // first of the two adjacent accumulator columns
+  const AccThread th = acc_thread();
   constexpr int NACC = BLOCK_N / 2;
   const bool post = (p.act & FB200_ACT_RESIDUAL_AFTER) != 0;
   const bool has_res = p.res != nullptr;
@@ -302,7 +300,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     int prev = -1;
     for (int kb = 0; kb < p.num_k_blocks; ++kb) {
       mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES) + (uint32_t)(g * 64 * BLOCK_K * 2);
+      const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES) + (uint32_t)(th.g * 64 * BLOCK_K * 2);
       const uint32_t sb = smem_u32(smem_b + stage * B_STAGE_BYTES);
       const uint64_t da = make_smem_desc<BLOCK_K>(sa), db = make_smem_desc<BLOCK_K>(sb);
       wgmma_fence();
@@ -340,7 +338,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       for (int j = 0; j < BLOCK_N / 8; ++j) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          const int n = tc.n0 + 8 * j + cq + e;
+          const int n = tc.n0 + 8 * j + th.cq + e;
           if (n < p.Cout) {
             const float s = scale_of(n), b = bias_of(n);
             m[0] = fmaxf(m[0], fmaf(acc[4 * j + e], s, b));
@@ -353,7 +351,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
         m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
         int64_t pix;
-        if ((lane & 3) == 0 && row_valid(r0 + 8 * h, pix)) atomic_max_float(p.rowmax + pix, m[h]);
+        if ((lane & 3) == 0 && row_valid(th.r0 + 8 * h, pix)) atomic_max_float(p.rowmax + pix, m[h]);
       }
       continue;
     }
@@ -364,15 +362,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       if (ch >= nch) break;  // uniform across the consumers
       uint8_t* stg = staging + (chunk_ctr % NSTG) * STAGING_BYTES;
       const uint8_t* res = stg;  // residual chunk, same swizzled layout as the staging tile
-      if (ct == 0) {
-        tma_store_wait_read<NSTG - 1>();  // the TMA store that last used this staging buffer has finished READING it
+      staging_open<NSTG>(th.ct, [&] {
         if constexpr (!RES_RING) if (has_res) {  // the [BW x BH x CHUNK_COLS] residual box lands in the staging buffer; each thread adds and overwrites its own elements
           mbar_arrive_expect_tx(res_bar, (uint32_t)(p.BW * p.BH * 128));
           tma_load_4d(&tmap_r, res_bar, stg, tc.n0 + c0, tc.w0, tc.h0, tc.img);
           if constexpr (PAIR) tma_load_4d(&tmap_r2, res_bar, stg + STAGING_BYTES / 2, tc.n0 + c0, tc.w0, tc.h0, tc.img);
         }
-      }
-      consumer_bar();
+      });
       if constexpr (RES_RING) {
         if (res_ring) {
           if (ch % RES_SLOTS == 0) mbar_wait(&full_bar[stage], phase);
@@ -386,18 +382,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       for (int jj = 0; jj < CHUNK_COLS / 8; ++jj) {
         const int j = c0 / 8 + jj;
         if (j >= BLOCK_N / 8) break;
-        const int lc = 8 * jj + cq;  // column inside the chunk
+        const int lc = 8 * jj + th.cq;  // column inside the chunk
         const int n = tc.n0 + c0 + lc;
         const float s0 = scale_of(n), s1 = scale_of(n + 1), b0 = bias_of(n), b1 = bias_of(n + 1);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
+          const int row = th.r0 + 8 * h;
           float v0 = fmaf(acc[4 * j + 2 * h], s0, b0), v1 = fmaf(acc[4 * j + 2 * h + 1], s1, b1);
-          // byte offset of (row, lc) in the swizzled staging tile: 16-byte piece index XOR the row phase
-          int off;
-          if constexpr (PAIR) off = row * 64 + ((((lc >> 3) ^ ((row >> 1) & 3)) << 4) | ((lc & 7) * 2));  // two 64-byte-row planes, 64-byte swizzle
-          else if constexpr (sizeof(TOut) == 2) off = row * 128 + ((((lc >> 3) ^ (row & 7)) << 4) | ((lc & 7) * 2));
-          else off = row * 128 + ((((lc >> 2) ^ (row & 7)) << 4) | ((lc & 3) * 4));
+          const int off = staging_offset<TOut>(row, lc);
           auto add_residual = [&]() {
             if (!has_res) return;
             if constexpr (PAIR) {
@@ -419,16 +411,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           v0 = act1<GELU>(v0, p.act);
           v1 = act1<GELU>(v1, p.act);
           if (post) add_residual();
-          if constexpr (PAIR) {
-            const __half2 hi = __floats2half2_rn(v0, v1);
-            const float2 hf = __half22float2(hi);
-            *reinterpret_cast<__half2*>(stg + off) = hi;
-            *reinterpret_cast<__half2*>(stg + STAGING_BYTES / 2 + off) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
-          } else if constexpr (sizeof(TOut) == 2) {
-            *reinterpret_cast<__half2*>(stg + off) = __floats2half2_rn(v0, v1);
-          } else {
-            *reinterpret_cast<float2*>(stg + off) = make_float2(v0, v1);
-          }
+          staging_store<TOut>(stg, off, v0, v1);
         }
       }
       if constexpr (RES_RING) {
@@ -438,17 +421,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
-      fence_proxy_async();
-      consumer_bar();
-      if (ct == 0) {
-        tma_store_4d(&tmap_d, stg, tc.n0 + c0, tc.w0, tc.h0, tc.img);
-        if constexpr (PAIR) tma_store_4d(&tmap_d2, stg + STAGING_BYTES / 2, tc.n0 + c0, tc.w0, tc.h0, tc.img);
-        tma_store_commit();
-      }
+      staging_close<TOut>(th.ct, stg, &tmap_d, &tmap_d2, tc.n0 + c0, tc.w0, tc.h0, tc.img);
       ++chunk_ctr;
     }
   }
-  if (ct == 0) tma_store_wait_all();
+  if (th.ct == 0) tma_store_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------- small-channel 3x3 fused-split kernel
@@ -473,7 +450,6 @@ template <int BLOCK_N, typename TOut>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_smallc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                       const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_d2, const KParams p) {
-  constexpr bool PAIR = is_pair<TOut>::value;
   constexpr int W_BYTES = sc_w_bytes<BLOCK_N>();
   constexpr int W_TAP = 2 * BLOCK_N * 64;  // [W_hi | W_lo] of one tap
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -532,17 +508,14 @@ conv_tc_smallc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
   }
 
   // ===================================================================== consumers: wgmma over the nine taps of one patch + epilogue
-  const int ct = threadIdx.x - 128;
-  const int g = ct >> 7;
-  const int r0 = g * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2);
-  const int cq = 2 * (lane & 3);
+  const AccThread th = acc_thread();
   float acc[BLOCK_N / 2];
   float sc[BLOCK_N / 4], bi[BLOCK_N / 4];  // folded BN of this thread's columns, the same for every tile
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j)
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      const int n = 8 * j + cq + e;
+      const int n = 8 * j + th.cq + e;
       sc[2 * j + e] = p.scale ? __ldg(p.scale + n) : 1.f;
       bi[2 * j + e] = p.bias ? __ldg(p.bias + n) : 0.f;
     }
@@ -553,7 +526,7 @@ conv_tc_smallc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
   for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
     const TileXY tc = tile_of(t);
     mbar_wait(&full_bar[stage], phase);
-    const uint32_t sa = smem_u32(smem_a + stage * SC_STAGE_BYTES) + (uint32_t)(g * 64 * 64);
+    const uint32_t sa = smem_u32(smem_a + stage * SC_STAGE_BYTES) + (uint32_t)(th.g * 64 * 64);
     wgmma_fence();
 #pragma unroll
     for (int tap = 0; tap < 9; ++tap) {
@@ -577,79 +550,27 @@ conv_tc_smallc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
 #pragma unroll
     for (int ch = 0; ch < NCHUNKS; ++ch) {
       uint8_t* stg = staging + (chunk_ctr & 1) * STAGING_BYTES;
-      if (ct == 0) tma_store_wait_read<1>();  // the TMA store that last used this staging buffer has finished reading it
-      consumer_bar();
+      staging_open<2>(th.ct, [] {});
 #pragma unroll
       for (int jj = 0; jj < CHUNK_COLS / 8; ++jj) {
         const int j = ch * (CHUNK_COLS / 8) + jj;
-        const int lc = 8 * jj + cq;
+        const int lc = 8 * jj + th.cq;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
+          const int row = th.r0 + 8 * h;
           const float v0 = act1<false>(fmaf(acc[4 * j + 2 * h], sc[2 * j], bi[2 * j]), p.act);
           const float v1 = act1<false>(fmaf(acc[4 * j + 2 * h + 1], sc[2 * j + 1], bi[2 * j + 1]), p.act);
-          if constexpr (PAIR) {  // two 64-byte-row planes, 64-byte swizzle
-            const int off = row * 64 + ((((lc >> 3) ^ ((row >> 1) & 3)) << 4) | ((lc & 7) * 2));
-            const __half2 hi = __floats2half2_rn(v0, v1);
-            const float2 hf = __half22float2(hi);
-            *reinterpret_cast<__half2*>(stg + off) = hi;
-            *reinterpret_cast<__half2*>(stg + STAGING_BYTES / 2 + off) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
-          } else {
-            const int off = row * 128 + ((((lc >> 2) ^ (row & 7)) << 4) | ((lc & 3) * 4));
-            *reinterpret_cast<float2*>(stg + off) = make_float2(v0, v1);
-          }
+          staging_store<TOut>(stg, staging_offset<TOut>(row, lc), v0, v1);
         }
       }
-      fence_proxy_async();
-      consumer_bar();
-      if (ct == 0) {
-        tma_store_4d(&tmap_d, stg, ch * CHUNK_COLS, tc.w0, tc.h0, tc.img);
-        if constexpr (PAIR) tma_store_4d(&tmap_d2, stg + STAGING_BYTES / 2, ch * CHUNK_COLS, tc.w0, tc.h0, tc.img);
-        tma_store_commit();
-      }
+      staging_close<TOut>(th.ct, stg, &tmap_d, &tmap_d2, ch * CHUNK_COLS, tc.w0, tc.h0, tc.img);
       ++chunk_ctr;
     }
   }
-  if (ct == 0) tma_store_wait_all();
+  if (th.ct == 0) tma_store_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------- host
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
-static int encode(CUtensorMap* m, CUtensorMapDataType dt, int elt, int rank, void* base, const uint64_t* dims, const uint64_t* strides_elts,
-                  const uint32_t* box, const char* what, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B,
-                  const uint32_t* elem_strides = nullptr) {
-  // elem_strides (null = all 1): traversal stride per dimension; a load then takes ceil(box[i] / elem_strides[i]) elements along dimension i
-  EncodeTiledFn fn = get_encode();
-  if (!fn) { set_error("conv_tc: cuTensorMapEncodeTiled unavailable"); return FB200_ERR_CUDA; }
-  cuuint64_t gdim[5], gstr[4];
-  cuuint32_t bdim[5], estr[5];
-  for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bdim[i] = box[i]; estr[i] = elem_strides ? elem_strides[i] : 1; }
-  for (int i = 1; i < rank; ++i) gstr[i - 1] = strides_elts[i] * (uint64_t)elt;  // bytes; dim0 stride is implicit
-  CUresult r = fn(m, dt, (cuuint32_t)rank, base, gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("conv_tc: cuTensorMapEncodeTiled(%s) failed with %d (rank %d dims %llu,%llu,%llu,%llu box %u,%u,%u,%u)", what, (int)r, rank,
-              (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 0),
-              (unsigned long long)(rank > 3 ? dims[3] : 0), box[0], box[1], rank > 2 ? box[2] : 0, rank > 3 ? box[3] : 0);
-    return FB200_ERR_CUDA;
-  }
-  return FB200_OK;
-}
-
-// best output rectangle (BW x BH <= 128 pixels) for an Ho x Wo map
 // best output rectangle (BW x BH <= 128 pixels) for an Ho x Wo map
 static void choose_tile(int Ho, int Wo, int* BW, int* BH) {
   double best = -1.0;
@@ -663,52 +584,29 @@ static void choose_tile(int Ho, int Wo, int* BW, int* BH) {
   }
 }
 
-static int num_sms() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
-template <int BLOCK_N, int STAGES, typename TOut, int BLOCK_K, int NSTG, bool GELU, bool FS = false>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& tr, const CUtensorMap& td2, const CUtensorMap& tr2,
-                  const KParams& kp, cudaStream_t st) {
-  auto kern = conv_tc_kernel<BLOCK_N, STAGES, TOut, BLOCK_K, NSTG, GELU, FS>;
-  constexpr int smem = smem_bytes<BLOCK_N, STAGES, BLOCK_K, NSTG, FS>();
-  static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) { set_error("conv_tc: cudaFuncSetAttribute(%d B) failed: %s", smem, cudaGetErrorString(e)); return FB200_ERR_CUDA; }
-    configured = true;
-  }
-  const int64_t cap = num_sms();
-  const unsigned grid = (unsigned)(kp.total_tiles < cap ? kp.total_tiles : cap);
-  kern<<<grid, NUM_THREADS, smem, st>>>(ta, tb, td, tr, td2, tr2, kp);
-  FB_CHECK_LAUNCH("conv_tc_kernel");
-  return FB200_OK;
-}
-
-template <int BLOCK_N, typename TOut>
-static int launch_smallc(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& td2, const KParams& kp, cudaStream_t st) {
-  auto kern = conv_tc_smallc_kernel<BLOCK_N, TOut>;
-  constexpr int smem = sc_smem_bytes<BLOCK_N>();
-  static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) { set_error("conv_tc: cudaFuncSetAttribute(%d B) failed: %s", smem, cudaGetErrorString(e)); return FB200_ERR_CUDA; }
-    configured = true;
-  }
-  const int64_t cap = num_sms();
-  const unsigned grid = (unsigned)(kp.total_tiles < cap ? kp.total_tiles : cap);
-  kern<<<grid, NUM_THREADS, smem, st>>>(ta, tb, td, td2, kp);
-  FB_CHECK_LAUNCH("conv_tc_smallc_kernel");
-  return FB200_OK;
+// Tensor maps of the output (d; d2 = the lo plane of a pair) and of the residual (r, r2), which has the output's format and geometry with its own pointer /
+// pitch.  One box is a staging chunk of a BW x BH tile: 128-byte rows of fp16 / fp32, or per plane of a pair 32 channels with 64-byte swizzle (hi at `out`,
+// lo `out_lo_off` elements further).  Maps the kernel does not read (no residual, no pair) are copies of d.
+struct OutMaps { CUtensorMap d, d2, r, r2; };
+static int encode_out_maps(OutMaps* m, const ConvParams& p, int Wo, int Ho, int B, int BW, int BH, uint64_t batch_stride) {
+  const bool pair = p.out_dtype == FB200_F16PAIR, f32 = p.out_dtype == FB200_F32;
+  const CUtensorMapDataType dt = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const int elt = f32 ? 4 : 2;
+  const CUtensorMapSwizzle swz = pair ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
+  const uint64_t OP = (uint64_t)p.out_pitch, RP = (uint64_t)p.res_pitch;
+  const uint64_t dims[4] = {(uint64_t)p.Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B};
+  const uint64_t str[4] = {1, OP, OP * Wo, batch_stride}, rstr[4] = {1, RP, RP * Wo, RP * Wo * Ho};
+  const uint32_t box[4] = {(uint32_t)(pair || f32 ? 32 : 64), (uint32_t)BW, (uint32_t)BH, 1};
+  int rc = encode(&m->d, dt, elt, 4, p.out, dims, str, box, pair ? "conv_tc: D(hi)" : "conv_tc: D", swz);
+  if (rc) return rc;
+  m->d2 = m->d;
+  if (pair) rc = encode(&m->d2, dt, elt, 4, static_cast<__half*>(p.out) + p.out_lo_off, dims, str, box, "conv_tc: D(lo)", swz);
+  if (rc) return rc;
+  m->r = m->d; m->r2 = m->d2;
+  if (!p.res) return FB200_OK;
+  rc = encode(&m->r, dt, elt, 4, const_cast<void*>(p.res), dims, rstr, box, pair ? "conv_tc: R(hi)" : "conv_tc: R", swz);
+  if (rc || !pair) return rc;
+  return encode(&m->r2, dt, elt, 4, const_cast<__half*>(static_cast<const __half*>(p.res)) + p.res_lo_off, dims, rstr, box, "conv_tc: R(lo)", swz);
 }
 
 // fused-split 3x3 / stride 1 / pad 1, Cin = 32, Cout = 32 or 64, no residual, fp32 or pair output
@@ -726,40 +624,34 @@ static int conv2d_tc_smallc(const ConvParams& p, cudaStream_t st) {
   const int64_t total = (int64_t)p.B * kp.tiles_w * kp.tiles_h;
   if (total > 0x7fffffffLL) { set_error("conv_tc: too many tiles (%lld)", (long long)total); return FB200_ERR_UNSUPPORTED; }
   kp.total_tiles = (int)total;
-  CUtensorMap ta, tb, td, td2;
+  CUtensorMap ta, tb;
+  OutMaps om;
   const uint64_t P = (uint64_t)p.x_pitch;
   {
     const uint64_t dims[4] = {(uint64_t)kp.lo_off + 32, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.B};
     const uint64_t str[4] = {1, P, P * p.W, P * p.W * p.H};
     const uint32_t box[4] = {32, SC_BW, SC_BH + 2, 1};
-    int rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "A(patch)", CU_TENSOR_MAP_SWIZZLE_64B);
+    int rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "conv_tc: A(patch)", CU_TENSOR_MAP_SWIZZLE_64B);
     if (rc) return rc;
   }
   {
     const uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.Cout};
     const uint64_t str[2] = {1, (uint64_t)p.K};
     const uint32_t box[2] = {32, (uint32_t)p.Cout};
-    int rc = encode(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2, const_cast<void*>(p.w), dims, str, box, "W", CU_TENSOR_MAP_SWIZZLE_64B);
+    int rc = encode(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2, const_cast<void*>(p.w), dims, str, box, "conv_tc: W", CU_TENSOR_MAP_SWIZZLE_64B);
     if (rc) return rc;
   }
+  if (int rc = encode_out_maps(&om, p, p.Wo, p.Ho, p.B, SC_BW, SC_BH, (uint64_t)p.out_bs)) return rc;
+  auto run = [&](auto blockn_tag, auto out_tag) -> int {
+    constexpr int BN_ = decltype(blockn_tag)::value;
+    return launch_persistent<conv_tc_smallc_kernel<BN_, decltype(out_tag)>, sc_smem_bytes<BN_>()>("conv_tc_smallc_kernel", kp.total_tiles, NUM_THREADS, st, ta, tb,
+                                                                                                 om.d, om.d2, kp);
+  };
+  typedef std::integral_constant<int, 32> N32;
+  typedef std::integral_constant<int, 64> N64;
   const bool outp = p.out_dtype == FB200_F16PAIR;
-  {
-    const uint64_t OP = (uint64_t)p.out_pitch;
-    const uint64_t dims[4] = {(uint64_t)p.Cout, (uint64_t)p.Wo, (uint64_t)p.Ho, (uint64_t)p.B};
-    const uint64_t str[4] = {1, OP, OP * p.Wo, (uint64_t)p.out_bs};
-    const uint32_t box[4] = {32, SC_BW, SC_BH, 1};
-    int rc;
-    if (outp) {  // two fp16 planes, 32-channel boxes with 64-byte swizzle
-      rc = encode(&td, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, p.out, dims, str, box, "D(hi)", CU_TENSOR_MAP_SWIZZLE_64B);
-      if (!rc) rc = encode(&td2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, static_cast<__half*>(p.out) + p.out_lo_off, dims, str, box, "D(lo)", CU_TENSOR_MAP_SWIZZLE_64B);
-    } else {
-      rc = encode(&td, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 4, p.out, dims, str, box, "D");
-      td2 = td;
-    }
-    if (rc) return rc;
-  }
-  if (p.Cout == 32) return outp ? launch_smallc<32, PairOut>(ta, tb, td, td2, kp, st) : launch_smallc<32, float>(ta, tb, td, td2, kp, st);
-  return outp ? launch_smallc<64, PairOut>(ta, tb, td, td2, kp, st) : launch_smallc<64, float>(ta, tb, td, td2, kp, st);
+  if (p.Cout == 32) return outp ? run(N32{}, PairOut{}) : run(N32{}, float{});
+  return outp ? run(N64{}, PairOut{}) : run(N64{}, float{});
 }
 
 }  // namespace tc
@@ -767,6 +659,7 @@ static int conv2d_tc_smallc(const ConvParams& p, cudaStream_t st) {
 bool conv2d_tc_supported(const ConvParams& p, int x_dtype, int out_dtype) {
   if (x_dtype != FB200_F16) return false;
   if (out_dtype != FB200_F16 && out_dtype != FB200_F32 && out_dtype != FB200_F16PAIR) return false;
+  if (p.split3 && out_dtype == FB200_F16) return false;  // split-precision convs write fp32 or the pair
   const int Clog = p.split3 ? p.Cin / 3 : p.Cin;  // channels of one K segment
   if (out_dtype == FB200_F16PAIR) {  // pair output: fused-split layers, planes 16-byte aligned
     if (!p.split3 || p.rowmax || p.w_bs != 0 || p.Cout % 8 != 0) return false;
@@ -802,11 +695,10 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   kp.KH = p.KH; kp.KW = p.KW; kp.pad = p.pad;
   const int Clog = p.split3 ? p.Cin / 3 : p.Cin;
   const int BK = (Clog % 64 == 0) ? 64 : 32;
-  kp.seg_chunks = p.split3 ? Clog / BK : 0;
   kp.lo_off = (p.split3 && p.x_lo_off) ? (int)p.x_lo_off : Clog;
   kp.w_seg = Clog;
   const CUtensorMapSwizzle swz = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  kp.cchunks = p.Cin / BK; kp.x_pitch = p.x_pitch;
+  kp.cchunks = Clog / BK; kp.x_pitch = p.x_pitch;  // split-precision: a k-block is (tap, channel chunk) with the hi / lo halves of both operands together
   kp.stride2 = (p.stride != 2) ? 0 : (p.H % 2 == 0 && p.W % 2 == 0) ? 1 : 2;
   kp.num_k_blocks = p.KH * p.KW * kp.cchunks;
   // geometry: 1x1 stride-1 convs and linears flatten to W = M, H = 1, B = 1
@@ -823,14 +715,15 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   kp.BW = BW; kp.BH = BH; kp.tiles_w = (Wo + BW - 1) / BW; kp.tiles_h = (Ho + BH - 1) / BH; kp.Ho = Ho; kp.Wo = Wo;
   const int64_t m_tiles = (int64_t)B * kp.tiles_w * kp.tiles_h;
 
-  CUtensorMap ta, tb, td;
+  CUtensorMap ta, tb;
+  OutMaps om;
   int rc;
   const uint64_t P = (uint64_t)p.x_pitch;
   if (!kp.stride2) {
     const uint64_t dims[4] = {(uint64_t)(p.split3 ? kp.lo_off + Clog : p.Cin), (uint64_t)W, (uint64_t)H, (uint64_t)B};
     const uint64_t str[4] = {1, P, P * W, P * W * H};
     const uint32_t box[4] = {(uint32_t)BK, (uint32_t)BW, (uint32_t)BH, 1};
-    rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "A", swz);
+    rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "conv_tc: A", swz);
   } else if (kp.stride2 == 2) {
     // odd H or W: the true (c, w, h, b) geometry, every other pixel of a 2BW x 2BH box.  The last tile's box runs one row / column past the
     // map, which the TMA unit zero-fills like the conv padding.  choose_tile keeps BW, BH <= 128, so the box stays within 256.
@@ -838,13 +731,15 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
     const uint64_t str[4] = {1, P, P * W, P * W * H};
     const uint32_t box[4] = {(uint32_t)BK, 2 * (uint32_t)BW, 2 * (uint32_t)BH, 1};
     const uint32_t estr[4] = {1, 2, 2, 1};
-    rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "A(s2 odd)", swz, estr);
+    rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.x), dims, str, box, "conv_tc: A(s2 odd)", swz, estr);
   } else {
     const uint64_t dims[5] = {2 * P, (uint64_t)W / 2, 2, (uint64_t)H / 2, (uint64_t)B};
     const uint64_t str[5] = {1, 2 * P, P * W, 2 * P * W, P * W * H};
     const uint32_t box[5] = {(uint32_t)BK, (uint32_t)BW, 1, (uint32_t)BH, 1};
-    rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 5, const_cast<void*>(p.x), dims, str, box, "A(s2)", swz);
+    rc = encode(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 5, const_cast<void*>(p.x), dims, str, box, "conv_tc: A(s2)", swz);
   }
+  if (rc) return rc;
+  rc = encode_out_maps(&om, p, Wo, Ho, B, BW, BH, flat ? (uint64_t)p.out_pitch * Wo * Ho : (uint64_t)p.out_bs);
   if (rc) return rc;
 
   auto run = [&](auto blockn_tag, auto stages_tag, auto bk_tag, auto gelu_tag, auto fs_tag) -> int {
@@ -857,68 +752,28 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
       const uint64_t dims[3] = {(uint64_t)p.K, (uint64_t)p.Cout, (uint64_t)p.B};
       const uint64_t str[3] = {1, (uint64_t)p.K, (uint64_t)p.w_bs};
       const uint32_t box[3] = {(uint32_t)BK_, (uint32_t)BN_, 1};
-      int r2 = encode(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, p.w_bs ? 3 : 2, const_cast<void*>(p.w), dims, str, box, "W", swz);
+      int r2 = encode(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, p.w_bs ? 3 : 2, const_cast<void*>(p.w), dims, str, box, "conv_tc: W", swz);
       if (r2) return r2;
     }
-    const bool out16 = p.out_dtype == FB200_F16;
-    const bool outp = p.out_dtype == FB200_F16PAIR;
-    CUtensorMap tr, td2, tr2;
-    if (outp) {  // two fp16 planes (hi at `out`, lo `out_lo_off` elements further), 32-channel boxes with 64-byte swizzle
-      const uint64_t OP = (uint64_t)p.out_pitch;
-      const uint64_t dims[4] = {(uint64_t)p.Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B};
-      const uint64_t str[4] = {1, OP, OP * Wo, flat ? OP * Wo * Ho : (uint64_t)p.out_bs};
-      const uint32_t box[4] = {32, (uint32_t)BW, (uint32_t)BH, 1};
-      int r2 = encode(&td, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, p.out, dims, str, box, "D(hi)", CU_TENSOR_MAP_SWIZZLE_64B);
-      if (r2) return r2;
-      r2 = encode(&td2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, static_cast<__half*>(p.out) + p.out_lo_off, dims, str, box, "D(lo)", CU_TENSOR_MAP_SWIZZLE_64B);
-      if (r2) return r2;
-      tr = td; tr2 = td2;
-      if (p.res) {
-        const uint64_t RP = (uint64_t)p.res_pitch;
-        const uint64_t rstr[4] = {1, RP, RP * Wo, RP * Wo * Ho};
-        r2 = encode(&tr, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(p.res), dims, rstr, box, "R(hi)", CU_TENSOR_MAP_SWIZZLE_64B);
-        if (r2) return r2;
-        r2 = encode(&tr2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<__half*>(static_cast<const __half*>(p.res)) + p.res_lo_off, dims, rstr, box, "R(lo)", CU_TENSOR_MAP_SWIZZLE_64B);
-        if (r2) return r2;
-      }
-    } else {
-      const uint64_t OP = (uint64_t)p.out_pitch;
-      const uint64_t dims[4] = {(uint64_t)p.Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B};
-      const uint64_t str[4] = {1, OP, OP * Wo, flat ? OP * Wo * Ho : (uint64_t)p.out_bs};
-      const uint32_t box[4] = {(uint32_t)(out16 ? 64 : 32), (uint32_t)BW, (uint32_t)BH, 1};
-      int r2 = encode(&td, out16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out16 ? 2 : 4, 4, p.out, dims, str, box, "D");
-      if (r2) return r2;
-      td2 = td; tr = td; tr2 = td;  // residual: same geometry as the output, its own pointer / pitch
-      if (p.res) {
-        const uint64_t RP = (uint64_t)p.res_pitch;
-        const uint64_t rstr[4] = {1, RP, RP * Wo, RP * Wo * Ho};
-        r2 = encode(&tr, out16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out16 ? 2 : 4, 4, const_cast<void*>(p.res), dims, rstr, box, "R");
-        if (r2) return r2;
-      }
-    }
-    KParams k2 = kp;
-    if constexpr (FS_) {  // fused split: k-blocks run over (tap, channel chunk); the hi / lo halves of both operands travel together
-      k2.cchunks = Clog / BK_;
-      k2.num_k_blocks = p.KH * p.KW * k2.cchunks;
-      k2.seg_chunks = 0;
-    }
-    k2.n_tiles = (p.Cout + BN_ - 1) / BN_;
-    const int64_t total = m_tiles * k2.n_tiles;
+    kp.n_tiles = (p.Cout + BN_ - 1) / BN_;
+    const int64_t total = m_tiles * kp.n_tiles;
     if (total > 0x7fffffffLL) { set_error("conv_tc: too many tiles (%lld)", (long long)total); return FB200_ERR_UNSUPPORTED; }
-    k2.total_tiles = (int)total;
-    if constexpr (decltype(gelu_tag)::value) return launch<BN_, ST_, __half, BK_, NS_, true>(ta, tb, td, tr, td2, tr2, k2, st);
-    else if constexpr (FS_) {  // fp32 or pair output (checked by the caller)
-      if (outp) return launch<BN_, ST_, PairOut, BK_, NS_, false, true>(ta, tb, td, tr, td2, tr2, k2, st);
-      return launch<BN_, ST_, float, BK_, NS_, false, true>(ta, tb, td, tr, td2, tr2, k2, st);
-    } else {
+    kp.total_tiles = (int)total;
+    auto launch = [&](auto out_tag) -> int {
+      return launch_persistent<conv_tc_kernel<BN_, ST_, decltype(out_tag), BK_, NS_, decltype(gelu_tag)::value, FS_>, smem_bytes<BN_, ST_, BK_, NS_, FS_>()>(
+          "conv_tc_kernel", kp.total_tiles, NUM_THREADS, st, ta, tb, om.d, om.r, om.d2, om.r2, kp);
+    };
+    const bool outp = p.out_dtype == FB200_F16PAIR;
+    if constexpr (decltype(gelu_tag)::value) return launch(__half{});
+    else if constexpr (FS_) return outp ? launch(PairOut{}) : launch(float{});  // fp32 or pair output (checked by the caller)
+    else {
       if (outp) { set_error("conv_tc: pair output is only produced by the fused-split configurations"); return FB200_ERR_UNSUPPORTED; }
-      if (out16) return launch<BN_, ST_, __half, BK_, NS_, false>(ta, tb, td, tr, td2, tr2, k2, st);
-      return launch<BN_, ST_, float, BK_, NS_, false>(ta, tb, td, tr, td2, tr2, k2, st);
+      return p.out_dtype == FB200_F16 ? launch(__half{}) : launch(float{});
     }
   };
   using std::integral_constant;
-  typedef std::false_type NF;  // segmented K (or no split)
-  typedef std::true_type FS;   // fused split
+  typedef std::false_type NF;  // fp16 operands, one product
+  typedef std::true_type FS;   // split-precision operands, fused split
   typedef integral_constant<int, 64> K64;
   typedef integral_constant<int, 32> K32;
   typedef integral_constant<int, 128> N128;
@@ -927,8 +782,7 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   typedef integral_constant<int, 3> S3;
   if ((p.act & 15) == FB200_ACT_GELU)  // exact-erf GELU: dedicated instantiation (fp16 out, Cin % 64 == 0; checked in conv2d_tc_supported)
     return run(N128{}, S4{}, K64{}, std::true_type{}, NF{});
-  // fp32-accurate mode: fused split (one TMA pass over A_hi, A_lo, W_hi, W_lo per chunk instead of three segmented passes over the operands)
-  if (p.split3 && (p.out_dtype == FB200_F32 || p.out_dtype == FB200_F16PAIR)) {
+  if (p.split3) {  // fp32-accurate mode: fused split (one TMA pass over A_hi, A_lo, W_hi, W_lo per chunk feeds the three products)
     if (BK == 64) {
       if (p.Cout > 64) return run(N128{}, S3{}, K64{}, std::false_type{}, FS{});   // 3 x 64 + 32 KiB
       return run(N64{}, S4{}, K64{}, std::false_type{}, FS{});                     // 4 x 48 + 32 KiB

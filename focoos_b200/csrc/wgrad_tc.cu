@@ -19,6 +19,7 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace fb200 {
@@ -39,26 +40,6 @@ struct WParams {
   int single;                          // 1: plain fp16 operands, ONE product per chunk (the reference's fp16-autocast numerics class); 0: [hi | lo] pairs, three products
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count)); }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done = 0, spins = 0;
-  while (true) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    if (done) break;
-    if (++spins > (1u << 26)) __trap();  // a descriptor / phase bug must not hang the GPU
-  }
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
 // MN-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 format): LBO = stride between 64-element MN blocks, SBO = stride between 8-row K groups
 __device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
   uint64_t d = 0;
@@ -194,35 +175,13 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ part, int splits, 
   out[i] = accumulate ? out[i] + s : s;
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess) fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
 // pair tensor [B,H,W,2C] fp16 -> 4-D map (channel, w, h, b) with a 64-channel x BW x BH box, SWIZZLE_128B, OOB = zero
 static int encode_pair(CUtensorMap* m, const void* base, int C2, int W, int H, int B, int BW, int BH, const char* what, int stride = 1) {
-  EncodeTiledFn fn = get_encode();
-  if (!fn) { set_error("wgrad_tc: cuTensorMapEncodeTiled unavailable"); return FB200_ERR_CUDA; }
-  const cuuint64_t gdim[4] = {(cuuint64_t)C2, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  const cuuint64_t gstr[3] = {(cuuint64_t)C2 * 2, (cuuint64_t)C2 * 2 * W, (cuuint64_t)C2 * 2 * W * H};
+  const uint64_t C = (uint64_t)C2;
+  const uint64_t dims[4] = {C, (uint64_t)W, (uint64_t)H, (uint64_t)B}, str[4] = {1, C, C * W, C * W * H};
   // with a traversal stride s the box spans s*BW x s*BH input pixels and delivers ceil(s*BW / s) x ceil(s*BH / s) = BW x BH of them
-  const cuuint32_t box[4] = {64, (cuuint32_t)(BW * stride), (cuuint32_t)(BH * stride), 1}, estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("wgrad_tc: cuTensorMapEncodeTiled(%s) failed with %d (C2=%d W=%d H=%d B=%d box %dx%d)", what, (int)r, C2, W, H, B, BW, BH); return FB200_ERR_CUDA; }
-  return FB200_OK;
-}
-
-static int num_sms() {
-  static int n = 0;
-  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
-  return n;
+  const uint32_t box[4] = {64, (uint32_t)(BW * stride), (uint32_t)(BH * stride), 1}, estr[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
+  return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, const_cast<void*>(base), dims, str, box, what, CU_TENSOR_MAP_SWIZZLE_128B, estr);
 }
 
 // pixel rectangle with EXACTLY 64 pixels (power-of-two width), maximising the covered fraction of the Ho x Wo map
@@ -289,9 +248,9 @@ static int wgrad_tc_launch(const void* x_pair, int B, int H, int W, int Cin, con
   const Plan pl = make_plan(B, Ho, Wo, Cin, Cout, taps);
   CUtensorMap tdy, tx;
   const int planes = single ? 1 : 2;  // channels per pixel of the operand tensors: C (plain fp16) or 2C ([hi | lo] pair)
-  int rc = encode_pair(&tdy, dy_pair, planes * Cout, Wo, Ho, B, pl.BW, pl.BH, "dY");
+  int rc = encode_pair(&tdy, dy_pair, planes * Cout, Wo, Ho, B, pl.BW, pl.BH, "wgrad_tc: dY");
   if (rc) return rc;
-  rc = encode_pair(&tx, x_pair, planes * Cin, W, H, B, pl.BW, pl.BH, "X", stride);
+  rc = encode_pair(&tx, x_pair, planes * Cin, W, H, B, pl.BW, pl.BH, "wgrad_tc: X", stride);
   if (rc) return rc;
   WParams p;
   p.Cout = Cout; p.Cin = Cin; p.KH = KH; p.KW = KW; p.pad = pad; p.stride = stride;
@@ -304,18 +263,9 @@ static int wgrad_tc_launch(const void* x_pair, int B, int H, int W, int Cin, con
   p.part = reinterpret_cast<float*>(workspace);
   p.single = single;
   cudaStream_t st = (cudaStream_t)stream;
-  const unsigned grid = (unsigned)(items < num_sms() ? items : num_sms());
-  if (pl.block_n == 128) {
-    static bool cfg = false;
-    if (!cfg) { cudaFuncSetAttribute(wgrad_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<128>()); cfg = true; }
-    static_assert(smem_bytes<128>() <= 227 * 1024, "shared memory budget exceeded");
-    wgrad_tc_kernel<128><<<grid, 384, smem_bytes<128>(), st>>>(tdy, tx, p);
-  } else {
-    static bool cfg = false;
-    if (!cfg) { cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<64>()); cfg = true; }
-    wgrad_tc_kernel<64><<<grid, 384, smem_bytes<64>(), st>>>(tdy, tx, p);
-  }
-  FB_CHECK_LAUNCH("conv_wgrad_tc");
+  rc = pl.block_n == 128 ? launch_persistent<wgrad_tc_kernel<128>, smem_bytes<128>()>("conv_wgrad_tc", items, 384, st, tdy, tx, p)
+                         : launch_persistent<wgrad_tc_kernel<64>, smem_bytes<64>()>("conv_wgrad_tc", items, 384, st, tdy, tx, p);
+  if (rc) return rc;
   const int64_t n = (int64_t)Cout * taps * Cin;
   wgrad_reduce_kernel<<<(unsigned)cdiv(n, 256), 256, 0, st>>>(p.part, pl.splits, n, dw, accumulate);
   FB_CHECK_LAUNCH("conv_wgrad_tc(reduce)");

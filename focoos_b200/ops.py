@@ -692,8 +692,9 @@ def conv2d(x, w, scale=None, bias=None, *, stride=1, pad=0, act=ACT_NONE, residu
     """NHWC conv with fused per-channel scale/bias (folded BN), residual add and activation.
     w: [Cout,KH,KW,Cin] (same dtype as x).  `out` may be a channel slice of a wider NHWC buffer."""
     assert x.dim() == 4 and w.dim() == 4 and w.is_contiguous() and w.dtype == x.dtype
-    if algo == ALGO_TCGEN05_SPLIT3:  # x = [hi|lo] pair (2C channels), w = [W_hi|W_lo|W_hi] (3C)
+    if algo == ALGO_TCGEN05_SPLIT3:  # x = [hi|lo] pair (2C channels), w = [W_hi|W_lo|W_hi] (3C), fp32 out
         assert x.dtype == torch.float16 and w.shape[3] * 2 == x.shape[3] * 3
+        out_dtype = out_dtype or torch.float32
     else:
         assert w.shape[3] == x.shape[3]
     B, H, W, _ = x.shape

@@ -38,7 +38,8 @@ typedef enum { FB200_ACT_NONE = 0, FB200_ACT_RELU = 1, FB200_ACT_SILU = 2, FB200
                FB200_ACT_RESIDUAL_AFTER = 16 /* OR-ed flag: out = act(conv) + residual instead of act(conv + residual) */ } fb200_act;
 typedef enum { FB200_ALGO_AUTO = 0, FB200_ALGO_SIMT = 1, FB200_ALGO_TCGEN05 = 2,
                /* fp32-accurate products on the fp16 tensor cores: x is the [hi|lo] fp16 pair of an fp32 tensor (fb200_split_f32_pair),
-                * w = [Cout][KH][KW][W_hi|W_lo|W_hi]; computes hi*W_hi + hi*W_lo + lo*W_hi with fp32 accumulation (error ~2^-21). */
+                * w = [Cout][KH][KW][W_hi|W_lo|W_hi]; computes hi*W_hi + hi*W_lo + lo*W_hi with fp32 accumulation (error ~2^-21).
+                * The output is FB200_F32 or FB200_F16PAIR; an FB200_F16 output is FB200_ERR_UNSUPPORTED. */
                FB200_ALGO_TCGEN05_SPLIT3 = 3 } fb200_algo;
 
 const char* fb200_last_error(void);

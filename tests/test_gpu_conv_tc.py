@@ -118,6 +118,17 @@ def test_split_precision_conv_matches_fp32(B, H, W, Cin, Cout, k, stride, res):
     assert err <= 2e-5 * scale, f"split-precision conv: max|d|={err:.3e} scale={scale:.2e}"
 
 
+def test_split_precision_conv_has_no_fp16_output():
+    """a split-precision conv writes fp32 or the pair: an fp16 output is refused on the host, before any launch, and fp32 is the default"""
+    from focoos_b200.fai_detr import _split3_weights
+
+    xp = ops.split_pair(rnd((2, 20, 20, 64), torch.float32, 1).to(DEV))
+    w3 = _split3_weights(rnd((64, 3, 3, 64), torch.float32, 2, 0.04)).to(DEV)
+    with pytest.raises(RuntimeError, match=r"\(-2\).*tensor-core path does not support.*split-precision convs write fp32 or the fp16 pair"):
+        ops.conv2d(xp, w3, pad=1, act=ops.ACT_RELU, out_dtype=torch.float16, algo=ops.ALGO_TCGEN05_SPLIT3)
+    assert ops.conv2d(xp, w3, pad=1, act=ops.ACT_RELU, algo=ops.ALGO_TCGEN05_SPLIT3).dtype == torch.float32
+
+
 @pytest.mark.parametrize("dtype", [torch.float16, torch.float32])
 @pytest.mark.parametrize("B,H,W,C,Q", [(3, 40, 52, 256, 100), (2, 64, 128, 128, 100), (5, 8, 8, 64, 7)])
 def test_per_image_weights_product(B, H, W, C, Q, dtype):
