@@ -50,7 +50,7 @@ def conv_any(x, w_khwc, bias, stride: int, pad: int, precision: str, act=ops.ACT
         return (y, x16) if return_pair else y
     if ok:
         xp = x_pair if x_pair is not None else ops.split_pair(x)
-        y = ops.conv2d(xp, _split3_weights(w_khwc), None, bias, stride=stride, pad=pad, act=act, out_dtype=torch.float32, algo=ops.ALGO_TCGEN05_SPLIT3)
+        y = ops.conv2d_pair(ops.Pair(xp), _split3_weights(w_khwc), None, bias, stride=stride, pad=pad, act=act, out_pair=False)
         return (y, xp) if return_pair else y
     if w_khwc.dtype != x.dtype:  # an "amp" caller packed the weight in fp16 but the shape does not take the tensor-core path: the CUDA-core kernel wants one dtype
         w_khwc = w_khwc.to(x.dtype)

@@ -87,7 +87,7 @@ struct ConvParams {
   int B, H, W, Cin, x_pitch, KH, KW, stride, pad, Ho, Wo, Cout, res_pitch, out_pitch, act;
   int64_t M; int K; int x_dtype, out_dtype, vec_ok; int split3; int64_t out_bs;  // out_bs: elements between images of `out`
   int64_t w_bs = 0;  // elements between the per-image weight sets (0 = one shared weight tensor)
-  int64_t x_lo_off = 0;     // split3: elements from the hi plane of x to its lo plane (0 = Cin/3, the dense [hi|lo] tensor)
+  int64_t x_lo_off = 0;     // split3: elements from the hi plane of x to its lo plane
   int64_t out_lo_off = 0, res_lo_off = 0;  // out_dtype == FB200_F16PAIR: elements from the hi plane to the lo plane of out / residual
   float* rowmax = nullptr;  // not null: no output tensor, only max over the Cout columns of every row (atomic max into a buffer pre-filled with -inf)
 };

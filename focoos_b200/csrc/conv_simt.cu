@@ -446,129 +446,55 @@ extern "C" int fb200_stem_conv3x3s2_u8(const uint8_t* img_nhwc, int B, int H, in
   return stem_launch(img_nhwc, true, B, H, W, w, scale, bias, mean3, std3, act, out, out_dtype, Cout, stream);
 }
 
-extern "C" int fb200_linear_rowmax_pair(const void* x, int64_t M, int K, int x_pitch, int64_t x_lo_off, const void* w3, const float* bias, int Cout, float* rowmax, void* stream) {
-  FB_CHECK_ARG(x && w3 && rowmax && M > 0 && M <= 0x7fffffffLL && K > 0 && Cout > 0, "linear_rowmax_pair: bad arguments");
-  FB_CHECK_ARG(x_lo_off >= K && x_pitch >= x_lo_off + K && K % 64 == 0, "linear_rowmax_pair: K must be a multiple of 64 and the lo plane must lie inside the row pitch");
-  ConvParams p;
-  p.split3 = 1;
-  p.x = x; p.w = w3; p.scale = nullptr; p.bias = bias; p.res = nullptr;
-  p.out = const_cast<void*>(x);  // never written
-  p.B = 1; p.H = 1; p.W = (int)M; p.Cin = 3 * K; p.x_pitch = x_pitch; p.KH = 1; p.KW = 1; p.stride = 1; p.pad = 0; p.Ho = 1; p.Wo = (int)M;
-  p.Cout = Cout; p.res_pitch = 0; p.out_pitch = (Cout + 3) / 4 * 4; p.act = FB200_ACT_NONE;
-  p.M = M; p.K = 3 * K; p.x_dtype = FB200_F16; p.out_dtype = FB200_F32; p.vec_ok = 1;
-  p.out_bs = (int64_t)M * p.out_pitch;
-  p.x_lo_off = x_lo_off;
-  p.rowmax = rowmax;
-  if (!conv2d_tc_supported(p, FB200_F16, FB200_F32)) {
-    set_error("linear_rowmax_pair: shape not supported by the tensor-core split path (K=%d)", K);
-    return FB200_ERR_UNSUPPORTED;
-  }
-  return conv2d_tc(p, (cudaStream_t)stream);
+// The ConvParams of every conv entry point.  x_lo_off != 0: x is the hi plane of a pair with C logical channels and w the [W_hi | W_lo | W_hi] triple,
+// so K runs over 3C per tap (the fp32-accurate split products); otherwise Cin = C.  out_batch_stride 0: dense images of Ho x Wo x out_pitch.
+static int conv_params(ConvParams* q, const char* who, const void* x, int x_dtype, int B, int H, int W, int C, int x_pitch, int64_t x_lo_off, const void* w,
+                       int64_t w_bs, int KH, int KW, int stride, int pad, const float* scale, const float* bias, const void* residual, int res_pitch,
+                       int64_t res_lo_off, int act, void* out, int out_dtype, int out_pitch, int64_t out_lo_off, int64_t out_batch_stride, int Cout) {
+  FB_CHECK_ARG(x && w && out, "%s: null pointer", who);
+  FB_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && Cout > 0 && KH > 0 && KW > 0 && stride > 0 && pad >= 0, "%s: bad shape", who);
+  ConvParams& p = *q;
+  p.split3 = x_lo_off != 0;
+  p.x = x; p.w = w; p.scale = scale; p.bias = bias; p.res = residual; p.out = out;
+  p.B = B; p.H = H; p.W = W; p.Cin = p.split3 ? 3 * C : C; p.x_pitch = x_pitch; p.KH = KH; p.KW = KW; p.stride = stride; p.pad = pad;
+  p.Ho = (H + 2 * pad - KH) / stride + 1; p.Wo = (W + 2 * pad - KW) / stride + 1;
+  FB_CHECK_ARG(p.Ho > 0 && p.Wo > 0, "%s: empty output", who);
+  p.Cout = Cout; p.res_pitch = res_pitch; p.out_pitch = out_pitch; p.act = act;
+  p.M = (int64_t)B * p.Ho * p.Wo; p.K = KH * KW * p.Cin; p.x_dtype = x_dtype; p.out_dtype = out_dtype;
+  p.out_bs = out_batch_stride > 0 ? out_batch_stride : (int64_t)p.Ho * p.Wo * out_pitch;
+  p.vec_ok = (out_pitch % 4 == 0) && (!residual || res_pitch % 4 == 0) && (p.out_bs % 4 == 0);  // the SIMT epilogue's 16-byte stores
+  p.w_bs = w_bs;
+  FB_CHECK_ARG(w_bs == 0 || w_bs >= (int64_t)Cout * p.K, "%s: weight batch stride smaller than one weight set", who);
+  FB_CHECK_ARG(w_bs == 0 || !residual, "%s: per-image weights take no residual", who);
+  p.x_lo_off = x_lo_off; p.out_lo_off = out_lo_off; p.res_lo_off = res_lo_off;
+  return FB200_OK;
 }
 
-static int conv2d_impl(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int64_t w_bs, int KH,
-                       int KW, int stride, int pad, const float* scale, const float* bias, const void* residual,
-                       int res_pitch, int act, void* out, int out_dtype, int out_pitch, int64_t out_batch_stride, int Cout,
-                       int algo, void* stream);
-
-extern "C" int fb200_conv2d(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int KH,
+extern "C" int fb200_conv2d(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int64_t w_batch_stride, int KH,
                             int KW, int stride, int pad, const float* scale, const float* bias, const void* residual,
                             int res_pitch, int act, void* out, int out_dtype, int out_pitch, int64_t out_batch_stride, int Cout,
                             int algo, void* stream) {
-  return conv2d_impl(x, x_dtype, B, H, W, Cin, x_pitch, w, 0, KH, KW, stride, pad, scale, bias, residual, res_pitch, act, out, out_dtype, out_pitch, out_batch_stride,
-                     Cout, algo, stream);
-}
-
-extern "C" int fb200_conv2d_per_image_weights(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int64_t w_batch_stride,
-                                              int KH, int KW, int stride, int pad, const float* scale, const float* bias, int act, void* out, int out_dtype,
-                                              int out_pitch, int Cout, int algo, void* stream) {
-  FB_CHECK_ARG(w_batch_stride >= (int64_t)Cout * KH * KW * Cin, "conv2d_per_image_weights: weight batch stride smaller than one weight set");
-  return conv2d_impl(x, x_dtype, B, H, W, Cin, x_pitch, w, w_batch_stride, KH, KW, stride, pad, scale, bias, nullptr, 0, act, out, out_dtype, out_pitch, 0, Cout, algo,
-                     stream);
-}
-
-extern "C" int fb200_conv2d_pair(const void* x, int B, int H, int W, int C, int x_pitch, int64_t x_lo_off, const void* w3, int KH, int KW, int stride, int pad,
-                                 const float* scale, const float* bias, const void* residual, int res_pitch, int64_t res_lo_off, int act, void* out, int out_dtype,
-                                 int out_pitch, int64_t out_lo_off, int64_t out_batch_stride, int Cout, void* stream) {
-  FB_CHECK_ARG(x && w3 && out, "conv2d_pair: null pointer");
-  FB_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && Cout > 0 && KH > 0 && KW > 0 && stride > 0 && pad >= 0, "conv2d_pair: bad shape");
-  FB_CHECK_ARG(out_dtype == FB200_F32 || out_dtype == FB200_F16PAIR, "conv2d_pair: output is fp32 or the fp16 pair");
-  FB_CHECK_ARG(x_lo_off >= C && x_pitch >= x_lo_off + C, "conv2d_pair: the lo plane must lie inside the pixel pitch, after the hi plane");
-  ConvParams p;
-  p.split3 = 1;
-  p.x = x; p.w = w3; p.scale = scale; p.bias = bias; p.res = residual; p.out = out;
-  p.B = B; p.H = H; p.W = W; p.Cin = 3 * C; p.x_pitch = x_pitch; p.KH = KH; p.KW = KW; p.stride = stride; p.pad = pad;
-  p.Ho = (H + 2 * pad - KH) / stride + 1; p.Wo = (W + 2 * pad - KW) / stride + 1;
-  FB_CHECK_ARG(p.Ho > 0 && p.Wo > 0, "conv2d_pair: empty output");
-  p.Cout = Cout; p.res_pitch = res_pitch; p.out_pitch = out_pitch; p.act = act;
-  p.M = (int64_t)B * p.Ho * p.Wo; p.K = KH * KW * 3 * C; p.x_dtype = FB200_F16; p.out_dtype = out_dtype; p.vec_ok = 1;
-  p.out_bs = out_batch_stride > 0 ? out_batch_stride : (int64_t)p.Ho * p.Wo * out_pitch;
-  p.x_lo_off = x_lo_off; p.out_lo_off = out_lo_off; p.res_lo_off = res_lo_off;
-  if (!conv2d_tc_supported(p, FB200_F16, out_dtype)) {
-    set_error("conv2d_pair: shape / alignment not supported by the tensor-core split path (C=%d Cout=%d k=%dx%d s=%d out_dtype=%d)", C, Cout, KH, KW, stride, out_dtype);
-    return FB200_ERR_UNSUPPORTED;
-  }
-  return conv2d_tc(p, (cudaStream_t)stream);
-}
-
-extern "C" int fb200_linear_rowmax(const void* x, int64_t M, int K, int x_pitch, const void* w, const float* bias, int Cout, float* rowmax, void* stream) {
-  FB_CHECK_ARG(x && w && rowmax && M > 0 && M <= 0x7fffffffLL && K > 0 && Cout > 0, "linear_rowmax: bad arguments");
-  ConvParams p;
-  p.split3 = 0;
-  p.x = x; p.w = w; p.scale = nullptr; p.bias = bias; p.res = nullptr;
-  p.out = const_cast<void*>(x);  // never written: the tensor map of the (absent) output only needs a valid aligned address
-  p.B = 1; p.H = 1; p.W = (int)M; p.Cin = K; p.x_pitch = x_pitch; p.KH = 1; p.KW = 1; p.stride = 1; p.pad = 0; p.Ho = 1; p.Wo = (int)M;
-  p.Cout = Cout; p.res_pitch = 0; p.out_pitch = (Cout + 3) / 4 * 4; p.act = FB200_ACT_NONE;
-  p.M = M; p.K = K; p.x_dtype = FB200_F16; p.out_dtype = FB200_F32; p.vec_ok = 1;
-  p.out_bs = (int64_t)M * p.out_pitch;
-  p.rowmax = rowmax;
-  if (!conv2d_tc_supported(p, FB200_F16, FB200_F32)) {
-    set_error("linear_rowmax: shape not supported by the tensor-core path (K=%d must be a multiple of 32, fp16 operands, 16-byte aligned)", K);
-    return FB200_ERR_UNSUPPORTED;
-  }
-  return conv2d_tc(p, (cudaStream_t)stream);
-}
-
-static int conv2d_impl(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int64_t w_bs, int KH,
-                       int KW, int stride, int pad, const float* scale, const float* bias, const void* residual,
-                       int res_pitch, int act, void* out, int out_dtype, int out_pitch, int64_t out_batch_stride, int Cout,
-                       int algo, void* stream) {
-  FB_CHECK_ARG(x && w && out, "conv2d: null pointer");
-  FB_CHECK_ARG(B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && KH > 0 && KW > 0 && stride > 0 && pad >= 0, "conv2d: bad shape");
+  FB_CHECK_ARG(algo == FB200_ALGO_AUTO || algo == FB200_ALGO_SIMT || algo == FB200_ALGO_TCGEN05,
+               "conv2d: unknown algo %d (split-precision products on [hi | lo] pairs are fb200_conv2d_pair)", algo);
   FB_CHECK_ARG(x_pitch >= Cin && out_pitch >= Cout, "conv2d: pitch smaller than channel count");
   ConvParams p;
-  p.split3 = 0;
-  if (algo == FB200_ALGO_TCGEN05_SPLIT3) {  // x = [hi | lo] fp16 pair tensor with Cin = 2C stored channels; w = [Cout][KH][KW][3C]
-    FB_CHECK_ARG(x_dtype == FB200_F16 && Cin % 2 == 0, "conv2d(split3): x must be the fp16 [hi|lo] pair tensor");
-    p.split3 = 1;
-    Cin = (Cin / 2) * 3;  // K runs over hi*W_hi, hi*W_lo, lo*W_hi
-    algo = FB200_ALGO_TCGEN05;
-  }
-  p.x = x; p.w = w; p.scale = scale; p.bias = bias; p.res = residual; p.out = out;
-  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.x_pitch = x_pitch; p.KH = KH; p.KW = KW; p.stride = stride; p.pad = pad;
-  p.Ho = (H + 2 * pad - KH) / stride + 1; p.Wo = (W + 2 * pad - KW) / stride + 1;
-  FB_CHECK_ARG(p.Ho > 0 && p.Wo > 0, "conv2d: empty output");
-  p.Cout = Cout; p.res_pitch = res_pitch; p.out_pitch = out_pitch; p.act = act;
-  p.M = (int64_t)B * p.Ho * p.Wo; p.K = KH * KW * Cin; p.x_dtype = x_dtype; p.out_dtype = out_dtype;
-  p.vec_ok = (out_pitch % 4 == 0) && (!residual || res_pitch % 4 == 0);
-  p.out_bs = out_batch_stride > 0 ? out_batch_stride : (int64_t)p.Ho * p.Wo * out_pitch;
-  p.vec_ok = p.vec_ok && (p.out_bs % 4 == 0);
+  if (int rc = conv_params(&p, "conv2d", x, x_dtype, B, H, W, Cin, x_pitch, 0, w, w_batch_stride, KH, KW, stride, pad, scale, bias, residual, res_pitch, 0, act,
+                           out, out_dtype, out_pitch, 0, out_batch_stride, Cout))
+    return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  p.w_bs = w_bs;
   const bool tc_ok = conv2d_tc_supported(p, x_dtype, out_dtype);
   if (algo == FB200_ALGO_TCGEN05 && !tc_ok) {
-    set_error("conv2d: tensor-core path does not support this shape/dtype (Cin=%d Cout=%d k=%dx%d s=%d dtype=%d/%d); split-precision convs write fp32 or the fp16 pair", Cin,
-              Cout, KH, KW, stride, x_dtype, out_dtype);
+    set_error("conv2d: tensor-core path does not support this shape/dtype (Cin=%d Cout=%d k=%dx%d s=%d dtype=%d/%d)", Cin, Cout, KH, KW, stride, x_dtype, out_dtype);
     return FB200_ERR_UNSUPPORTED;
   }
   if ((algo == FB200_ALGO_AUTO && tc_ok) || algo == FB200_ALGO_TCGEN05) return conv2d_tc(p, st);
-  if (w_bs != 0) {  // CUDA-core path: one launch per image (the parity mode; the tensor-core path batches them)
+  if (w_batch_stride != 0) {  // CUDA-core path: one launch per image (the parity mode; the tensor-core path batches them)
     const size_t xe = x_dtype == FB200_F16 ? 2 : 4, oe = out_dtype == FB200_F16 ? 2 : 4;
     ConvParams q = p;
     q.B = 1; q.M = (int64_t)p.Ho * p.Wo; q.w_bs = 0;
     for (int b = 0; b < B; ++b) {
       q.x = static_cast<const char*>(x) + (size_t)b * H * W * x_pitch * xe;
-      q.w = static_cast<const char*>(w) + (size_t)b * w_bs * xe;
+      q.w = static_cast<const char*>(w) + (size_t)b * w_batch_stride * xe;
       q.out = static_cast<char*>(out) + (size_t)b * p.out_bs * oe;
       const int rc = conv2d_simt(q, x_dtype, out_dtype, st);
       if (rc) return rc;
@@ -576,4 +502,47 @@ static int conv2d_impl(const void* x, int x_dtype, int B, int H, int W, int Cin,
     return FB200_OK;
   }
   return conv2d_simt(p, x_dtype, out_dtype, st);
+}
+
+extern "C" int fb200_conv2d_pair(const void* x, int B, int H, int W, int C, int x_pitch, int64_t x_lo_off, const void* w3, int64_t w_batch_stride, int KH, int KW,
+                                 int stride, int pad, const float* scale, const float* bias, const void* residual, int res_pitch, int64_t res_lo_off, int act,
+                                 void* out, int out_dtype, int out_pitch, int64_t out_lo_off, int64_t out_batch_stride, int Cout, void* stream) {
+  FB_CHECK_ARG(out_dtype == FB200_F32 || out_dtype == FB200_F16 || out_dtype == FB200_F16PAIR, "conv2d_pair: bad output dtype %d", out_dtype);
+  FB_CHECK_ARG(x_lo_off >= C && x_pitch >= x_lo_off + C, "conv2d_pair: the lo plane must lie inside the pixel pitch, after the hi plane");
+  ConvParams p;
+  if (int rc = conv_params(&p, "conv2d_pair", x, FB200_F16, B, H, W, C, x_pitch, x_lo_off, w3, w_batch_stride, KH, KW, stride, pad, scale, bias, residual,
+                           res_pitch, res_lo_off, act, out, out_dtype, out_pitch, out_lo_off, out_batch_stride, Cout))
+    return rc;
+  if (!conv2d_tc_supported(p, FB200_F16, out_dtype)) {
+    set_error("conv2d_pair: tensor-core path does not support this shape / alignment / output (C=%d Cout=%d k=%dx%d s=%d out_dtype=%d); split-precision convs write fp32 or "
+              "the fp16 pair", C, Cout, KH, KW, stride, out_dtype);
+    return FB200_ERR_UNSUPPORTED;
+  }
+  return conv2d_tc(p, (cudaStream_t)stream);
+}
+
+// rowmax: a linear over M rows is the 1x1 conv of one [1, 1, M, K] image whose epilogue keeps only the row maxima; `out` is never written, the tensor
+// map of the absent output only needs a valid aligned address.
+static int linear_rowmax_launch(const char* who, const void* x, int64_t M, int K, int x_pitch, int64_t x_lo_off, const void* w, const float* bias, int Cout,
+                                float* rowmax, void* stream) {
+  FB_CHECK_ARG(x && w && rowmax && M > 0 && M <= 0x7fffffffLL && K > 0 && Cout > 0, "%s: bad arguments", who);
+  ConvParams p;
+  if (int rc = conv_params(&p, who, x, FB200_F16, 1, 1, (int)M, K, x_pitch, x_lo_off, w, 0, 1, 1, 1, 0, nullptr, bias, nullptr, 0, 0, FB200_ACT_NONE,
+                           const_cast<void*>(x), FB200_F32, (Cout + 3) / 4 * 4, 0, 0, Cout))
+    return rc;
+  p.rowmax = rowmax;
+  if (!conv2d_tc_supported(p, FB200_F16, FB200_F32)) {
+    set_error("%s: shape not supported by the tensor-core path (K=%d must be a multiple of 32, fp16 operands, 16-byte aligned)", who, K);
+    return FB200_ERR_UNSUPPORTED;
+  }
+  return conv2d_tc(p, (cudaStream_t)stream);
+}
+
+extern "C" int fb200_linear_rowmax(const void* x, int64_t M, int K, int x_pitch, const void* w, const float* bias, int Cout, float* rowmax, void* stream) {
+  return linear_rowmax_launch("linear_rowmax", x, M, K, x_pitch, 0, w, bias, Cout, rowmax, stream);
+}
+
+extern "C" int fb200_linear_rowmax_pair(const void* x, int64_t M, int K, int x_pitch, int64_t x_lo_off, const void* w3, const float* bias, int Cout, float* rowmax, void* stream) {
+  FB_CHECK_ARG(x_lo_off >= K && x_pitch >= x_lo_off + K && K % 64 == 0, "linear_rowmax_pair: K must be a multiple of 64 and the lo plane must lie inside the row pitch");
+  return linear_rowmax_launch("linear_rowmax_pair", x, M, K, x_pitch, x_lo_off, w3, bias, Cout, rowmax, stream);
 }

@@ -618,7 +618,7 @@ static bool smallc_fits(const ConvParams& p) {
 static int conv2d_tc_smallc(const ConvParams& p, cudaStream_t st) {
   KParams kp{};
   kp.scale = p.scale; kp.bias = p.bias; kp.act = p.act; kp.Cout = p.Cout;
-  kp.lo_off = p.x_lo_off ? (int)p.x_lo_off : 32;
+  kp.lo_off = (int)p.x_lo_off;
   kp.w_seg = 32;
   kp.tiles_w = (p.Wo + SC_BW - 1) / SC_BW; kp.tiles_h = (p.Ho + SC_BH - 1) / SC_BH; kp.Ho = p.Ho; kp.Wo = p.Wo;
   const int64_t total = (int64_t)p.B * kp.tiles_w * kp.tiles_h;
@@ -666,7 +666,7 @@ bool conv2d_tc_supported(const ConvParams& p, int x_dtype, int out_dtype) {
     if ((p.out_lo_off * 2) % 16 != 0 || (p.out_pitch * 2) % 16 != 0 || (p.out_bs * 2) % 16 != 0) return false;
     if (p.res && ((p.res_lo_off * 2) % 16 != 0 || (p.res_pitch * 2) % 16 != 0 || p.Cout % 32 != 0)) return false;
   }
-  if (p.split3 && p.x_lo_off && (p.x_lo_off * 2) % 16 != 0) return false;
+  if (p.split3 && (p.x_lo_off * 2) % 16 != 0) return false;
   if (Clog % 32 != 0 || p.x_pitch % 8 != 0) return false;
   if (p.split3 && p.Cin % 3 != 0) return false;
   if ((reinterpret_cast<uintptr_t>(p.x) | reinterpret_cast<uintptr_t>(p.w) | reinterpret_cast<uintptr_t>(p.out)) & 15) return false;
@@ -695,7 +695,7 @@ int conv2d_tc(const ConvParams& p, cudaStream_t st) {
   kp.KH = p.KH; kp.KW = p.KW; kp.pad = p.pad;
   const int Clog = p.split3 ? p.Cin / 3 : p.Cin;
   const int BK = (Clog % 64 == 0) ? 64 : 32;
-  kp.lo_off = (p.split3 && p.x_lo_off) ? (int)p.x_lo_off : Clog;
+  kp.lo_off = p.split3 ? (int)p.x_lo_off : Clog;
   kp.w_seg = Clog;
   const CUtensorMapSwizzle swz = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   kp.cchunks = Clog / BK; kp.x_pitch = p.x_pitch;  // split-precision: a k-block is (tap, channel chunk) with the hi / lo halves of both operands together

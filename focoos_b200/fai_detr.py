@@ -225,7 +225,7 @@ def aifi_position_embedding(h, w, num_pos_feats=128, temperature=10000.0):
 # the fused graph
 # --------------------------------------------------------------------------------------------------
 def _split3_weights(w):
-    """fp32 [..., C] -> fp16 [..., 3C] = [W_hi | W_lo | W_hi] (operands of FB200_ALGO_TCGEN05_SPLIT3)."""
+    """fp32 [..., C] -> fp16 [..., 3C] = [W_hi | W_lo | W_hi] (the weight operand of fb200_conv2d_pair)."""
     hi = w.half()
     lo = (w - hi.float()).half()
     return torch.cat([hi, lo, hi], dim=-1).contiguous()

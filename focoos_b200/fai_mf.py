@@ -288,7 +288,7 @@ class MFEngine(DetrEngine):
         if self.pair:
             # the same GEMM as three fp16 tensor-core products on the mask_features pair and the per-image embeddings as [W_hi | W_lo | W_hi] triples.
             # (On the CUDA-core fp32 kernel this product was a third of the parity-mode step: 16.9 of 50.4 ms at bs=16 800x800.)
-            ops.conv2d_per_image(mask_features.buf, _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=masks[..., :Q], algo=ops.ALGO_TCGEN05_SPLIT3)
+            ops.conv2d_per_image(mask_features, _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=masks[..., :Q])
         else:
             ops.conv2d_per_image(mask_features, me.reshape(B, Q, 1, 1, C), out=masks[..., :Q], algo=A)
         attn = None

@@ -184,38 +184,32 @@ class CudaBackend:
         self._call("fb200_stem_conv3x3s2_u8" if u8 else "fb200_stem_conv3x3s2", _p(img), B, H, W, _p(w), _p(scale), _p(bias), m, s, act, _p(out), _dt(out), out.shape[-1], _stream())
 
     def conv2d(self, x, w, scale, bias, stride, pad, act, residual, out, algo):
+        """w: [Cout,KH,KW,Cin], or [B,Cout,KH,KW,Cin] with one weight set per image"""
         self._cuda(x, w, out)
         B, H, W, Cin = x.shape
-        Cout, KH, KW, _ = w.shape
+        Cout, KH, KW, _ = w.shape[-4:]
         if _trace is not None:
             _trace_note.append(dict(op="conv", B=B, H=H, W=W, Cin=Cin, Cout=Cout, k=KH, stride=stride, res=residual is not None, xdt=str(x.dtype)[6:], odt=str(out.dtype)[6:], algo=algo))
-        self._call("fb200_conv2d", _p(x), _dt(x), B, H, W, Cin, _pitch(x), _p(w), KH, KW, stride, pad, _p(scale), _p(bias), _p(residual),
-                   0 if residual is None else _pitch(residual), act, _p(out), _dt(out), _pitch(out, True), _batch_stride(out), Cout, algo, _stream())
-
-    def conv2d_per_image(self, x, w, act, out, algo):
-        self._cuda(x, w, out)
-        B, H, W, Cin = x.shape
-        _, Cout, KH, KW, _ = w.shape
-        self._call("fb200_conv2d_per_image_weights", _p(x), _dt(x), B, H, W, Cin, _pitch(x), _p(w), w.stride(0), KH, KW, 1, (KH - 1) // 2, None, None, act,
-                   _p(out), _dt(out), _pitch(out, True), Cout, algo, _stream())
+        self._call("fb200_conv2d", _p(x), _dt(x), B, H, W, Cin, _pitch(x), _p(w), w.stride(0) if w.dim() == 5 else 0, KH, KW, stride, pad, _p(scale), _p(bias),
+                   _p(residual), 0 if residual is None else _pitch(residual), act, _p(out), _dt(out), _pitch(out, True), _batch_stride(out), Cout, algo, _stream())
 
     def linear_rowmax(self, x2d, w, bias, out):
         self._cuda(x2d, w, out)
         self._call("fb200_linear_rowmax", _p(x2d), x2d.shape[0], x2d.shape[1], x2d.stride(0), _p(w), _p(bias), w.shape[0], _p(out), _stream())
 
     def conv2d_pair(self, x, w3, scale, bias, stride, pad, act, residual, out):
-        """x / residual / out: `Pair` (hi + lo fp16 planes) - residual and out may also be plain fp32 tensors (both, or neither)"""
+        """x / residual / out: `Pair` (hi + lo fp16 planes) - residual and out may also be plain fp32 tensors (both, or neither); w3 as w of conv2d"""
         out_pair = isinstance(out, Pair)
         xh = x.hi
         self._cuda(xh, w3, out.hi if out_pair else out)
         B, H, W, C = xh.shape
-        Cout, KH, KW, _ = w3.shape
+        Cout, KH, KW, _ = w3.shape[-4:]
         oh = out.hi if out_pair else out
         rh = None if residual is None else (residual.hi if out_pair else residual)
         if _trace is not None:
             _trace_note.append(dict(op="conv", B=B, H=H, W=W, Cin=C, Cout=Cout, k=KH, stride=stride, res=residual is not None, xdt="pair", odt="pair" if out_pair else "float32", algo=3))
-        self._call("fb200_conv2d_pair", _p(xh), B, H, W, C, _pitch(xh), x.lo_off, _p(w3), KH, KW, stride, pad, _p(scale), _p(bias), _p(rh),
-                   0 if rh is None else _pitch(rh), residual.lo_off if (out_pair and residual is not None) else 0, act, _p(oh), F16PAIR if out_pair else F32,
+        self._call("fb200_conv2d_pair", _p(xh), B, H, W, C, _pitch(xh), x.lo_off, _p(w3), w3.stride(0) if w3.dim() == 5 else 0, KH, KW, stride, pad, _p(scale),
+                   _p(bias), _p(rh), 0 if rh is None else _pitch(rh), residual.lo_off if (out_pair and residual is not None) else 0, act, _p(oh), F16PAIR if out_pair else _dt(oh),
                    _pitch(oh, True), out.lo_off if out_pair else 0, _batch_stride(oh), Cout, _stream())
 
     def image_resize(self, images, out):
@@ -690,18 +684,18 @@ def stem_conv(img: torch.Tensor, w, scale, bias, mean: Sequence[float], std: Seq
 
 def conv2d(x, w, scale=None, bias=None, *, stride=1, pad=0, act=ACT_NONE, residual=None, out=None, out_dtype=None, algo=ALGO_AUTO):
     """NHWC conv with fused per-channel scale/bias (folded BN), residual add and activation.
-    w: [Cout,KH,KW,Cin] (same dtype as x).  `out` may be a channel slice of a wider NHWC buffer."""
-    assert x.dim() == 4 and w.dim() == 4 and w.is_contiguous() and w.dtype == x.dtype
-    if algo == ALGO_TCGEN05_SPLIT3:  # x = [hi|lo] pair (2C channels), w = [W_hi|W_lo|W_hi] (3C), fp32 out
-        assert x.dtype == torch.float16 and w.shape[3] * 2 == x.shape[3] * 3
-        out_dtype = out_dtype or torch.float32
-    else:
-        assert w.shape[3] == x.shape[3]
+    w: [Cout,KH,KW,Cin] (same dtype as x), or [B,Cout,KH,KW,Cin] per image.  `out` may be a channel slice of a wider NHWC buffer.
+    algo=ALGO_TCGEN05_SPLIT3: x is the dense [hi|lo] pair tensor of an fp32 activation and w the [W_hi|W_lo|W_hi] triple - conv2d_pair, fp32 out by default."""
+    assert x.dim() == 4 and w.dim() in (4, 5) and w.is_contiguous() and w.dtype == x.dtype
     B, H, W, _ = x.shape
-    Cout, KH, KW, _ = w.shape
+    Cout, KH, KW, _ = w.shape[-4:]
     Ho, Wo = (H + 2 * pad - KH) // stride + 1, (W + 2 * pad - KW) // stride + 1
+    split = algo == ALGO_TCGEN05_SPLIT3
     if out is None:
-        out = torch.empty((B, Ho, Wo, Cout), dtype=out_dtype or x.dtype, device=x.device)
+        out = torch.empty((B, Ho, Wo, Cout), dtype=out_dtype or (torch.float32 if split else x.dtype), device=x.device)
+    if split:
+        return conv2d_pair(Pair(x), w, scale, bias, stride=stride, pad=pad, act=act, residual=residual, out=out, out_pair=False)
+    assert w.shape[-1] == x.shape[3]
     assert tuple(out.shape) == (B, Ho, Wo, Cout), (tuple(out.shape), (B, Ho, Wo, Cout))
     if residual is not None:
         assert residual.shape == out.shape and residual.dtype == out.dtype
@@ -710,20 +704,13 @@ def conv2d(x, w, scale=None, bias=None, *, stride=1, pad=0, act=ACT_NONE, residu
 
 
 def conv2d_per_image(x, w, *, act=ACT_NONE, out=None, out_dtype=None, algo=ALGO_AUTO):
-    """conv with one weight set per image: x [B,H,W,Cin], w [B,Cout,KH,KW,Cin] -> [B,H,W,Cout]  (the per-query mask product, one launch per batch)."""
-    assert x.dim() == 4 and w.dim() == 5 and w.shape[0] == x.shape[0] and w.dtype == x.dtype and w.stride(-1) == 1
-    if algo == ALGO_TCGEN05_SPLIT3:  # fp32-accurate: x = the [hi|lo] pair of the fp32 activation (2C channels), w = per-image [W_hi|W_lo|W_hi] triples (3C), fp32 out
-        assert x.dtype == torch.float16 and w.shape[-1] * 2 == x.shape[-1] * 3, (w.shape, x.shape)
-        out_dtype = out_dtype or torch.float32
-    else:
-        assert w.shape[-1] == x.shape[-1]
-    B, H, W, _ = x.shape
-    Cout = w.shape[1]
-    if out is None:
-        out = torch.empty((B, H, W, Cout), dtype=out_dtype or x.dtype, device=x.device)
-    assert tuple(out.shape) == (B, H, W, Cout)
-    _be().conv2d_per_image(x, w.contiguous(), act, out, algo)
-    return out
+    """conv with one weight set per image: x [B,H,W,Cin], w [B,Cout,KH,KW,Cin] -> [B,H,W,Cout]  (the per-query mask product, one launch per batch).
+    x may be a Pair: w then holds the per-image [W_hi|W_lo|W_hi] triples and the fp32-accurate product (conv2d_pair) writes fp32."""
+    assert w.dim() == 5 and w.shape[0] == x.shape[0] and w.stride(-1) == 1
+    pad = (w.shape[2] - 1) // 2
+    if isinstance(x, Pair):
+        return conv2d_pair(x, w.contiguous(), pad=pad, act=act, out=out, out_pair=False)
+    return conv2d(x, w.contiguous(), pad=pad, act=act, out=out, out_dtype=out_dtype, algo=algo)
 
 
 def linear_rowmax(x, w, bias=None):
@@ -761,9 +748,9 @@ def to_pair(x) -> Pair:
 def conv2d_pair(x: Pair, w3, scale=None, bias=None, *, stride=1, pad=0, act=ACT_NONE, residual=None, out=None, out_pair: bool = True):
     """fp32-accurate conv (three fp16 wgmma products) on a pair-format input.  `out_pair`: write the result as a Pair (for a following conv / pair pool) or
     as a plain fp32 tensor (for the non-conv consumers: LayerNorm, attention, deformable attention, selection).  The residual has the output's format."""
-    assert isinstance(x, Pair) and w3.dtype == torch.float16 and w3.shape[3] == 3 * x.C, (w3.shape, x.C)
+    assert isinstance(x, Pair) and w3.dtype == torch.float16 and w3.shape[-1] == 3 * x.C, (w3.shape, x.C)
     B, H, W, _ = x.shape
-    Cout, KH, KW, _ = w3.shape
+    Cout, KH, KW, _ = w3.shape[-4:]
     Ho, Wo = (H + 2 * pad - KH) // stride + 1, (W + 2 * pad - KW) // stride + 1
     if out is None:
         out = Pair.empty((B, Ho, Wo, Cout), x.device) if out_pair else torch.empty((B, Ho, Wo, Cout), dtype=torch.float32, device=x.device)

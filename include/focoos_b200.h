@@ -31,16 +31,13 @@ extern "C" {
 
 typedef enum { FB200_OK = 0, FB200_ERR_INVALID = -1, FB200_ERR_UNSUPPORTED = -2, FB200_ERR_CUDA = -3 } fb200_status;
 typedef enum { FB200_F32 = 0, FB200_F16 = 1,
-               /* an fp32 value stored as TWO fp16 planes: hi = fp16(v), lo = fp16(v - hi) (exact to ~2^-22): the operand format of FB200_ALGO_TCGEN05_SPLIT3, accepted as
-                * conv output / residual so that activations stay in it between two convs (fb200_conv2d_pair) */
+               /* an fp32 value stored as TWO fp16 planes: hi = fp16(v), lo = fp16(v - hi) (exact to ~2^-22): the operand format of fb200_conv2d_pair, also accepted
+                * as its output / residual so that activations stay in it between two convs */
                FB200_F16PAIR = 2 } fb200_dtype;
 typedef enum { FB200_ACT_NONE = 0, FB200_ACT_RELU = 1, FB200_ACT_SILU = 2, FB200_ACT_GELU = 3, FB200_ACT_SIGMOID = 4 /* SIMT path only */,
                FB200_ACT_RESIDUAL_AFTER = 16 /* OR-ed flag: out = act(conv) + residual instead of act(conv + residual) */ } fb200_act;
-typedef enum { FB200_ALGO_AUTO = 0, FB200_ALGO_SIMT = 1, FB200_ALGO_TCGEN05 = 2,
-               /* fp32-accurate products on the fp16 tensor cores: x is the [hi|lo] fp16 pair of an fp32 tensor (fb200_split_f32_pair),
-                * w = [Cout][KH][KW][W_hi|W_lo|W_hi]; computes hi*W_hi + hi*W_lo + lo*W_hi with fp32 accumulation (error ~2^-21).
-                * The output is FB200_F32 or FB200_F16PAIR; an FB200_F16 output is FB200_ERR_UNSUPPORTED. */
-               FB200_ALGO_TCGEN05_SPLIT3 = 3 } fb200_algo;
+/* the kernel of fb200_conv2d; the fp32-accurate split-precision products are fb200_conv2d_pair */
+typedef enum { FB200_ALGO_AUTO = 0, FB200_ALGO_SIMT = 1, FB200_ALGO_TCGEN05 = 2 } fb200_algo;
 
 const char* fb200_last_error(void);
 int fb200_version(void);
@@ -65,21 +62,25 @@ int fb200_stem_conv3x3s2_u8(const uint8_t* img_nhwc, int B, int H, int W, const 
  * H=1,W=M tokens: modelling.py:848-882,1204-1207; nn/layers/base.py:51-62).
  *   out[m, n] = act( (sum_k A[m,k] * w[n,k]) * scale[n] + bias[n] + residual[m,n] )
  * x: [B,H,W,Cin] (pitch x_pitch), w: [Cout][KH][KW][Cin] same dtype as x.
+ * w_batch_stride: 0 = one weight set for the batch; otherwise w is [B][Cout][KH][KW][Cin] with w_batch_stride elements between images (at least one
+ * weight set; no residual).  This is the per-query mask product einsum("bqc,bchw->bqhw") of PredictionHeads.forward (models/fai_mf/modelling.py:86,
+ * bisenetformer/modelling.py:364): x = mask features [B,h,w,C], "weights" = the B x Q mask embeddings; one tensor-core launch for the batch.
  * scale/bias: fp32 [Cout] or NULL (=1 / 0).  residual: NULL or same dtype as out, [B,Ho,Wo,Cout]
  * (pitch res_pitch).  out dtype may differ from x dtype (fp32 heads on fp16 features).
  * out_batch_stride: elements between consecutive images of `out` (0 = dense Ho*Wo*out_pitch); lets a level's
  * projection be written straight into its rows of the concatenated [B, sum(HW), C] memory (modelling.py:1165).
- * algo: FB200_ALGO_AUTO picks the tensor-core kernel when dtype==F16 and the shape qualifies. */
-int fb200_conv2d(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int KH, int KW,
+ * algo: FB200_ALGO_AUTO picks the tensor-core kernel when dtype==F16 and the shape qualifies; any value outside fb200_algo is FB200_ERR_INVALID. */
+int fb200_conv2d(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int64_t w_batch_stride, int KH, int KW,
                  int stride, int pad, const float* scale, const float* bias, const void* residual, int res_pitch,
                  int act, void* out, int out_dtype, int out_pitch, int64_t out_batch_stride, int Cout, int algo, void* stream);
 
 /* fp32-accurate conv on pair-format activations (precision "fp32_tc"): x is the HI plane of a [hi | lo] pair tensor with C logical channels, its lo plane
- * `x_lo_off` elements further (pitch x_pitch covers both); w3 = [Cout][KH][KW][W_hi | W_lo | W_hi] (3C); three fp16 tensor-core products per chunk, fp32 accumulation.
+ * `x_lo_off` elements further (pitch x_pitch covers both); w3 = [Cout][KH][KW][W_hi | W_lo | W_hi] (3C), or per image as in fb200_conv2d (w_batch_stride);
+ * hi*W_hi + hi*W_lo + lo*W_hi as three fp16 tensor-core products per chunk, fp32 accumulation (error ~2^-21).
  * out_dtype FB200_F32: fp32 output / residual as in fb200_conv2d.  out_dtype FB200_F16PAIR: the epilogue writes the result AS a pair (hi plane at `out`, lo plane
  * `out_lo_off` elements further, pitch out_pitch) and reads the residual as a pair (`res_lo_off`), so consecutive convs exchange activations without a split pass
  * (replaces the fb200_split_f32_pair launch in front of every conv: nn/layers/conv.py:78-98 chains such as resnet.py:106-121). */
-int fb200_conv2d_pair(const void* x, int B, int H, int W, int C, int x_pitch, int64_t x_lo_off, const void* w3, int KH, int KW, int stride, int pad,
+int fb200_conv2d_pair(const void* x, int B, int H, int W, int C, int x_pitch, int64_t x_lo_off, const void* w3, int64_t w_batch_stride, int KH, int KW, int stride, int pad,
                       const float* scale, const float* bias, const void* residual, int res_pitch, int64_t res_lo_off, int act, void* out, int out_dtype,
                       int out_pitch, int64_t out_lo_off, int64_t out_batch_stride, int Cout, void* stream);
 
@@ -88,13 +89,6 @@ int fb200_conv2d_pair(const void* x, int B, int H, int W, int C, int x_pitch, in
  * align_corners=False) of the FPN / PAN (fai_detr/modelling.py:334,342).  Arithmetic in fp32 on hi + lo, result re-split. */
 int fb200_pair_pool(int mode, const void* x, int64_t x_lo_off, int x_pitch, int B, int H, int W, int C, void* out, int64_t out_lo_off, int out_pitch, int Ho, int Wo,
                     void* stream);
-
-/* Same conv with one weight set PER IMAGE: w [B][Cout][KH][KW][Cin] (w_batch_stride elements apart).  This is the per-query mask product
- * einsum("bqc,bchw->bqhw") of PredictionHeads.forward (models/fai_mf/modelling.py:86, bisenetformer/modelling.py:364): x = mask features
- * [B,h,w,C], "weights" = the B x Q mask embeddings; one launch for the batch (3-D weight tensor map, third coordinate = image). */
-int fb200_conv2d_per_image_weights(const void* x, int x_dtype, int B, int H, int W, int Cin, int x_pitch, const void* w, int64_t w_batch_stride,
-                                   int KH, int KW, int stride, int pad, const float* scale, const float* bias, int act, void* out, int out_dtype,
-                                   int out_pitch, int Cout, int algo, void* stream);
 
 /* rowmax[m] = max_n (x[m,:] . w[n,:] + bias[n]) for fp16 x [M,K] / w [Cout,K] on the tensor cores, WITHOUT writing the [M,Cout] product:
  * the query-selection score enc_outputs_class.max(-1) of _get_decoder_input (models/fai_detr/modelling.py:1204-1214; 268 800 x 365 fp32 logits = 395 MB at

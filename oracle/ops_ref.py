@@ -78,21 +78,24 @@ class RefBackend:
             return
         out.copy_(_act(y, act).permute(0, 2, 3, 1).to(out.dtype))
 
-    def conv2d(self, x, w, scale, bias, stride, pad, act, residual, out, algo):
-        if algo == 3:  # split-precision operands: x = [hi|lo], w = [W_hi|W_lo|W_hi] -> the fp32 values they encode
-            C = x.shape[-1] // 2
-            x = x[..., :C].float() + x[..., C:].float()
-            w = w[..., :C].float() + w[..., C:2 * C].float()
-        y = F.conv2d(x.float().permute(0, 3, 1, 2), w.float().permute(0, 3, 1, 2), None, stride, pad)
+    @staticmethod
+    def _conv(x, w, scale, bias, stride, pad, act, residual):
+        """fp32 NHWC conv + folded BN + residual + activation of both conv entry points; a 5-D w holds one weight set per image"""
+        if w.dim() == 5:
+            return torch.cat([RefBackend._conv(x[b:b + 1], w[b], scale, bias, stride, pad, act, None if residual is None else residual[b:b + 1])
+                              for b in range(x.shape[0])])
+        y = F.conv2d(x.permute(0, 3, 1, 2), w.permute(0, 3, 1, 2), None, stride, pad)
         if scale is not None:
             y = y * scale.view(1, -1, 1, 1)
         if bias is not None:
             y = y + bias.view(1, -1, 1, 1)
         y = y.permute(0, 2, 3, 1)
         post = bool(act & 16)  # FB200_ACT_RESIDUAL_AFTER
-        r = 0.0 if residual is None else residual.float()
-        y = _act(y, act & 15) + r if post else _act(y + r, act & 15)
-        out.copy_(y.to(out.dtype))
+        r = 0.0 if residual is None else residual
+        return _act(y, act & 15) + r if post else _act(y + r, act & 15)
+
+    def conv2d(self, x, w, scale, bias, stride, pad, act, residual, out, algo):
+        out.copy_(self._conv(x.float(), w.float(), scale, bias, stride, pad, act, _f(residual)).to(out.dtype))
 
     @staticmethod
     def _pair_write(pr, v):
@@ -103,16 +106,7 @@ class RefBackend:
     def conv2d_pair(self, x, w3, scale, bias, stride, pad, act, residual, out):
         """the fp32 conv the pair operands encode; pair outputs are re-split exactly as the CUDA epilogue does (hi = fp16(v), lo = fp16(v - hi))"""
         C = x.C
-        xv = x.float()
-        w = w3[..., :C].float() + w3[..., C:2 * C].float()
-        y = F.conv2d(xv.permute(0, 3, 1, 2), w.permute(0, 3, 1, 2), None, stride, pad)
-        if scale is not None:
-            y = y * scale.view(1, -1, 1, 1)
-        if bias is not None:
-            y = y + bias.view(1, -1, 1, 1)
-        y = y.permute(0, 2, 3, 1)
-        r = 0.0 if residual is None else residual.float()
-        y = _act(y, act & 15) + r if (act & 16) else _act(y + r, act & 15)
+        y = self._conv(x.float(), w3[..., :C].float() + w3[..., C:2 * C].float(), scale, bias, stride, pad, act, _f(residual))
         if hasattr(out, "hi"):
             self._pair_write(out, y)
         else:
@@ -316,10 +310,6 @@ class RefBackend:
         if bias is not None:
             y = y + bias
         out.copy_(y.max(-1).values)
-
-    def conv2d_per_image(self, x, w, act, out, algo):
-        for b in range(x.shape[0]):
-            self.conv2d(x[b:b + 1], w[b], None, None, 1, (w.shape[2] - 1) // 2, act, None, out[b:b + 1], algo)
 
     # ---- MaskFormer family ---------------------------------------------------------------------------------------------
     def upsample_nearest_add(self, y, cur, out):

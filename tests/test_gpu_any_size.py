@@ -76,8 +76,7 @@ def _run_tc(x, w, sc, bi, mode):
     if mode == "f16":
         out = ops.conv2d(x, w.to(DEV), sc, bi, stride=2, pad=1, act=ops.ACT_RELU, out_dtype=torch.float16, algo=ops.ALGO_TCGEN05)
     elif mode == "fs32":
-        out = ops.conv2d(ops.split_pair(x), _split3_weights(w).to(DEV), sc, bi, stride=2, pad=1, act=ops.ACT_RELU, out_dtype=torch.float32,
-                         algo=ops.ALGO_TCGEN05_SPLIT3)
+        out = ops.conv2d_pair(ops.to_pair(x), _split3_weights(w).to(DEV), sc, bi, stride=2, pad=1, act=ops.ACT_RELU, out_pair=False)
     else:
         out = ops.conv2d_pair(ops.Pair(ops.split_pair(x)), _split3_weights(w).to(DEV), sc, bi, stride=2, pad=1, act=ops.ACT_RELU, out_pair=True)
     torch.cuda.synchronize()

@@ -111,22 +111,43 @@ def test_split_precision_conv_matches_fp32(B, H, W, Cin, Cout, k, stride, res):
     xp = ops.split_pair(x.to(DEV))
     hi = x.half()
     assert torch.equal(xp.cpu()[..., :Cin], hi) and torch.equal(xp.cpu()[..., Cin:], (x - hi.float()).half())
-    out = ops.conv2d(xp, _split3_weights(w).to(DEV), sc.to(DEV), bi.to(DEV), stride=stride, pad=pad, act=1, residual=None if r is None else r.to(DEV),
-                     out_dtype=torch.float32, algo=ops.ALGO_TCGEN05_SPLIT3)
+    out = ops.conv2d_pair(ops.Pair(xp), _split3_weights(w).to(DEV), sc.to(DEV), bi.to(DEV), stride=stride, pad=pad, act=1, residual=None if r is None else r.to(DEV),
+                          out_pair=False)
     err = float((out.cpu() - ref).abs().max())
     scale = max(1.0, float(ref.abs().max()))
     assert err <= 2e-5 * scale, f"split-precision conv: max|d|={err:.3e} scale={scale:.2e}"
 
 
 def test_split_precision_conv_has_no_fp16_output():
-    """a split-precision conv writes fp32 or the pair: an fp16 output is refused on the host, before any launch, and fp32 is the default"""
+    """a split-precision conv writes fp32 or the pair: an fp16 output is refused on the host, before any launch, and fp32 is the default.  ops.conv2d with
+    ALGO_TCGEN05_SPLIT3 on the dense [hi|lo] tensor is conv2d_pair with a plain output, bit for bit."""
     from focoos_b200.fai_detr import _split3_weights
 
     xp = ops.split_pair(rnd((2, 20, 20, 64), torch.float32, 1).to(DEV))
     w3 = _split3_weights(rnd((64, 3, 3, 64), torch.float32, 2, 0.04)).to(DEV)
     with pytest.raises(RuntimeError, match=r"\(-2\).*tensor-core path does not support.*split-precision convs write fp32 or the fp16 pair"):
         ops.conv2d(xp, w3, pad=1, act=ops.ACT_RELU, out_dtype=torch.float16, algo=ops.ALGO_TCGEN05_SPLIT3)
-    assert ops.conv2d(xp, w3, pad=1, act=ops.ACT_RELU, algo=ops.ALGO_TCGEN05_SPLIT3).dtype == torch.float32
+    out = ops.conv2d(xp, w3, pad=1, act=ops.ACT_RELU, algo=ops.ALGO_TCGEN05_SPLIT3)
+    assert out.dtype == torch.float32
+    assert torch.equal(out, ops.conv2d_pair(ops.Pair(xp), w3, pad=1, act=ops.ACT_RELU, out_pair=False))
+
+
+def test_conv2d_refuses_the_split_algo_and_per_image_weights_with_a_residual():
+    """split-precision products are fb200_conv2d_pair's alone: fb200_conv2d refuses algo 3 (and any other unknown algo); per-image weights take no residual"""
+    be = ops._be()
+    x, out = torch.zeros((2, 8, 8, 64), dtype=torch.float16, device=DEV), torch.zeros((2, 8, 8, 64), dtype=torch.float16, device=DEV)
+    w = torch.zeros((64, 1, 1, 64), dtype=torch.float16, device=DEV)
+    for algo in (3, 7):
+        with pytest.raises(RuntimeError, match=r"\(-1\).*unknown algo.*fb200_conv2d_pair"):
+            be.conv2d(x, w, None, None, 1, 0, ops.ACT_NONE, None, out, algo)
+    w5 = torch.zeros((2, 64, 1, 1, 64), dtype=torch.float16, device=DEV)
+    with pytest.raises(RuntimeError, match=r"\(-1\).*per-image weights take no residual"):
+        be.conv2d(x, w5, None, None, 1, 0, ops.ACT_NONE, torch.zeros_like(out), out, ops.ALGO_AUTO)
+    xp, w35 = ops.Pair(torch.zeros((2, 8, 8, 128), dtype=torch.float16, device=DEV)), torch.zeros((2, 64, 1, 1, 192), dtype=torch.float16, device=DEV)
+    out32 = torch.zeros((2, 8, 8, 64), device=DEV)
+    with pytest.raises(RuntimeError, match=r"\(-1\).*per-image weights take no residual"):
+        be.conv2d_pair(xp, w35, None, None, 1, 0, ops.ACT_NONE, torch.zeros_like(out32), out32)
+    torch.cuda.synchronize()
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.float32])

@@ -89,14 +89,14 @@ def test_masked_attention_split_precision(hw, Q):
 
 @pytest.mark.parametrize("B,h,w,C,Q", [(3, 40, 52, 256, 100), (2, 37, 45, 256, 100), (2, 64, 128, 128, 100), (1, 200, 200, 256, 100)])
 def test_per_image_mask_product_split_precision(B, h, w, C, Q):
-    """einsum("bqc,bchw->bqhw") with per-image weights on the fp32-accurate tensor-core path (fb200_conv2d_per_image_weights, algo TCGEN05_SPLIT3: x = the [hi|lo] pair of
+    """einsum("bqc,bchw->bqhw") with per-image weights on the fp32-accurate tensor-core path (fb200_conv2d_pair with a weight batch stride: x = the Pair of
     mask_features, w = per-image [W_hi|W_lo|W_hi] triples) vs fp64, into the first Q columns of a padded NHWC buffer like MFEngine._heads does."""
     from focoos_b200.fai_detr import _split3_weights
     x, me = rnd((B, h, w, C), torch.float32, 11), rnd((B, Q, C), torch.float32, 12, 0.5)
     ref = torch.einsum("bqc,bhwc->bhwq", me.double(), x.double())
     Qp = (Q + 7) // 8 * 8
     out = torch.zeros((B, h, w, Qp), dtype=torch.float32, device=DEV)
-    ops.conv2d_per_image(ops.split_pair(x.to(DEV)), _split3_weights(me.to(DEV)).reshape(B, Q, 1, 1, 3 * C), out=out[..., :Q], algo=ops.ALGO_TCGEN05_SPLIT3)
+    ops.conv2d_per_image(ops.to_pair(x.to(DEV)), _split3_weights(me.to(DEV)).reshape(B, Q, 1, 1, 3 * C), out=out[..., :Q])
     close(out[..., :Q], ref.float(), 2e-5, "per-image mask product (split)")
     assert float(out[..., Q:].abs().max()) == 0.0, "the padding columns of the buffer must stay untouched"
 

@@ -1,6 +1,7 @@
-"""precision="fp32_tc" host orchestration of the three families on the CPU operator references: the engine's layer call is the only place that picks a
-conv / linear kernel, so the split-precision tensor-core products are reached only through conv2d_pair and every conv2d call is the fp32 CUDA-core conv
-on the fp32 storage weight (at 160x192 that includes MaskFormer's 1/32 encoder: under 64 tokens it stays on the CUDA-core conv)."""
+"""precision="fp32_tc" host orchestration of the three families on the CPU operator references: the split-precision tensor-core products - the engine's
+convs and linears, and the per-query mask product of MaskFormer / BisenetFormer (per-image weights) - are reached only through conv2d_pair, and every
+conv2d call is the fp32 CUDA-core conv on the fp32 storage weight (at 160x192 that includes MaskFormer's 1/32 encoder: under 64 tokens it stays on the
+CUDA-core conv)."""
 import pytest
 import torch
 
@@ -33,4 +34,5 @@ def test_fp32_tc_reaches_split_products_only_through_conv2d_pair(ref_backend, fa
     ops._backend = calls = ConvCalls(ops._backend)
     m(x)
     assert calls.w["conv2d_pair"]
+    assert any(w.dim() == 5 for w in calls.w["conv2d_pair"]) == (family != "fai_detr"), "the mask product runs as conv2d_pair with per-image weights"
     assert all(w.dtype == torch.float32 for w in calls.w["conv2d"]), sorted({str(w.dtype) for w in calls.w["conv2d"]})

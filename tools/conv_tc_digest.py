@@ -100,7 +100,7 @@ ops.conv2d_pair(yp.slice(0, C), _split3_weights(rnd((C, 3, 3, C), s=0.03)), None
                 out=dst.slice(C, 2 * C))
 record("fs_pair_channel_slices", dst.buf)
 
-# split-precision conv through the general conv entry point
+# split-precision conv spelled through ops.conv2d (the dense [hi|lo] tensor, forwarded to conv2d_pair)
 record("fs_conv2d_entry", ops.conv2d(ops.split_pair(rnd((2, 20, 20, 128), s=3.0)), _split3_weights(rnd((128, 3, 3, 128), s=0.03)), *folded_bn(128), pad=1, act=RELU,
                                      out_dtype=F32, algo=ops.ALGO_TCGEN05_SPLIT3))
 
@@ -111,7 +111,7 @@ out = torch.zeros((B, H, W, 104), dtype=F16, device=DEV)
 ops.conv2d_per_image(x.half(), me.half().reshape(B, Q, 1, 1, C), out=out[..., :Q])
 record("f16_per_image_weights", out)
 out = torch.zeros((B, H, W, 104), dtype=F32, device=DEV)
-ops.conv2d_per_image(ops.split_pair(x), _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=out[..., :Q], algo=ops.ALGO_TCGEN05_SPLIT3)
+ops.conv2d_per_image(ops.to_pair(x), _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=out[..., :Q])
 record("fs_per_image_weights", out)
 
 # row-max-only epilogue
