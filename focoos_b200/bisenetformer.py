@@ -22,26 +22,9 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .fai_detr import _bn_fold, _channels, _Conv, _CriterionStub, _packed_layers, _unpair
+from .fai_detr import STDC, ConvX, _bn_fold, _Conv, _CriterionStub, _packed_layers, _unpair
 from .fai_mf import MaskFormerModelOutput, MFEngine, PredictionHeads, _AttnLayer, _ConvBN, _FFNLayer, _SegmentationModel
-from .ports import ModelOutput
-
-
-@dataclass
-class STDCConfig:
-    """nn/backbone/stdc.py:175-186."""
-
-    in_chans: int = 3
-    base: int = 64
-    layers: List[int] = field(default_factory=lambda: [4, 5, 3])
-    out_features: List[str] = field(default_factory=lambda: ["res2", "res3", "res4", "res5"])
-    model_type: str = "stdc"
-    block_num: int = 4
-    block_type: str = "cat"
-    backbone_url: Optional[str] = None
-    size: Optional[str] = None
-    use_conv_last: bool = False
-    use_pretrained: bool = False
+from .ports import ModelOutput, STDCConfig
 
 
 @dataclass
@@ -95,40 +78,6 @@ BisenetFormerOutput = MaskFormerModelOutput  # models/bisenetformer/ports.py: sa
 
 
 # ---- parameter containers -------------------------------------------------------------------------
-class ConvX(nn.Module):  # nn/backbone/stdc.py:20 — also ConvBNReLU (bisenetformer/modelling.py:122)
-    def __init__(self, cin, cout, k=3, stride=1):
-        super().__init__()
-        self.conv = nn.Conv2d(cin, cout, k, stride, padding=k // 2, bias=False)
-        self.bn = nn.BatchNorm2d(cout)
-
-
-class CatBottleneck(nn.Module):  # nn/backbone/stdc.py:109
-    def __init__(self, cin, cout, stride):
-        super().__init__()
-        self.stride = stride
-        if stride == 2:
-            self.avd_layer = nn.Sequential(nn.Conv2d(cout // 2, cout // 2, 3, 2, 1, groups=cout // 2, bias=False), nn.BatchNorm2d(cout // 2))
-        self.conv_list = nn.ModuleList([ConvX(cin, cout // 2, 1), ConvX(cout // 2, cout // 4), ConvX(cout // 4, cout // 8), ConvX(cout // 8, cout // 8)])
-
-
-class STDC(nn.Module):  # nn/backbone/stdc.py:189
-    def __init__(self, cfg: STDCConfig):
-        super().__init__()
-        assert cfg.block_type == "cat" and cfg.block_num == 4, "focoos_b200 implements the CatBottleneck STDC (block_num 4)"
-        base, feats = cfg.base, []
-        feats += [ConvX(cfg.in_chans, base // 2, 3, 2), ConvX(base // 2, base, 3, 2)]
-        for i, n in enumerate(cfg.layers):
-            for j in range(n):
-                if i == 0 and j == 0:
-                    feats.append(CatBottleneck(base, base * 4, 2))
-                elif j == 0:
-                    feats.append(CatBottleneck(base * 2 ** (i + 1), base * 2 ** (i + 2), 2))
-                else:
-                    feats.append(CatBottleneck(base * 2 ** (i + 2), base * 2 ** (i + 2), 1))
-        self.features = nn.Sequential(*feats)
-        self.out_channels = [base, base * 4, base * 8, base * 16]
-
-
 class AttentionRefinementModule(nn.Module):  # bisenetformer/modelling.py:149
     def __init__(self, cin, cout):
         super().__init__()
@@ -189,26 +138,7 @@ class BisenetEngine(MFEngine):
     def _pack(self, sd):
         cfg = self.cfg
         self.nhead, self.d = 8, cfg.transformer_predictor_hidden_dim
-        bb = "pixel_decoder.backbone.features"
-        w = sd[bb + ".0.conv.weight"].float()
-        s, b = _bn_fold(sd, bb + ".0.bn")
-        self.stem_w, self.stem_s, self.stem_b = self._f32(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b)
-        self.stem2 = self._convx(sd, bb + ".1", 2)
-        self.blocks = []
-        idx = 2
-        for n in cfg.backbone_config.layers:
-            stage = []
-            for j in range(n):
-                p = f"{bb}.{idx}"
-                stride = 2 if j == 0 else 1
-                blk = {"stride": stride, "convs": [self._convx(sd, f"{p}.conv_list.{i}", 1) for i in range(4)]}
-                if stride == 2:
-                    wd = sd[p + ".avd_layer.0.weight"].float()  # [C,1,3,3]
-                    sa, ba = _bn_fold(sd, p + ".avd_layer.1")
-                    blk["avd"] = (self._f32(wd.reshape(wd.shape[0], 9).t()), self._f32(sa), self._f32(ba))
-                stage.append(blk)
-                idx += 1
-            self.blocks.append(stage)
+        self._pack_backbone(sd)
         cp, ffm = "pixel_decoder.cp", "pixel_decoder.ffm"
         self.conv_avg = self._convx(sd, cp + ".conv_avg", 1)
         self.arm = {}
@@ -231,49 +161,10 @@ class BisenetEngine(MFEngine):
         """the decoder linears (whether an STDC block runs in the pair format depends on its shapes: _pair_block_ok)"""
         return list(_packed_layers([self.dec, self.mask_mlp]))
 
-    def _convx(self, sd, p, stride):
-        w = sd[p + ".conv.weight"].float()
-        s, b = _bn_fold(sd, p + ".bn")
-        return _Conv(self._to(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b), stride, w.shape[-1] // 2, ops.ACT_RELU)
-
     def _gate(self, conv, vec):
         """tiny [B,C] GEMM(s) of the channel-attention gates, SIMT path (M = batch size)."""
         B, C = vec.shape
         return self._conv(conv, vec.reshape(B, 1, 1, C), algo=ops.ALGO_SIMT).reshape(B, -1)
-
-    def _cat_bottleneck(self, x, blk):
-        """CatBottleneck, concat-free: each conv writes its channel slice of the block's output buffer, which the next conv reads in place.  A block that
-        _pair_block_ok takes keeps the buffer as a Pair (no split pass inside the block); a stride-2 block's first conv reads a Pair input and writes fp32."""
-        c = blk["convs"]
-        half = c[0].w.shape[0]
-        B, H, W, _ = x.shape
-        if blk["stride"] == 2:
-            out1 = self._conv(c[0], x)
-            buf = torch.empty((B, (H - 1) // 2 + 1, (W - 1) // 2 + 1, 2 * half), dtype=self.dt, device=x.device)
-            ops.avgpool3x3s2(out1, out=buf[..., :half])
-            src = ops.dwconv3x3s2(out1, *blk["avd"])
-        else:
-            shape = (B, H, W, 2 * half)
-            buf = ops.Pair.empty(shape, x.device) if self._pair_block_ok(blk, H, W) else torch.empty(shape, dtype=self.dt, device=x.device)
-            src = self._conv(c[0], x, out=_channels(buf, 0, half))
-        o = half
-        for i in (1, 2, 3):
-            w = c[i].w.shape[0]
-            src = self._conv(c[i], src, out=_channels(buf, o, o + w))
-            o += w
-        return buf
-
-    def _pair_block_ok(self, blk, H, W) -> bool:
-        """conv2d_pair takes the block: every conv has its weight triple; a 32-channel 3x3 input needs the halo mode (rows of at least 64 pixels, Cout <= 64)"""
-        if blk["stride"] != 1 or not self.pair:
-            return False
-        for cv in blk["convs"]:
-            cin, cout, k = cv.w.shape[3], cv.w.shape[0], cv.w.shape[1]
-            if cv.w3 is None or cout % 8:
-                return False
-            if cin % 64 and not (cin == 32 and k == 3 and W >= 64 and cout <= 64):
-                return False
-        return True
 
     @torch.no_grad()
     def forward(self, images: torch.Tensor, taps: Optional[dict] = None):
@@ -284,14 +175,7 @@ class BisenetEngine(MFEngine):
             assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
             B, _, H, W = images.shape
         # any H x W, like the reference (its processor does not resize): odd maps from the stride-2 convs and pools run on the same kernels
-        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, self.dt)
-        x = self._conv(self.stem2, x)  # res2
-        feats = []
-        for stage in self.blocks:
-            for blk in stage:
-                x = self._cat_bottleneck(x, blk)
-            feats.append(x)
-        res3, res4, res5 = feats
+        _, res3, res4, res5 = self._run_backbone(images)
         res5 = _unpair(res5)  # global average pool + ARM gates work on fp32 (33 M elements at bs=64 1024x512)
         # context path; the convs that read res4 / res3 take a Pair to fp32 themselves
         avg = self._gate(self.conv_avg, ops.global_avgpool(res5))

@@ -28,7 +28,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .ports import DETRConfig, DETRModelOutput, ResnetConfig
+from .ports import DETRConfig, DETRModelOutput, ResnetConfig, STDCConfig
 
 RESNET_BLOCKS = {50: [3, 4, 6, 3], 101: [3, 4, 23, 3]}
 
@@ -86,6 +86,40 @@ class ResNet(nn.Module):  # nn/backbone/resnet.py:164 (variant d, depth >= 50)
         self.out_channels = [256, 512, 1024, 2048]
 
 
+class ConvX(nn.Module):  # nn/backbone/stdc.py:20 — also ConvBNReLU (bisenetformer/modelling.py:122)
+    def __init__(self, cin, cout, k=3, stride=1):
+        super().__init__()
+        self.conv = nn.Conv2d(cin, cout, k, stride, padding=k // 2, bias=False)
+        self.bn = nn.BatchNorm2d(cout)
+
+
+class CatBottleneck(nn.Module):  # nn/backbone/stdc.py:109
+    def __init__(self, cin, cout, stride):
+        super().__init__()
+        self.stride = stride
+        if stride == 2:
+            self.avd_layer = nn.Sequential(nn.Conv2d(cout // 2, cout // 2, 3, 2, 1, groups=cout // 2, bias=False), nn.BatchNorm2d(cout // 2))
+        self.conv_list = nn.ModuleList([ConvX(cin, cout // 2, 1), ConvX(cout // 2, cout // 4), ConvX(cout // 4, cout // 8), ConvX(cout // 8, cout // 8)])
+
+
+class STDC(nn.Module):  # nn/backbone/stdc.py:189
+    def __init__(self, cfg: STDCConfig):
+        super().__init__()
+        assert cfg.block_type == "cat" and cfg.block_num == 4, "focoos_b200 implements the CatBottleneck STDC (block_num 4)"
+        base, feats = cfg.base, []
+        feats += [ConvX(cfg.in_chans, base // 2, 3, 2), ConvX(base // 2, base, 3, 2)]
+        for i, n in enumerate(cfg.layers):
+            for j in range(n):
+                if i == 0 and j == 0:
+                    feats.append(CatBottleneck(base, base * 4, 2))
+                elif j == 0:
+                    feats.append(CatBottleneck(base * 2 ** (i + 1), base * 2 ** (i + 2), 2))
+                else:
+                    feats.append(CatBottleneck(base * 2 ** (i + 2), base * 2 ** (i + 2), 1))
+        self.features = nn.Sequential(*feats)
+        self.out_channels = [base, base * 4, base * 8, base * 16]
+
+
 class RepVggBlock(nn.Module):  # modelling.py:30
     def __init__(self, ch):
         super().__init__()
@@ -117,7 +151,8 @@ class TransformerEncoder(nn.Module):  # nn/layers/transformer.py:471
 
 
 class Encoder(nn.Module):  # modelling.py:195 ("pixel_decoder")
-    def __init__(self, backbone: ResNet, feat_dim, out_dim, nhead, dff, num_encoder_layers):
+    def __init__(self, backbone, feat_dim, out_dim, nhead, dff, num_encoder_layers):
+        """backbone: ResNet or STDC; the input projections read its res3 / res4 / res5 channels.  num_encoder_layers 0 holds no AIFI parameters."""
         super().__init__()
         self.backbone = backbone
         in_ch = backbone.out_channels[1:]
@@ -361,14 +396,21 @@ class DetrEngine:
         return both, reps
 
     def _pack_backbone(self, sd, bb="pixel_decoder.backbone"):
-        """ResNet-vd (nn/backbone/resnet.py:164): stem + bottleneck stages with folded BN (shared by every model family)."""
+        """the trunk named by cfg.backbone_config.model_type, with folded BN (shared by every model family): ResNet-vd or STDC"""
+        if self.cfg.backbone_config.model_type == "stdc":
+            self._pack_stdc(sd, bb + ".features")
+        else:
+            self._pack_resnet(sd, bb)
+
+    def _pack_resnet(self, sd, bb):
+        """ResNet-vd (nn/backbone/resnet.py:164): stem + bottleneck stages."""
         w = sd[bb + ".conv1.conv1_1.conv.weight"].float()
         s, b = _bn_fold(sd, bb + ".conv1.conv1_1.norm")
         self.stem_w, self.stem_s, self.stem_b = self._f32(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b)
         self.stem2 = self._cnl(sd, bb + ".conv1.conv1_2", "relu")
         self.stem3 = self._cnl(sd, bb + ".conv1.conv1_3", "relu")
         self.stages = []
-        for si, count in enumerate(RESNET_BLOCKS[self.depth]):
+        for si, count in enumerate(RESNET_BLOCKS[self.cfg.backbone_config.depth]):
             blocks = []
             for bi in range(count):
                 p = f"{bb}.res_layers.{si}.blocks.{bi}"
@@ -380,8 +422,41 @@ class DetrEngine:
                 blocks.append(blk)
             self.stages.append(blocks)
 
+    def _pack_stdc(self, sd, bb):
+        """STDC (nn/backbone/stdc.py:189): two stride-2 ConvX stems + CatBottleneck stages; stride-2 blocks keep the depthwise 3x3/s2 + BN weights fp32 [9, C]."""
+        w = sd[bb + ".0.conv.weight"].float()
+        s, b = _bn_fold(sd, bb + ".0.bn")
+        self.stem_w, self.stem_s, self.stem_b = self._f32(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b)
+        self.stem2 = self._convx(sd, bb + ".1", 2)
+        self.blocks = []
+        idx = 2
+        for n in self.cfg.backbone_config.layers:
+            stage = []
+            for j in range(n):
+                p = f"{bb}.{idx}"
+                stride = 2 if j == 0 else 1
+                blk = {"stride": stride, "convs": [self._convx(sd, f"{p}.conv_list.{i}", 1) for i in range(4)]}
+                if stride == 2:
+                    wd = sd[p + ".avd_layer.0.weight"].float()  # [C,1,3,3]
+                    sa, ba = _bn_fold(sd, p + ".avd_layer.1")
+                    blk["avd"] = (self._f32(wd.reshape(wd.shape[0], 9).t()), self._f32(sa), self._f32(ba))
+                stage.append(blk)
+                idx += 1
+            self.blocks.append(stage)
+
+    def _convx(self, sd, p, stride):
+        w = sd[p + ".conv.weight"].float()
+        s, b = _bn_fold(sd, p + ".bn")
+        return _Conv(self._to(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b), stride, w.shape[-1] // 2, ops.ACT_RELU)
+
     def _run_backbone(self, images):
-        """-> [res2, res3, res4, res5] NHWC (nn/backbone/resnet.py:252-266): Pairs under fp32_tc (shared by every model family with this backbone)."""
+        """-> [res2, res3, res4, res5] NHWC of the packed trunk (shared by every model family)"""
+        if self.cfg.backbone_config.model_type == "stdc":
+            return self._run_stdc(images)
+        return self._run_resnet(images)
+
+    def _run_resnet(self, images):
+        """nn/backbone/resnet.py:252-266: Pairs under fp32_tc"""
         cfg = self.cfg
         x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, self.dt, out_pair=self.pair)
         x = self._conv(self.stem3, self._conv(self.stem2, x, out_pair=True), out_pair=True)
@@ -394,6 +469,52 @@ class DetrEngine:
                 x = self._conv(blk["c"], y, residual=short, out_pair=True)
             feats.append(x)
         return feats
+
+    def _run_stdc(self, images):
+        """nn/backbone/stdc.py:314: res2 fp32 under fp32_tc; res3-5 are Pairs where the stage's last block runs in the pair format (_pair_block_ok)"""
+        cfg = self.cfg
+        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, self.dt)
+        x = self._conv(self.stem2, x)  # res2
+        feats = [x]
+        for stage in self.blocks:
+            for blk in stage:
+                x = self._cat_bottleneck(x, blk)
+            feats.append(x)
+        return feats
+
+    def _cat_bottleneck(self, x, blk):
+        """CatBottleneck, concat-free: each conv writes its channel slice of the block's output buffer, which the next conv reads in place.  A block that
+        _pair_block_ok takes keeps the buffer as a Pair (no split pass inside the block); a stride-2 block's first conv reads a Pair input and writes fp32."""
+        c = blk["convs"]
+        half = c[0].w.shape[0]
+        B, H, W, _ = x.shape
+        if blk["stride"] == 2:
+            out1 = self._conv(c[0], x)
+            buf = torch.empty((B, (H - 1) // 2 + 1, (W - 1) // 2 + 1, 2 * half), dtype=self.dt, device=x.device)
+            ops.avgpool3x3s2(out1, out=buf[..., :half])
+            src = ops.dwconv3x3s2(out1, *blk["avd"])
+        else:
+            shape = (B, H, W, 2 * half)
+            buf = ops.Pair.empty(shape, x.device) if self._pair_block_ok(blk, H, W) else torch.empty(shape, dtype=self.dt, device=x.device)
+            src = self._conv(c[0], x, out=_channels(buf, 0, half))
+        o = half
+        for i in (1, 2, 3):
+            w = c[i].w.shape[0]
+            src = self._conv(c[i], src, out=_channels(buf, o, o + w))
+            o += w
+        return buf
+
+    def _pair_block_ok(self, blk, H, W) -> bool:
+        """conv2d_pair takes the block: every conv has its weight triple; a 32-channel 3x3 input needs the halo mode (rows of at least 64 pixels, Cout <= 64)"""
+        if blk["stride"] != 1 or not self.pair:
+            return False
+        for cv in blk["convs"]:
+            cin, cout, k = cv.w.shape[3], cv.w.shape[0], cv.w.shape[1]
+            if cv.w3 is None or cout % 8:
+                return False
+            if cin % 64 and not (cin == 32 and k == 3 and W >= 64 and cout <= 64):
+                return False
+        return True
 
     # ---- the layer call: the one place that picks a conv / linear kernel from the precision and the operand's format ---------------------------------
     def _on_pairs(self, layer, x, algo, out_pair):
@@ -433,12 +554,12 @@ class DetrEngine:
 
     def _pack(self, sd):
         cfg = self.cfg
-        self.depth, self.nhead, self.d = cfg.backbone_config.depth, cfg.transformer_predictor_nhead, cfg.transformer_predictor_hidden_dim
+        self.nhead, self.d = cfg.transformer_predictor_nhead, cfg.transformer_predictor_hidden_dim
         self._pack_backbone(sd)
         pd = "pixel_decoder"
         self.enc_in = [self._seq_conv_bn(sd, f"{pd}.input_proj.{i}.0", f"{pd}.input_proj.{i}.1") for i in range(3)]
-        e = f"{pd}.encoder.0.layers.0"
-        self.aifi = self._pack_attn_block(sd, e, ffn_norms=("norm1", "norm2"))
+        # the AIFI layer on the 1/32 map (fai-detr-l-*); fai-detr-m-coco has none (pixel_decoder_num_encoder_layers 0)
+        self.aifi = self._pack_attn_block(sd, f"{pd}.encoder.0.layers.0", ffn_norms=("norm1", "norm2")) if cfg.pixel_decoder_num_encoder_layers else None
         self.lateral = [self._cnl(sd, f"{pd}.lateral_convs.{i}", "silu") for i in range(2)]
         self.fpn = [self._csp(sd, f"{pd}.fpn_blocks.{i}") for i in range(2)]
         self.down = [self._cnl(sd, f"{pd}.downsample_convs.{i}", "silu") for i in range(2)]
@@ -484,10 +605,9 @@ class DetrEngine:
         if key not in self._consts:
             shapes = [(h32, w32), (h32 * 2, w32 * 2), (h32 * 4, w32 * 4)]
             anchors, valid = generate_anchors(shapes)
-            self._consts[key] = {
-                "shapes": shapes, "anchors": self._f32(anchors), "valid": valid.to(self.device, torch.uint8).contiguous(),
-                "pos": self._to(aifi_position_embedding(h32, w32, self.cfg.pixel_decoder_feat_dim // 2)),
-            }
+            self._consts[key] = {"shapes": shapes, "anchors": self._f32(anchors), "valid": valid.to(self.device, torch.uint8).contiguous()}
+            if self.aifi is not None:
+                self._consts[key]["pos"] = self._to(aifi_position_embedding(h32, w32, self.cfg.pixel_decoder_feat_dim // 2))
         return self._consts[key]
 
     # ---- forward -------------------------------------------------------------------------------
@@ -546,14 +666,19 @@ class DetrEngine:
         cat4 = self._empty((B, h32, w32, 2 * C), dev)          # [down(pan0) | lat0]
         self._conv(self.enc_in[0], res3, out=_channels(cat2, C, 2 * C))
         self._conv(self.enc_in[1], res4, out=_channels(cat1, C, 2 * C))
-        src = self._conv(self.enc_in[2], res5).reshape(B, h32 * w32, C)  # tokens for the AIFI block: fp32 in the pair flow (LayerNorm / attention work on fp32)
-        # AIFI (modelling.py:315-324)
-        if self.pair:
-            src, src_p = self._aifi_pair(src, K["pos"])
+        if self.aifi is None:  # no encoder layer (modelling.py:315): the projected res5 feeds lateral_convs.0, as a Pair in the pair flow
+            lat_in = self._conv(self.enc_in[2], res5, out_pair=True)
         else:
-            src = self._ffn(self.aifi, self._mha(self.aifi, src, K["pos"]), ops.ACT_GELU)
-        p5 = src.reshape(B, h32, w32, C)
-        lat_in = ops.Pair(src_p.buf.reshape(B, h32, w32, 2 * C)) if self.pair else p5  # the pair flow's conv reads the pair its LayerNorm wrote
+            src = self._conv(self.enc_in[2], res5).reshape(B, h32 * w32, C)  # tokens for the AIFI block: fp32 in the pair flow (LayerNorm / attention work on fp32)
+            # AIFI (modelling.py:315-324)
+            if self.pair:
+                src, src_p = self._aifi_pair(src, K["pos"])
+            else:
+                src = self._ffn(self.aifi, self._mha(self.aifi, src, K["pos"]), ops.ACT_GELU)
+            p5 = src.reshape(B, h32, w32, C)
+            lat_in = ops.Pair(src_p.buf.reshape(B, h32, w32, 2 * C)) if self.pair else p5  # the pair flow's conv reads the pair its LayerNorm wrote
+            if taps is not None:
+                taps["aifi"] = p5
         # top-down FPN (modelling.py:328-336)
         lat0 = self._conv(self.lateral[0], lat_in, out=_channels(cat4, C, 2 * C))
         ops.resize_bilinear(lat0, (h32 * 2, w32 * 2), out=_channels(cat1, 0, C))
@@ -568,8 +693,7 @@ class DetrEngine:
         pan1 = self._csp_run(self.pan[1], cat4)
         enc_outs = [pan1, pan0, fpn1]  # outs[::-1] (modelling.py:347): 1/32, 1/16, 1/8
         if taps is not None:
-            taps.update(res3=_unpair(res3), res4=_unpair(res4), res5=_unpair(res5), aifi=p5, fpn0=_unpair(fpn0), fpn1=_unpair(fpn1), pan0=_unpair(pan0),
-                        pan1=_unpair(pan1))
+            taps.update(res3=_unpair(res3), res4=_unpair(res4), res5=_unpair(res5), fpn0=_unpair(fpn0), fpn1=_unpair(fpn1), pan0=_unpair(pan0), pan1=_unpair(pan1))
         # predictor: memory [B, S, d] (modelling.py:1145-1167), each level written in place
         shapes = K["shapes"]
         memory = self._empty((B, sum(h * w for h, w in shapes), self.d), dev)
@@ -746,7 +870,8 @@ class FAIDetr(_EngineModel):
     def __init__(self, config: DETRConfig, precision: str = "fp16"):
         super().__init__(config, precision)
         c = config
-        self.pixel_decoder = Encoder(ResNet(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_nhead,
+        backbone = STDC(c.backbone_config) if c.backbone_config.model_type == "stdc" else ResNet(c.backbone_config)
+        self.pixel_decoder = Encoder(backbone, c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_nhead,
                                      c.pixel_decoder_dim_feedforward, c.pixel_decoder_num_encoder_layers)
         self.head = DETRHead(TransformerPredictor(c.pixel_decoder_out_dim, c.num_classes, c.transformer_predictor_hidden_dim, c.num_queries,
                                                   c.transformer_predictor_nhead, c.transformer_predictor_dec_layers,
@@ -766,8 +891,16 @@ class FAIDetr(_EngineModel):
         self._engine = None  # packed (BN-folded, re-parameterised) weights are rebuilt from the parameters at the next eval forward
         return super().train(mode)
 
+    def check_trainable(self):
+        """fine-tuning runs on the ResNet trunk only: the backward kernels of the STDC trunk (depthwise 3x3/s2, 3x3/s2 average pool, the concat-free
+        CatBottleneck) are not built, so an STDC-trunk detector (fai-detr-m-coco) serves inference only"""
+        if self.config.backbone_config.model_type != "resnet":
+            raise NotImplementedError(f"focoos_b200 fine-tunes fai-detr on the ResNet trunk only: the {self.config.backbone_config.model_type!r} trunk's "
+                                      "backward kernels are not built (inference runs)")
+
     def train_graph(self):
         """training-mode forward built from the autograd ops (fai_detr_train.py); fp32 storage, tensor-core split products by default"""
+        self.check_trainable()
         from .fai_detr_train import DetrTrainGraph
         # train_precision: "amp" = one tensor-core product on fp16-rounded operands, fp32 accumulation / storage (the reference's torch.autocast(fp16) arithmetic,
         # trainer/trainer.py:735; the trainer sets it from TrainerArgs.amp_enabled); None = follow the inference precision (fp32-accurate products / CUDA-core fp32)

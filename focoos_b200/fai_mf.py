@@ -216,7 +216,7 @@ class MFEngine(DetrEngine):
 
     def _pack(self, sd):
         cfg = self.cfg
-        self.depth, self.nhead, self.d = cfg.backbone_config.depth, 8, cfg.transformer_predictor_hidden_dim
+        self.nhead, self.d = 8, cfg.transformer_predictor_hidden_dim
         self._pack_backbone(sd)
         pd = "pixel_decoder"
         self.pd_in = self._conv_bias(sd, pd + ".input_proj", 0)

@@ -29,6 +29,14 @@ _REGISTRY: Dict[str, dict] = {
                                                      "resolution": 640, "threshold": 0.5}},
     "fai-detr-l-coco": {"im_size": 640, "config": {"num_classes": 80, "backbone_config": {"model_type": "resnet", "depth": 50, "variant": "d"}, "num_queries": 300,
                                                    "resolution": 640, "threshold": 0.5}},
+    "fai-detr-m-coco": {"im_size": 640, "config": {"num_classes": 80, "backbone_config": {"model_type": "stdc", "in_chans": 3, "base": 64, "layers": [4, 5, 3],
+                                                                            "out_features": ["res2", "res3", "res4", "res5"], "block_num": 4,
+                                                                            "block_type": "cat", "use_conv_last": False},
+                                                   "num_queries": 300, "resolution": 640, "pixel_decoder_out_dim": 128, "pixel_decoder_feat_dim": 128,
+                                                   "pixel_decoder_num_encoder_layers": 0, "pixel_decoder_expansion": 1.0, "pixel_decoder_dim_feedforward": 1024,
+                                                   "transformer_predictor_out_dim": 128, "transformer_predictor_hidden_dim": 256,
+                                                   "transformer_predictor_dec_layers": 3, "transformer_predictor_dim_feedforward": 1024, "head_out_dim": 128,
+                                                   "pixel_decoder_nhead": 8, "transformer_predictor_nhead": 8, "threshold": 0.5}},
     "fai-mf-l-coco-ins": {"family": "fai_mf", "im_size": 1024, "config": {"num_classes": 80, "backbone_config": {"model_type": "resnet", "depth": 101, "variant": "d"},
                                                                            "num_queries": 100, "postprocessing_type": "instance", "predict_all_pixels": False,
                                                                            "use_mask_score": True, "threshold": 0.5}},

@@ -3,7 +3,7 @@
 from __future__ import annotations
 
 from dataclasses import dataclass, field, fields
-from typing import List, Optional
+from typing import List, Optional, Union
 
 import torch
 
@@ -108,10 +108,30 @@ class ResnetConfig:
 
 
 @dataclass
+class STDCConfig:
+    """nn/backbone/stdc.py:175-186."""
+
+    in_chans: int = 3
+    base: int = 64
+    layers: List[int] = field(default_factory=lambda: [4, 5, 3])
+    out_features: List[str] = field(default_factory=lambda: ["res2", "res3", "res4", "res5"])
+    model_type: str = "stdc"
+    block_num: int = 4
+    block_type: str = "cat"
+    backbone_url: Optional[str] = None
+    size: Optional[str] = None
+    use_conv_last: bool = False
+    use_pretrained: bool = False
+
+
+_BACKBONE_CONFIGS = {"resnet": ResnetConfig, "stdc": STDCConfig}
+
+
+@dataclass
 class DETRConfig:
     """models/fai_detr/config.py:9-61 (same field names and defaults)."""
 
-    backbone_config: ResnetConfig = field(default_factory=ResnetConfig)
+    backbone_config: Union[ResnetConfig, STDCConfig] = field(default_factory=ResnetConfig)
     num_classes: int = 365
     num_queries: int = 300
     resolution: Optional[int] = 640
@@ -150,12 +170,21 @@ class DETRConfig:
     matcher_alpha: float = 0.25
     matcher_gamma: float = 2.0
 
+    def __post_init__(self):
+        # the registry ships hybrid encoders with one AIFI layer (fai-detr-l-*) or none (fai-detr-m-coco); the engine runs exactly these two
+        if self.pixel_decoder_num_encoder_layers not in (0, 1):
+            raise ValueError(f"pixel_decoder_num_encoder_layers must be 0 or 1 (got {self.pixel_decoder_num_encoder_layers})")
+
     @classmethod
     def from_dict(cls, d: dict) -> "DETRConfig":
         d = dict(d)
         bc = d.pop("backbone_config", {}) or {}
         if isinstance(bc, dict):
-            bc = ResnetConfig(**{k: v for k, v in bc.items() if k in {f.name for f in fields(ResnetConfig)}})
+            kind = bc.get("model_type", "resnet")
+            if kind not in _BACKBONE_CONFIGS:
+                raise ValueError(f"Invalid backbone model_type for DETRConfig: {kind!r} (expected one of {sorted(_BACKBONE_CONFIGS)})")
+            bcls = _BACKBONE_CONFIGS[kind]
+            bc = bcls(**{k: v for k, v in bc.items() if k in {f.name for f in fields(bcls)}})
         known = {f.name for f in fields(cls)}
         unknown = set(d) - known
         if unknown:

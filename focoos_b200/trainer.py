@@ -164,6 +164,7 @@ def run_train_entry(fm, args: TrainerArgs, data_train, data_val=None):
     assert args.num_gpus, "Training without GPUs is not supported. num_gpus must be greater than 0"  # focoos_model.py:249
     if type(fm.model).__name__ != "FAIDetr":
         raise NotImplementedError("focoos_b200 fine-tunes the fai-detr family (the segmentation families run inference only)")
+    fm.model.check_trainable()
     out_dir = os.path.join(args.output_dir, args.run_name)
     if args.num_gpus > 1:
         import torch.multiprocessing as mp
