@@ -1,4 +1,4 @@
-// LayerNorm(+residual) and small-sequence multi-head attention (L = 300/400, head_dim = 32).
+// LayerNorm(+residual) and small-sequence multi-head attention (head_dim 32, and head_dim 16 for the 128-wide MaskFormer pixel-decoder encoder).
 #include "common.cuh"
 
 namespace fb200 {
@@ -127,6 +127,11 @@ inline size_t attention_mma_smem(int Lk) { return ((size_t)2 * ((Lk + 63) & ~63)
 // attention_mma_split_kernel with NW warps (16 queries each) per CTA: L <= 640 for self-attention, Lk <= 704 for Lq <= 32
 inline size_t attention_split_smem(int Lk, int NW) { return ((size_t)4 * ((Lk + 63) & ~63) + 2 * 16 * NW) * AM_PITCH * sizeof(__half); }
 int attention_split_warps(int Lq);
+// head_dim 16 (defined below): CUDA-core, fp16 tensor-core and split-precision tensor-core paths, each with a resident and a streaming kernel
+int attention_hd16_simt(const void* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, void* out, int out_pitch, int dtype, int B, int Lq, int Lk,
+                        int heads, float scale, cudaStream_t st);
+int attention_hd16_mma(bool split, const void* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, void* out, int out_pitch, int B, int Lq, int Lk,
+                       int heads, float scale, cudaStream_t st);
 }  // namespace fb200
 using namespace fb200;
 
@@ -146,16 +151,22 @@ extern "C" int fb200_attention(const void* q, int q_pitch, const void* k, int k_
                                int out_pitch, int dtype, int B, int Lq, int Lk, int heads, int head_dim, float scale,
                                void* stream) {
   FB_CHECK_ARG(q && k && v && out, "attention: null pointer");
-  FB_CHECK_ARG(head_dim == 32, "attention: head_dim must be 32 (got %d)", head_dim);
+  FB_CHECK_ARG(head_dim == 32 || head_dim == 16, "attention: head_dim must be 16 or 32 (got %d)", head_dim);
   FB_CHECK_ARG(B > 0 && Lq > 0 && Lk > 0 && heads > 0, "attention: B, Lq, Lk and heads must be positive (got %d, %d, %d, %d)", B, Lq, Lk, heads);
   FB_CHECK_ARG(q_pitch % 4 == 0 && k_pitch % 4 == 0 && v_pitch % 4 == 0, "attention: pitches must be multiples of 4");
-  const int w = heads * 32;  // a pitch below the row width would make neighbouring rows overlap
-  FB_CHECK_ARG(q_pitch >= w, "attention: q_pitch (%d) < heads*32 (%d)", q_pitch, w);
-  FB_CHECK_ARG(k_pitch >= w, "attention: k_pitch (%d) < heads*32 (%d)", k_pitch, w);
-  FB_CHECK_ARG(v_pitch >= w, "attention: v_pitch (%d) < heads*32 (%d)", v_pitch, w);
-  FB_CHECK_ARG(out_pitch >= w, "attention: out_pitch (%d) < heads*32 (%d)", out_pitch, w);
-  if (dtype == FB200_F16 && q_pitch % 8 == 0 && k_pitch % 8 == 0 && v_pitch % 8 == 0 && out_pitch % 2 == 0 &&
-      (((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0 && ((uintptr_t)out & 3) == 0) {
+  const int w = heads * head_dim;  // a pitch below the row width would make neighbouring rows overlap
+  FB_CHECK_ARG(q_pitch >= w, "attention: q_pitch (%d) < heads*%d (%d)", q_pitch, head_dim, w);
+  FB_CHECK_ARG(k_pitch >= w, "attention: k_pitch (%d) < heads*%d (%d)", k_pitch, head_dim, w);
+  FB_CHECK_ARG(v_pitch >= w, "attention: v_pitch (%d) < heads*%d (%d)", v_pitch, head_dim, w);
+  FB_CHECK_ARG(out_pitch >= w, "attention: out_pitch (%d) < heads*%d (%d)", out_pitch, head_dim, w);
+  const bool mma_ok = dtype == FB200_F16 && q_pitch % 8 == 0 && k_pitch % 8 == 0 && v_pitch % 8 == 0 && out_pitch % 2 == 0 &&
+                      (((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0 && ((uintptr_t)out & 3) == 0;
+  if (head_dim == 16) {
+    FB_CHECK_ARG(dtype == FB200_F32 || dtype == FB200_F16, "attention: bad dtype");
+    if (mma_ok) return attention_hd16_mma(false, q, q_pitch, k, k_pitch, v, v_pitch, out, out_pitch, B, Lq, Lk, heads, scale, (cudaStream_t)stream);
+    return attention_hd16_simt(q, q_pitch, k, k_pitch, v, v_pitch, out, out_pitch, dtype, B, Lq, Lk, heads, scale, (cudaStream_t)stream);
+  }
+  if (mma_ok) {
     if (attention_mma_smem(Lk) <= kAttnSmemMax)
       return attention_mma((const __half*)q, q_pitch, (const __half*)k, k_pitch, (const __half*)v, v_pitch, (__half*)out, out_pitch, B, Lq, Lk, heads, scale,
                            (cudaStream_t)stream);
@@ -208,16 +219,20 @@ extern "C" int fb200_attention_masked_split(const float* q, int q_pitch, const v
 extern "C" int fb200_attention_split(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, void* out, int out_dtype, int out_pitch, int B,
                                      int Lq, int Lk, int heads, int head_dim, float scale, void* stream) {
   FB_CHECK_ARG(q && k && v && out, "attention_split: null pointer");
-  FB_CHECK_ARG(head_dim == 32, "attention_split: head_dim must be 32 (got %d)", head_dim);
+  FB_CHECK_ARG(head_dim == 32 || head_dim == 16, "attention_split: head_dim must be 16 or 32 (got %d)", head_dim);
   FB_CHECK_ARG(B > 0 && Lq > 0 && Lk > 0 && heads > 0, "attention_split: B, Lq, Lk and heads must be positive (got %d, %d, %d, %d)", B, Lq, Lk, heads);
   FB_CHECK_ARG(q_pitch % 4 == 0 && k_pitch % 4 == 0 && v_pitch % 4 == 0 && out_pitch % 2 == 0 && (((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0 &&
                    ((uintptr_t)out & 7) == 0, "attention_split: pitches / alignment");
   FB_CHECK_ARG(out_dtype == FB200_F32 || out_dtype == FB200_F16PAIR, "attention_split: out_dtype must be F32 or F16PAIR");
-  const int w = heads * 32;  // a pitch below the row width would make neighbouring rows overlap
-  FB_CHECK_ARG(q_pitch >= w, "attention_split: q_pitch (%d) < heads*32 (%d)", q_pitch, w);
-  FB_CHECK_ARG(k_pitch >= w, "attention_split: k_pitch (%d) < heads*32 (%d)", k_pitch, w);
-  FB_CHECK_ARG(v_pitch >= w, "attention_split: v_pitch (%d) < heads*32 (%d)", v_pitch, w);
-  FB_CHECK_ARG(out_pitch >= w, "attention_split: out_pitch (%d) < heads*32 (%d)", out_pitch, w);
+  const int w = heads * head_dim;  // a pitch below the row width would make neighbouring rows overlap
+  FB_CHECK_ARG(q_pitch >= w, "attention_split: q_pitch (%d) < heads*%d (%d)", q_pitch, head_dim, w);
+  FB_CHECK_ARG(k_pitch >= w, "attention_split: k_pitch (%d) < heads*%d (%d)", k_pitch, head_dim, w);
+  FB_CHECK_ARG(v_pitch >= w, "attention_split: v_pitch (%d) < heads*%d (%d)", v_pitch, head_dim, w);
+  FB_CHECK_ARG(out_pitch >= w, "attention_split: out_pitch (%d) < heads*%d (%d)", out_pitch, head_dim, w);
+  if (head_dim == 16) {
+    FB_CHECK_ARG(out_dtype == FB200_F32, "attention_split: head_dim 16 writes fp32 rows only (out_dtype F32)");
+    return attention_hd16_mma(true, q, q_pitch, k, k_pitch, v, v_pitch, out, out_pitch, B, Lq, Lk, heads, scale, (cudaStream_t)stream);
+  }
   FB_CHECK_ARG(out_dtype != FB200_F16PAIR || out_pitch >= 2 * heads * 32, "attention_split: pair rows are [hi(heads*32) | lo(heads*32)]");
   // fp32 rows above the resident kernel's shared memory: the masked streaming kernel without a mask (keys staged 256 at a time); pair rows are refused there
   if (out_dtype == FB200_F32 && attention_split_smem(Lk, attention_split_warps(Lq)) > kAttnSmemMax)
@@ -885,6 +900,320 @@ int attention_mma_stream(const __half* q, int q_pitch, const __half* k, int k_pi
   attention_mma_stream_kernel<<<grid, 128, 0, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, mask, LkP, allowed, out, out_pitch, Lq, Lk, heads,
                                                     scale * 1.4426950408889634f);
   FB_CHECK_LAUNCH("attention_mma_stream");
+  return FB200_OK;
+}
+
+}  // namespace fb200
+
+// ------------------------------------------------------------------------------------------------
+// head_dim 16: the encoder of the 128-wide MaskFormer pixel decoders (fai-mf-m / -s: 8 heads x 16 channels, unmasked self-attention over
+// ceil(H/32) * ceil(W/32) tokens per image).  Three arithmetics, each with a kernel that keeps the whole K / V of a (batch, head) in shared memory
+// (STREAM = false) and one that stages them CHUNK keys at a time with the online softmax carried across chunks (STREAM = true), taken above the
+// resident kernel's shared-memory ceiling.  Both variants run the same code; the resident one has a single chunk.
+// ------------------------------------------------------------------------------------------------
+namespace fb200 {
+
+// CUDA-core kernel (fp32 rows, and fp16 rows the tensor-core kernel cannot read): a warp runs two queries at once, one per half-warp, lane & 15 = channel;
+// 8 warps x 4 query pairs = 64 queries per CTA.  grid (B*heads, ceil(Lq/64)), block 256.
+// smem (floats): Ks[CH][17] + Vs[CH][16] + P[16][CH+1] (one row per half-warp) + Qs[64][16]
+constexpr int ATT16_QT = 64, ATT16_PAIRS = 4, ATT16_CHUNK = 256;
+inline size_t attention_hd16_simt_smem(int keys) { return ((size_t)keys * 17 + (size_t)keys * 16 + (size_t)16 * (keys + 1) + ATT16_QT * 16) * sizeof(float); }  // resident: Lk <= 1164
+
+__device__ __forceinline__ float half_warp_max(float v) {
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__device__ __forceinline__ float half_warp_sum(float v) {
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+template <typename T, bool STREAM>
+__global__ void __launch_bounds__(256) attention_hd16_kernel(const T* __restrict__ q, int q_pitch, const T* __restrict__ k, int k_pitch, const T* __restrict__ v,
+                                                             int v_pitch, T* __restrict__ out, int out_pitch, int Lq, int Lk, int heads, float scale) {
+  extern __shared__ float sm[];
+  const int CH = STREAM ? ATT16_CHUNK : Lk;  // keys staged at a time
+  float* Ks = sm;                           // [CH][17]
+  float* Vs = Ks + (size_t)CH * 17;         // [CH][16]
+  float* Ps = Vs + (size_t)CH * 16;         // [16][CH + 1]
+  float* Qs = Ps + (size_t)16 * (CH + 1);   // [64][16]
+  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, hq = lane >> 4, c = lane & 15;
+  const int q0 = blockIdx.y * ATT16_QT;
+  for (int i = threadIdx.x; i < ATT16_QT * 4; i += blockDim.x) {  // the CTA's queries, scaled (torch scales q before QK^T); rows past Lq are zero
+    const int r = i >> 2, cc = (i & 3) * 4;
+    float qv[4] = {0.f, 0.f, 0.f, 0.f};
+    if (q0 + r < Lq) load4(q + ((int64_t)b * Lq + q0 + r) * q_pitch + h * 16 + cc, qv);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) Qs[r * 16 + cc + j] = qv[j] * scale;
+  }
+  float* P = Ps + (size_t)(warp * 2 + hq) * (CH + 1);
+  float o[ATT16_PAIRS], m[ATT16_PAIRS], l[ATT16_PAIRS];
+#pragma unroll
+  for (int p = 0; p < ATT16_PAIRS; ++p) { o[p] = 0.f; m[p] = -INFINITY; l[p] = 0.f; }
+  for (int c0 = 0; c0 < Lk; c0 += CH) {
+    const int n = min(CH, Lk - c0);
+    __syncthreads();  // the previous chunk has been consumed by every warp
+    for (int i = threadIdx.x; i < n * 4; i += blockDim.x) {
+      const int r = i >> 2, cc = (i & 3) * 4;
+      float kv[4], vv[4];
+      load4(k + ((int64_t)b * Lk + c0 + r) * k_pitch + h * 16 + cc, kv);
+      load4(v + ((int64_t)b * Lk + c0 + r) * v_pitch + h * 16 + cc, vv);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { Ks[r * 17 + cc + j] = kv[j]; Vs[r * 16 + cc + j] = vv[j]; }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int p = 0; p < ATT16_PAIRS; ++p) {
+      const float* Q = Qs + ((warp * ATT16_PAIRS + p) * 2 + hq) * 16;
+      float mx = -INFINITY;
+      for (int j = c; j < n; j += 16) {
+        float s = 0.f;
+#pragma unroll
+        for (int d = 0; d < 16; ++d) s = fmaf(Q[d], Ks[j * 17 + d], s);
+        P[j] = s;
+        mx = fmaxf(mx, s);
+      }
+      const float nm = fmaxf(m[p], half_warp_max(mx));  // finite: every chunk holds at least one key
+      const float a = expf(m[p] - nm);                  // 0 on the first chunk
+      float sum = 0.f;
+      for (int j = c; j < n; j += 16) {
+        const float e = expf(P[j] - nm);
+        P[j] = e;
+        sum += e;
+      }
+      l[p] = l[p] * a + half_warp_sum(sum);
+      m[p] = nm;
+      __syncwarp();
+      float acc = 0.f;
+      for (int j = 0; j < n; ++j) acc = fmaf(P[j], Vs[j * 16 + c], acc);
+      o[p] = o[p] * a + acc;
+      __syncwarp();
+    }
+  }
+#pragma unroll
+  for (int p = 0; p < ATT16_PAIRS; ++p) {
+    const int qi = q0 + (warp * ATT16_PAIRS + p) * 2 + hq;
+    if (qi < Lq) out[((int64_t)b * Lq + qi) * out_pitch + h * 16 + c] = from_f<T>(o[p] / l[p]);
+  }
+}
+
+int attention_hd16_simt(const void* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, void* out, int out_pitch, int dtype, int B, int Lq, int Lk,
+                        int heads, float scale, cudaStream_t st) {
+  const bool stream = attention_hd16_simt_smem(Lk) > kAttnSmemMax;
+  const size_t smem = attention_hd16_simt_smem(stream ? ATT16_CHUNK : Lk);
+  static bool configured = false;
+  if (!configured) {  // raise the dynamic-smem ceiling once (not inside a stream capture)
+    cudaFuncSetAttribute(attention_hd16_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(attention_hd16_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(attention_hd16_kernel<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);   // 53 KiB chunks
+    cudaFuncSetAttribute(attention_hd16_kernel<__half, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    configured = true;
+  }
+  dim3 grid(B * heads, (unsigned)cdiv(Lq, ATT16_QT));
+  if (stream) {
+    FB_DISPATCH_DTYPE(dtype, T, (attention_hd16_kernel<T, true><<<grid, 256, smem, st>>>((const T*)q, q_pitch, (const T*)k, k_pitch, (const T*)v, v_pitch, (T*)out, out_pitch,
+                                                                                         Lq, Lk, heads, scale)));
+  } else {
+    FB_DISPATCH_DTYPE(dtype, T, (attention_hd16_kernel<T, false><<<grid, 256, smem, st>>>((const T*)q, q_pitch, (const T*)k, k_pitch, (const T*)v, v_pitch, (T*)out, out_pitch,
+                                                                                          Lq, Lk, heads, scale)));
+  }
+  FB_CHECK_LAUNCH("attention_hd16");
+  return FB200_OK;
+}
+
+// Tensor-core kernels (mma.sync.m16n8k16, 16 queries per warp): QK^T is a single k-step per 8-key tile, PV two n8 tiles.  SPLIT = false: fp16 rows in and out
+// (the "fp16" mode).  SPLIT = true: fp32 rows in and out (the "fp32_tc" mode), Q, K, V split into fp16 [hi | lo] planes while staged, three products per
+// term (hi*hi + hi*lo + lo*hi) and the softmax in fp32, as attention_mma_split_kernel does for 32-channel heads.
+// smem (halves): K / V planes [CH][AM16_PITCH] (2 fp16, 4 split) + Q planes [16*NW][AM16_PITCH] (1 fp16, 2 split); CH = keys rounded up to 64 (resident) or 256
+constexpr int AM16_PITCH = 24;  // halves per smem row (16 + 8 pad): the 8 rows of an ldmatrix land in distinct banks
+constexpr int AM16_CHUNK = 256;
+inline size_t attention_hd16_mma_smem(bool split, int keys, int NW) {  // resident: Lk <= 2368 (fp16, 4 warps); self-attention L <= 1088 (split, NW from attention_split_warps)
+  return ((size_t)(split ? 4 : 2) * ((keys + 63) & ~63) + (size_t)(split ? 2 : 1) * 16 * NW) * AM16_PITCH * sizeof(__half);
+}
+
+template <bool SPLIT, bool STREAM>
+__global__ void __launch_bounds__(384) attention_hd16_mma_kernel(const void* __restrict__ q_, int q_pitch, const void* __restrict__ k_, int k_pitch,
+                                                                 const void* __restrict__ v_, int v_pitch, void* __restrict__ out_, int out_pitch, int Lq, int Lk,
+                                                                 int heads, float scale_log2) {
+  extern __shared__ __align__(16) __half smh[];
+  const int CH = STREAM ? AM16_CHUNK : ((Lk + 63) & ~63);  // keys staged at a time
+  const size_t kv = (size_t)CH * AM16_PITCH;
+  __half* Kh = smh; __half* Vh = Kh + kv;
+  __half* Kl = Vh + kv; __half* Vl = Kl + kv;  // split only
+  const int QB = (int)(blockDim.x >> 5) * 16;   // queries per CTA
+  __half* Qh = smh + (SPLIT ? 4 : 2) * kv; __half* Ql = Qh + QB * AM16_PITCH;
+  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+  const int q0 = blockIdx.y * QB;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if constexpr (SPLIT) {
+    const float* q = reinterpret_cast<const float*>(q_);
+    for (int i = tid; i < QB * 4; i += (int)blockDim.x) {  // 4 x float4 per 16-wide row
+      const int r = i >> 2, c = (i & 3) * 4;
+      float4 qq = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (q0 + r < Lq) qq = *reinterpret_cast<const float4*>(q + ((int64_t)b * Lq + q0 + r) * q_pitch + h * 16 + c);
+      split_store4(Qh + r * AM16_PITCH + c, Ql + r * AM16_PITCH + c, qq);
+    }
+  } else {
+    const __half* q = reinterpret_cast<const __half*>(q_);
+    for (int i = tid; i < QB * 2; i += (int)blockDim.x) {  // 2 x 16 bytes per row
+      const int r = i >> 1, c = (i & 1) * 8;
+      uint4 qv = make_uint4(0, 0, 0, 0);
+      if (q0 + r < Lq) qv = *reinterpret_cast<const uint4*>(q + ((int64_t)b * Lq + q0 + r) * q_pitch + h * 16 + c);
+      *reinterpret_cast<uint4*>(Qh + r * AM16_PITCH + c) = qv;
+    }
+  }
+  __syncthreads();
+  uint32_t qah[4], qal[4];  // A fragments of this warp's 16 queries (one k-step: d 0-15)
+  {
+    const int r = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+    const int c = (lane >> 4) * 8;
+    ldsm_x4(qah, Qh + r * AM16_PITCH + c);
+    if constexpr (SPLIT) ldsm_x4(qal, Ql + r * AM16_PITCH + c);
+  }
+  float o[2][4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) o[i][j] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;  // rows lane/4 and lane/4+8
+  for (int c0 = 0; c0 < Lk; c0 += CH) {
+    const int rows = min(CH, (Lk - c0 + 63) & ~63);  // staged rows: whole 64-key blocks, zero past Lk
+    __syncthreads();  // the previous chunk has been consumed by every warp
+    if constexpr (SPLIT) {
+      const float* k = reinterpret_cast<const float*>(k_);
+      const float* v = reinterpret_cast<const float*>(v_);
+      for (int i = tid; i < rows * 4; i += (int)blockDim.x) {
+        const int r = i >> 2, c = (i & 3) * 4;
+        float4 kk = make_float4(0.f, 0.f, 0.f, 0.f), vv = kk;
+        if (c0 + r < Lk) {
+          kk = *reinterpret_cast<const float4*>(k + ((int64_t)b * Lk + c0 + r) * k_pitch + h * 16 + c);
+          vv = *reinterpret_cast<const float4*>(v + ((int64_t)b * Lk + c0 + r) * v_pitch + h * 16 + c);
+        }
+        split_store4(Kh + r * AM16_PITCH + c, Kl + r * AM16_PITCH + c, kk);
+        split_store4(Vh + r * AM16_PITCH + c, Vl + r * AM16_PITCH + c, vv);
+      }
+    } else {
+      const __half* k = reinterpret_cast<const __half*>(k_);
+      const __half* v = reinterpret_cast<const __half*>(v_);
+      for (int i = tid; i < rows * 2; i += (int)blockDim.x) {
+        const int r = i >> 1, c = (i & 1) * 8;
+        uint4 kk = make_uint4(0, 0, 0, 0), vv = kk;
+        if (c0 + r < Lk) {
+          kk = *reinterpret_cast<const uint4*>(k + ((int64_t)b * Lk + c0 + r) * k_pitch + h * 16 + c);
+          vv = *reinterpret_cast<const uint4*>(v + ((int64_t)b * Lk + c0 + r) * v_pitch + h * 16 + c);
+        }
+        *reinterpret_cast<uint4*>(Kh + r * AM16_PITCH + c) = kk;
+        *reinterpret_cast<uint4*>(Vh + r * AM16_PITCH + c) = vv;
+      }
+    }
+    __syncthreads();
+    for (int kb = 0; kb < rows; kb += 64) {
+      float s[8][4];
+#pragma unroll
+      for (int nt = 0; nt < 8; nt += 2) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { s[nt][j] = 0.f; s[nt + 1][j] = 0.f; }
+        // one x4 ldmatrix = the B fragments of two 8-key tiles: (keys nt*8.., d 0-7 | d 8-15), (keys nt*8+8.., d 0-7 | d 8-15)
+        const int off = (kb + nt * 8 + (lane & 7) + (lane >> 4) * 8) * AM16_PITCH + ((lane >> 3) & 1) * 8;
+        uint32_t kh[4];
+        ldsm_x4(kh, Kh + off);
+        if constexpr (SPLIT) {
+          uint32_t kl[4];
+          ldsm_x4(kl, Kl + off);
+          mma16816(s[nt], qal, kh[0], kh[1]); mma16816(s[nt + 1], qal, kh[2], kh[3]);  // small terms first
+          mma16816(s[nt], qah, kl[0], kl[1]); mma16816(s[nt + 1], qah, kl[2], kl[3]);
+        }
+        mma16816(s[nt], qah, kh[0], kh[1]); mma16816(s[nt + 1], qah, kh[2], kh[3]);
+      }
+      float bm0 = -INFINITY, bm1 = -INFINITY;
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const int key = c0 + kb + nt * 8 + (lane & 3) * 2;
+        if (key >= Lk) { s[nt][0] = -INFINITY; s[nt][2] = -INFINITY; }
+        if (key + 1 >= Lk) { s[nt][1] = -INFINITY; s[nt][3] = -INFINITY; }
+        bm0 = fmaxf(bm0, fmaxf(s[nt][0], s[nt][1]));
+        bm1 = fmaxf(bm1, fmaxf(s[nt][2], s[nt][3]));
+      }
+      bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1)); bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
+      bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1)); bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+      const float nm0 = fmaxf(m0, bm0), nm1 = fmaxf(m1, bm1);  // finite: every 64-key block holds at least one real key
+      const float a0 = exp2f((m0 - nm0) * scale_log2), a1 = exp2f((m1 - nm1) * scale_log2);
+      m0 = nm0; m1 = nm1;
+      l0 *= a0; l1 *= a1;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) { o[i][0] *= a0; o[i][1] *= a0; o[i][2] *= a1; o[i][3] *= a1; }
+      uint32_t pah[4][4], pal[4][4];  // P as A fragments: 4 k-steps of 16 keys
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const float p0 = exp2f((s[nt][0] - m0) * scale_log2), p1 = exp2f((s[nt][1] - m0) * scale_log2);
+        const float p2 = exp2f((s[nt][2] - m1) * scale_log2), p3 = exp2f((s[nt][3] - m1) * scale_log2);
+        l0 += p0 + p1; l1 += p2 + p3;
+        const __half2 h01 = __floats2half2_rn(p0, p1), h23 = __floats2half2_rn(p2, p3);
+        pah[nt >> 1][(nt & 1) * 2 + 0] = *reinterpret_cast<const uint32_t*>(&h01);
+        pah[nt >> 1][(nt & 1) * 2 + 1] = *reinterpret_cast<const uint32_t*>(&h23);
+        if constexpr (SPLIT) {
+          const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
+          pal[nt >> 1][(nt & 1) * 2 + 0] = pack_h2(p0 - f01.x, p1 - f01.y);
+          pal[nt >> 1][(nt & 1) * 2 + 1] = pack_h2(p2 - f23.x, p3 - f23.y);
+        }
+      }
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {  // 16 keys per step; one x4.trans ldmatrix = (d 0-7, d 8-15) x (keys 0-7, 8-15)
+        const int off = (kb + ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * AM16_PITCH + (lane >> 4) * 8;
+        uint32_t vh[4];
+        ldsm_x4_trans(vh, Vh + off);
+        if constexpr (SPLIT) {
+          uint32_t vl[4];
+          ldsm_x4_trans(vl, Vl + off);
+          mma16816(o[0], pal[ks], vh[0], vh[1]); mma16816(o[1], pal[ks], vh[2], vh[3]);
+          mma16816(o[0], pah[ks], vl[0], vl[1]); mma16816(o[1], pah[ks], vl[2], vl[3]);
+        }
+        mma16816(o[0], pah[ks], vh[0], vh[1]); mma16816(o[1], pah[ks], vh[2], vh[3]);
+      }
+    }
+  }
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float i0 = 1.f / l0, i1 = 1.f / l1;
+  const int r0 = q0 + warp * 16 + (lane >> 2), r1 = r0 + 8;
+#pragma unroll
+  for (int nt = 0; nt < 2; ++nt) {
+    const int c = h * 16 + nt * 8 + (lane & 3) * 2;
+    if constexpr (SPLIT) {
+      float* out = reinterpret_cast<float*>(out_);
+      if (r0 < Lq) *reinterpret_cast<float2*>(out + ((int64_t)b * Lq + r0) * out_pitch + c) = make_float2(o[nt][0] * i0, o[nt][1] * i0);
+      if (r1 < Lq) *reinterpret_cast<float2*>(out + ((int64_t)b * Lq + r1) * out_pitch + c) = make_float2(o[nt][2] * i1, o[nt][3] * i1);
+    } else {
+      __half* out = reinterpret_cast<__half*>(out_);
+      if (r0 < Lq) *reinterpret_cast<uint32_t*>(out + ((int64_t)b * Lq + r0) * out_pitch + c) = pack_h2(o[nt][0] * i0, o[nt][1] * i0);
+      if (r1 < Lq) *reinterpret_cast<uint32_t*>(out + ((int64_t)b * Lq + r1) * out_pitch + c) = pack_h2(o[nt][2] * i1, o[nt][3] * i1);
+    }
+  }
+}
+
+int attention_hd16_mma(bool split, const void* q, int q_pitch, const void* k, int k_pitch, const void* v, int v_pitch, void* out, int out_pitch, int B, int Lq, int Lk,
+                       int heads, float scale, cudaStream_t st) {
+  const int NW = split ? attention_split_warps(Lq) : 4;  // 16 queries per warp
+  const bool stream = attention_hd16_mma_smem(split, Lk, NW) > kAttnSmemMax;
+  const size_t smem = attention_hd16_mma_smem(split, stream ? AM16_CHUNK : Lk, NW);
+  static bool configured = false;
+  if (!configured) {
+    cudaFuncSetAttribute(attention_hd16_mma_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(attention_hd16_mma_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(attention_hd16_mma_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(attention_hd16_mma_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);   // up to 66 KiB
+    configured = true;
+  }
+  dim3 grid(B * heads, (unsigned)cdiv(Lq, 16 * NW));
+  const float sl2 = scale * 1.4426950408889634f;
+  if (split && stream) attention_hd16_mma_kernel<true, true><<<grid, 32 * NW, smem, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, out, out_pitch, Lq, Lk, heads, sl2);
+  else if (split) attention_hd16_mma_kernel<true, false><<<grid, 32 * NW, smem, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, out, out_pitch, Lq, Lk, heads, sl2);
+  else if (stream) attention_hd16_mma_kernel<false, true><<<grid, 32 * NW, smem, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, out, out_pitch, Lq, Lk, heads, sl2);
+  else attention_hd16_mma_kernel<false, false><<<grid, 32 * NW, smem, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, out, out_pitch, Lq, Lk, heads, sl2);
+  FB_CHECK_LAUNCH("attention_hd16_mma");
   return FB200_OK;
 }
 

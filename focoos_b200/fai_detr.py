@@ -588,9 +588,9 @@ class DetrEngine:
             self.dec.append(blk)
         self.dec_score = self._lin(sd, f"{hp}.dec_score_classifier.{L - 1}")
 
-    def _pack_attn_block(self, sd, p, ffn_norms):
-        """MultiheadAttention (packed in_proj: rows [0,d)=Q, [d,2d)=K, [2d,3d)=V) + FFN + the two LayerNorms around them."""
-        d = self.d
+    def _pack_attn_block(self, sd, p, ffn_norms, d=None):
+        """MultiheadAttention (packed in_proj: rows [0,d)=Q, [d,2d)=K, [2d,3d)=V) + FFN + the two LayerNorms around them; d defaults to self.d."""
+        d = self.d if d is None else d
         w, b = sd[p + ".self_attn.in_proj_weight"].float(), sd[p + ".self_attn.in_proj_bias"].float()
         n_attn, n_ffn = ffn_norms
         return {

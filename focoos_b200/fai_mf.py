@@ -216,11 +216,14 @@ class MFEngine(DetrEngine):
 
     def _pack(self, sd):
         cfg = self.cfg
-        self.nhead, self.d = 8, cfg.transformer_predictor_hidden_dim
+        self.nhead, self.d = 8, cfg.transformer_predictor_hidden_dim  # masked decoder
+        # the pixel-decoder encoder has its own width and heads: 256 x 8 heads of 32 channels (fai-mf-l), 128 x 8 heads of 16 channels (fai-mf-m / -s)
+        self.pd_d, self.pd_nhead = cfg.pixel_decoder_feat_dim, cfg.pixel_decoder_transformer_nheads
         self._pack_backbone(sd)
         pd = "pixel_decoder"
         self.pd_in = self._conv_bias(sd, pd + ".input_proj", 0)
-        self.enc = [self._pack_attn_block(sd, f"{pd}.transformer.encoder.layers.{i}", ffn_norms=("norm1", "norm2")) for i in range(cfg.pixel_decoder_transformer_layers)]
+        self.enc = [self._pack_attn_block(sd, f"{pd}.transformer.encoder.layers.{i}", ffn_norms=("norm1", "norm2"), d=self.pd_d)
+                    for i in range(cfg.pixel_decoder_transformer_layers)]
         self.enc_norm = (self._f32(sd[pd + ".transformer.encoder.norm.weight"]), self._f32(sd[pd + ".transformer.encoder.norm.bias"]))
         self.layer = {i: self._conv_bn(sd, f"{pd}.layer_{i}", 1, ops.ACT_RELU) for i in (1, 2, 3, 4)}
         self.adapter = {i: self._conv_bn(sd, f"{pd}.adapter_{i}", 0, ops.ACT_NONE) for i in (1, 2, 3)}
@@ -263,10 +266,12 @@ class MFEngine(DetrEngine):
         s, b = _bn_fold(sd, p + ".norm")
         return _Conv(self._to(sd[p + ".weight"].float().permute(0, 2, 3, 1)), self._f32(s), self._f32(b), 1, pad, act)
 
-    def _pos(self, h, w):
-        key = ("pos", h, w)
+    def _pos(self, h, w, d=None):
+        """the normalised sine embedding of an h x w map for a d-wide sequence (default: the decoder width self.d)"""
+        d = self.d if d is None else d
+        key = ("pos", h, w, d)
         if key not in self._consts:
-            self._consts[key] = self._to(position_embedding_sine_normalized(h, w, self.d // 2))
+            self._consts[key] = self._to(position_embedding_sine_normalized(h, w, d // 2))
         return self._consts[key]
 
     def _heads(self, out, mask_features, size, want_class):
@@ -308,12 +313,12 @@ class MFEngine(DetrEngine):
         # fp32_tc: the backbone keeps its activations as fp16 [hi | lo] planes between convs (no split pass in front of every conv); the four pixel-decoder
         # convs that consume res2..res5 read the pairs and write the fp32 tensors the transformer / FPN arithmetic below works on
         res2, res3, res4, res5 = self._run_backbone(images)
-        d, nh = self.d, self.nhead
+        d, nh = self.pd_d, self.pd_nhead
         scale = 1.0 / math.sqrt(d // nh)
         # ---- pixel decoder (TransformerFPN.forward_features)
         x = self._conv(self.pd_in, res5)
         h, w = x.shape[1], x.shape[2]
-        pos = self._pos(h, w)
+        pos = self._pos(h, w, d)
         src = x.reshape(B, h * w, d)
         for blk in self.enc:  # pre-norm encoder layer (nn/layers/transformer.py:583-601 with normalize_before)
             s2 = ops.layernorm(src, *blk["n_attn"])

@@ -40,6 +40,14 @@ _REGISTRY: Dict[str, dict] = {
     "fai-mf-l-coco-ins": {"family": "fai_mf", "im_size": 1024, "config": {"num_classes": 80, "backbone_config": {"model_type": "resnet", "depth": 101, "variant": "d"},
                                                                            "num_queries": 100, "postprocessing_type": "instance", "predict_all_pixels": False,
                                                                            "use_mask_score": True, "threshold": 0.5}},
+    **{name: {"family": "fai_mf", "im_size": 1024, "config": {"num_classes": 80, "backbone_config": {"model_type": "resnet", "depth": depth, "variant": "d"},
+                                                             "num_queries": 100, "resolution": 1024, "pixel_decoder_out_dim": 128, "pixel_decoder_feat_dim": 128,
+                                                             "pixel_decoder_transformer_layers": 3, "pixel_decoder_transformer_nheads": 8,
+                                                             "pixel_decoder_transformer_dim_feedforward": 1024, "transformer_predictor_out_dim": 128,
+                                                             "transformer_predictor_hidden_dim": 256, "transformer_predictor_dec_layers": 6,
+                                                             "transformer_predictor_dim_feedforward": 1024, "head_out_dim": 128, "postprocessing_type": "instance",
+                                                             "predict_all_pixels": False, "use_mask_score": True, "threshold": 0.5}}
+       for name, depth in (("fai-mf-m-coco-ins", 101), ("fai-mf-s-coco-ins", 50))},
     "bisenetformer-l-ade": {"family": "bisenetformer", "im_size": 640, "config": {"num_classes": 150, "backbone_config": {"model_type": "stdc", "base": 64, "layers": [4, 5, 3]},
                                                                                    "num_queries": 100, "postprocessing_type": "semantic", "predict_all_pixels": True,
                                                                                    "use_mask_score": False, "threshold": 0.5}},

@@ -230,6 +230,13 @@ class MaskFormerProcessor(DETRProcessor):
         self.mask_threshold, self.use_mask_score, self.predict_all_pixels = config.mask_threshold, config.use_mask_score, config.predict_all_pixels
         self.training = False
 
+    def export_postprocess(self, output, inputs, class_names=(), top_k=None, threshold: float = 0.5):
+        """fai_mf/processor.py:308-337: output = (masks, logits) of an exported graph."""
+        from .fai_mf import MaskFormerModelOutput
+
+        masks, logits = (torch.from_numpy(t) if isinstance(t, np.ndarray) else t for t in output[:2])
+        return self.postprocess(MaskFormerModelOutput(masks=masks, logits=logits, loss=None), inputs, class_names, top_k, threshold)
+
     def postprocess_tensors(self, output, threshold=None, use_mask_score=None, predict_all_pixels=None):
         """-> list over images of (query idx [n], scores [n], labels [n]) on the host, plus the device masks tensor."""
         threshold = threshold or self.threshold
