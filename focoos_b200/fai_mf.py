@@ -20,21 +20,21 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field, fields
-from typing import List, Optional
+from typing import List, Optional, Union
 
 import torch
 import torch.nn as nn
 
 from . import ops
-from .fai_detr import _split3_weights, MLP, DetrEngine, ResNet, _bn_fold, _Conv, _CriterionStub, _EngineModel, _Linear, _packed_layers
-from .ports import ModelOutput, ResnetConfig
+from .fai_detr import _split3_weights, MLP, STDC, DetrEngine, ResNet, _bn_fold, _Conv, _CriterionStub, _EngineModel, _Linear, _packed_layers
+from .ports import ModelOutput, ResnetConfig, STDCConfig, backbone_config_from_dict
 
 
 @dataclass
 class MaskFormerConfig:
     """models/fai_mf/config.py (same field names / defaults as the registry JSONs use)."""
 
-    backbone_config: ResnetConfig = field(default_factory=lambda: ResnetConfig(depth=101))
+    backbone_config: Union[ResnetConfig, STDCConfig] = field(default_factory=lambda: ResnetConfig(depth=101))
     num_classes: int = 80
     num_queries: int = 100
     resolution: Optional[int] = 1024
@@ -72,9 +72,7 @@ class MaskFormerConfig:
     @classmethod
     def from_dict(cls, d: dict) -> "MaskFormerConfig":
         d = dict(d)
-        bc = d.pop("backbone_config", {}) or {}
-        if isinstance(bc, dict):
-            bc = ResnetConfig(**{k: v for k, v in bc.items() if k in {f.name for f in fields(ResnetConfig)}})
+        bc = backbone_config_from_dict(d.pop("backbone_config", {}), "MaskFormerConfig")
         unknown = set(d) - {f.name for f in fields(cls)}
         if unknown:
             raise ValueError(f"Invalid parameters for MaskFormerConfig: {sorted(unknown)}")
@@ -142,16 +140,18 @@ class _EncoderOnly(nn.Module):  # fai_mf/modelling.py:130
 
 
 class TransformerFPN(nn.Module):  # fai_mf/modelling.py:201
-    def __init__(self, backbone: ResNet, feat_dim, out_dim, layers, nhead, dff):
+    def __init__(self, backbone: Union[ResNet, STDC], feat_dim, out_dim, layers, nhead, dff):
         super().__init__()
         self.backbone = backbone
         ch = backbone.out_channels  # res2..res5
-        self.input_proj = _ConvBN(ch[3], feat_dim, 1, bias=True, norm=False)
-        self.transformer = _EncoderOnly(feat_dim, nhead, dff, layers)
+        if layers > 0:
+            self.input_proj = _ConvBN(ch[3], feat_dim, 1, bias=True, norm=False)
+            self.transformer = _EncoderOnly(feat_dim, nhead, dff, layers)
         for idx in (1, 2, 3):
             self.add_module(f"adapter_{idx}", _ConvBN(ch[idx - 1], feat_dim, 1))
             self.add_module(f"layer_{idx}", _ConvBN(feat_dim, feat_dim, 3))
-        self.layer_4 = _ConvBN(feat_dim, feat_dim, 3)
+        # without an encoder (fai-mf-*-ade: :241-284) layer_4 reads res5 itself
+        self.layer_4 = _ConvBN(feat_dim if layers > 0 else ch[3], feat_dim, 3)
         self.mask_features = _ConvBN(feat_dim, out_dim, 3, bias=True, norm=False)
 
 
@@ -221,18 +221,28 @@ class MFEngine(DetrEngine):
         self.pd_d, self.pd_nhead = cfg.pixel_decoder_feat_dim, cfg.pixel_decoder_transformer_nheads
         self._pack_backbone(sd)
         pd = "pixel_decoder"
-        self.pd_in = self._conv_bias(sd, pd + ".input_proj", 0)
+        # no encoder (fai-mf-*-ade): no input_proj, no encoder layers, no final LayerNorm - layer_4 reads res5
+        self.pd_in = self.enc_norm = None
         self.enc = [self._pack_attn_block(sd, f"{pd}.transformer.encoder.layers.{i}", ffn_norms=("norm1", "norm2"), d=self.pd_d)
                     for i in range(cfg.pixel_decoder_transformer_layers)]
-        self.enc_norm = (self._f32(sd[pd + ".transformer.encoder.norm.weight"]), self._f32(sd[pd + ".transformer.encoder.norm.bias"]))
+        if self.enc:
+            self.pd_in = self._conv_bias(sd, pd + ".input_proj", 0)
+            self.enc_norm = (self._f32(sd[pd + ".transformer.encoder.norm.weight"]), self._f32(sd[pd + ".transformer.encoder.norm.bias"]))
         self.layer = {i: self._conv_bn(sd, f"{pd}.layer_{i}", 1, ops.ACT_RELU) for i in (1, 2, 3, 4)}
         self.adapter = {i: self._conv_bn(sd, f"{pd}.adapter_{i}", 0, ops.ACT_NONE) for i in (1, 2, 3)}
         self.mask_features = self._conv_bias(sd, pd + ".mask_features", 1)
         self._pack_decoder(sd, 3)
 
     def _pair_layers(self):
-        """the backbone, the pixel-decoder convs that read its pairs, the 1/4-resolution chain into mask_features, and the decoder linears"""
-        return list(_packed_layers([self.stem2, self.stem3, self.stages, self.pd_in, self.adapter, self.layer[1], self.mask_features, self.dec, self.mask_mlp]))
+        """the backbone, the pixel-decoder convs that read its pairs, the 1/4-resolution chain into mask_features, and the decoder linears.
+        ResNet trunk: its stems and bottleneck stages; STDC trunk: its second stem and the CatBottleneck convs (whether a block runs on pairs is
+        _pair_block_ok's call).  res5 is read by input_proj, or without an encoder by layer_4 itself."""
+        if self.cfg.backbone_config.model_type == "stdc":
+            trunk = [self.stem2, [blk["convs"] for stage in self.blocks for blk in stage]]
+        else:
+            trunk = [self.stem2, self.stem3, self.stages]
+        res5_reader = self.pd_in if self.enc else self.layer[4]
+        return list(_packed_layers([trunk, res5_reader, self.adapter, self.layer[1], self.mask_features, self.dec, self.mask_mlp]))
 
     def _pack_decoder(self, sd, num_levels):
         """head.predictor.* of the masked transformer decoder (same key names in fai_mf and bisenetformer)."""
@@ -316,19 +326,22 @@ class MFEngine(DetrEngine):
         d, nh = self.pd_d, self.pd_nhead
         scale = 1.0 / math.sqrt(d // nh)
         # ---- pixel decoder (TransformerFPN.forward_features)
-        x = self._conv(self.pd_in, res5)
-        h, w = x.shape[1], x.shape[2]
-        pos = self._pos(h, w, d)
-        src = x.reshape(B, h * w, d)
-        for blk in self.enc:  # pre-norm encoder layer (nn/layers/transformer.py:583-601 with normalize_before)
-            s2 = ops.layernorm(src, *blk["n_attn"])
-            qk = self._linear(blk["qk"], ops.add(s2, pos))
-            a = ops.attention(qk[..., :d], qk[..., d:], self._linear(blk["v"], s2), nh, scale, split=self.pair)
-            src = self._linear(blk["out"], a, residual=src)
-            s2 = ops.layernorm(src, *blk["n_ffn"])
-            src = self._linear(blk["l2"], self._linear(blk["l1"], s2, act=ops.ACT_RELU), residual=src)
-        src = ops.layernorm(src, *self.enc_norm)
-        y = self._conv(self.layer[4], src.reshape(B, h, w, d))
+        if self.enc:
+            x = self._conv(self.pd_in, res5)
+            h, w = x.shape[1], x.shape[2]
+            pos = self._pos(h, w, d)
+            src = x.reshape(B, h * w, d)
+            for blk in self.enc:  # pre-norm encoder layer (nn/layers/transformer.py:583-601 with normalize_before)
+                s2 = ops.layernorm(src, *blk["n_attn"])
+                qk = self._linear(blk["qk"], ops.add(s2, pos))
+                a = ops.attention(qk[..., :d], qk[..., d:], self._linear(blk["v"], s2), nh, scale, split=self.pair)
+                src = self._linear(blk["out"], a, residual=src)
+                s2 = ops.layernorm(src, *blk["n_ffn"])
+                src = self._linear(blk["l2"], self._linear(blk["l1"], s2, act=ops.ACT_RELU), residual=src)
+            src = ops.layernorm(src, *self.enc_norm)
+            y = self._conv(self.layer[4], src.reshape(B, h, w, d))
+        else:  # no encoder: the 3x3 output conv reads res5 (a Pair under fp32_tc)
+            y = self._conv(self.layer[4], res5)
         ms = [y]
         # fp32_tc: the 1/4-resolution layer feeds only the mask_features conv, whose output is only ever read as a tensor-core operand (the per-image mask product):
         # both stay in the pair format - no fp32 copy of the two largest activations of the pixel decoder, no split pass over them
@@ -339,7 +352,9 @@ class MFEngine(DetrEngine):
                 ms.append(y)
         mask_features = self._conv(self.mask_features, y, out_pair=True)
         if taps is not None:
-            taps.update(res5=res5.float(), enc_memory=src.reshape(B, h, w, d), mask_features=mask_features.float(), multi_scale=ms)
+            taps.update(res5=res5.float(), mask_features=mask_features.float(), multi_scale=ms)
+            if self.enc:
+                taps["enc_memory"] = src.reshape(B, h, w, d)
         return self._run_decoder(ms, mask_features, B, H, W, taps)
 
     def _run_decoder(self, ms, mask_features, B, H, W, taps=None):
@@ -350,7 +365,8 @@ class MFEngine(DetrEngine):
         scale = 1.0 / math.sqrt(d // nh)
         nl = len(ms)
         if self.pair:  # every _heads call reads mask_features as a Pair: MaskFormer's conv writes one, BisenetFormer's fp32 output is split once here
-            assert mask_features.shape[-1] % 64 == 0, mask_features.shape
+            # the tensor-core product takes channel counts in 32-channel chunks (bisenetformer-m-ade: 96 = 3 chunks per plane)
+            assert mask_features.shape[-1] % 32 == 0, mask_features.shape
             mask_features = ops.to_pair(mask_features)
         srcs, kpos, sizes = [], [], []
         for i in range(nl):
@@ -431,7 +447,8 @@ class FAIMaskFormer(_SegmentationModel):
         c = config
         if c.postprocessing_type not in ("semantic", "instance"):
             raise ValueError(f"Invalid postprocessing type: {c.postprocessing_type}. Must be one of: ['semantic', 'instance']")
-        self.pixel_decoder = TransformerFPN(ResNet(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_transformer_layers,
+        backbone = STDC(c.backbone_config) if c.backbone_config.model_type == "stdc" else ResNet(c.backbone_config)
+        self.pixel_decoder = TransformerFPN(backbone, c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_transformer_layers,
                                             c.pixel_decoder_transformer_nheads, c.pixel_decoder_transformer_dim_feedforward)
         self.head = MaskFormerHead(MultiScaleMaskedTransformerDecoder(c.pixel_decoder_out_dim, c.transformer_predictor_out_dim, c.num_classes,
                                                                       c.transformer_predictor_hidden_dim, c.num_queries, 8,

@@ -51,6 +51,28 @@ _REGISTRY: Dict[str, dict] = {
     "bisenetformer-l-ade": {"family": "bisenetformer", "im_size": 640, "config": {"num_classes": 150, "backbone_config": {"model_type": "stdc", "base": 64, "layers": [4, 5, 3]},
                                                                                    "num_queries": 100, "postprocessing_type": "semantic", "predict_all_pixels": True,
                                                                                    "use_mask_score": False, "threshold": 0.5}},
+    # ADE20K semantic MaskFormers: no pixel-decoder encoder (layer_4 reads res5), ResNet-101-vd (-l) or STDC-2 (-m) trunk
+    **{name: {"family": "fai_mf", "im_size": 640, "config": {"num_classes": 150, "backbone_config": bc, "num_queries": 100, "resolution": 640,
+                                                            "pixel_decoder_out_dim": 128, "pixel_decoder_feat_dim": 128, "pixel_decoder_transformer_layers": 0,
+                                                            "pixel_decoder_transformer_nheads": 8, "pixel_decoder_transformer_dim_feedforward": 1024,
+                                                            "transformer_predictor_out_dim": 128, "transformer_predictor_hidden_dim": 256,
+                                                            "transformer_predictor_dec_layers": dec_layers, "transformer_predictor_dim_feedforward": dff,
+                                                            "head_out_dim": 128, "postprocessing_type": "semantic", "mask_threshold": 0.5, "predict_all_pixels": True,
+                                                            "use_mask_score": False, "threshold": 0.5, "top_k": 100}}
+       for name, bc, dec_layers, dff in (
+           ("fai-mf-l-ade", {"model_type": "resnet", "depth": 101, "variant": "d"}, 6, 1024),
+           ("fai-mf-m-ade", {"model_type": "stdc", "in_chans": 3, "base": 64, "layers": [4, 5, 3], "out_features": ["res2", "res3", "res4", "res5"],
+                             "block_num": 4, "block_type": "cat", "use_conv_last": False}, 3, 512))},
+    # ADE20K BisenetFormers: -m has a 96-wide pixel decoder and 4 decoder layers, -s the STDC-1 trunk (layers [2, 2, 2])
+    **{name: {"family": "bisenetformer", "im_size": 640, "config": {"num_classes": 150, "backbone_config": {"model_type": "stdc", "in_chans": 3, "base": 64, "layers": layers,
+                                                                                                           "out_features": ["res2", "res3", "res4", "res5"], "block_num": 4,
+                                                                                                           "block_type": "cat", "use_conv_last": False},
+                                                                   "num_queries": 100, "pixel_decoder_out_dim": width, "pixel_decoder_feat_dim": width,
+                                                                   "transformer_predictor_out_dim": width, "transformer_predictor_hidden_dim": 256,
+                                                                   "transformer_predictor_dec_layers": dec_layers, "transformer_predictor_dim_feedforward": dff,
+                                                                   "head_out_dim": width, "postprocessing_type": "semantic", "top_k": 100, "mask_threshold": 0.5,
+                                                                   "predict_all_pixels": True, "use_mask_score": False, "threshold": 0.5}}
+       for name, layers, width, dec_layers, dff in (("bisenetformer-m-ade", [4, 5, 3], 96, 4, 512), ("bisenetformer-s-ade", [2, 2, 2], 128, 6, 1024))},
 }
 
 # model family -> (config class, nn.Module class, processor class, resize inputs to im_size?) — ModelManager.register_model / ProcessorManager

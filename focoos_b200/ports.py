@@ -127,6 +127,19 @@ class STDCConfig:
 _BACKBONE_CONFIGS = {"resnet": ResnetConfig, "stdc": STDCConfig}
 
 
+def backbone_config_from_dict(bc, owner: str):
+    """the trunk dataclass named by a registry `backbone_config` dict's model_type ("resnet" when absent); a dataclass passes through.
+    `owner` names the model config in the error raised for an unknown model_type."""
+    bc = bc or {}
+    if not isinstance(bc, dict):
+        return bc
+    kind = bc.get("model_type", "resnet")
+    if kind not in _BACKBONE_CONFIGS:
+        raise ValueError(f"Invalid backbone model_type for {owner}: {kind!r} (expected one of {sorted(_BACKBONE_CONFIGS)})")
+    bcls = _BACKBONE_CONFIGS[kind]
+    return bcls(**{k: v for k, v in bc.items() if k in {f.name for f in fields(bcls)}})
+
+
 @dataclass
 class DETRConfig:
     """models/fai_detr/config.py:9-61 (same field names and defaults)."""
@@ -178,13 +191,7 @@ class DETRConfig:
     @classmethod
     def from_dict(cls, d: dict) -> "DETRConfig":
         d = dict(d)
-        bc = d.pop("backbone_config", {}) or {}
-        if isinstance(bc, dict):
-            kind = bc.get("model_type", "resnet")
-            if kind not in _BACKBONE_CONFIGS:
-                raise ValueError(f"Invalid backbone model_type for DETRConfig: {kind!r} (expected one of {sorted(_BACKBONE_CONFIGS)})")
-            bcls = _BACKBONE_CONFIGS[kind]
-            bc = bcls(**{k: v for k, v in bc.items() if k in {f.name for f in fields(bcls)}})
+        bc = backbone_config_from_dict(d.pop("backbone_config", {}), "DETRConfig")
         known = {f.name for f in fields(cls)}
         unknown = set(d) - known
         if unknown:

@@ -1,20 +1,26 @@
 """Config 4 of BASELINE.json: bisenetformer-l-ade, bs=64, 1024x512 on one GPU (forward + GPU part of the semantic post-process).
-    python tools/bench_bisenet.py [batch] [H] [W]"""
-import json, os, sys, collections
+    python tools/bench_bisenet.py [batch] [H] [W]
+FB200_BENCH_MODEL picks another bisenetformer registry entry (default bisenetformer-l-ade; bisenetformer-m-ade, bisenetformer-s-ade), FB200_BENCH_PRECISION
+the precision (default fp16, which also runs fp32_tc in a second process).  FB200_BENCH_LATENCY=N adds the p50 / p90 of N single-image FocoosModel calls
+(uint8 image at 640x640, CUDA graph replay, post-processing included).  The JSON line carries the card, its power limit, and the median SM clock and the
+throttle reasons sampled with nvidia-smi during the timed window."""
+import json, os, sys, collections, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
-from focoos_b200 import ops
-from focoos_b200.bisenetformer import BisenetFormer, BisenetFormerConfig
+from focoos_b200 import ModelManager, ops
 from focoos_b200.utils.seeded_weights import seeded_state_dict
+from tools.smi import SmiSampler
 
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 64
 H = int(sys.argv[2]) if len(sys.argv) > 2 else 512
 W = int(sys.argv[3]) if len(sys.argv) > 3 else 1024
-with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "bisenetformer_l_ade_state_dict_manifest.json")) as f:
+NAME = os.environ.get("FB200_BENCH_MODEL", "bisenetformer-l-ade")
+with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", NAME.replace("-", "_") + "_state_dict_manifest.json")) as f:
     man = json.load(f)
 sd = seeded_state_dict({k: torch.empty(v[0], dtype=getattr(torch, v[1])) for k, v in man.items()}, 0)
 PREC = os.environ.get("FB200_BENCH_PRECISION", "fp16")
-m = BisenetFormer(BisenetFormerConfig(), precision=PREC); m.load_state_dict(sd, strict=True); m.cuda()
+fm = ModelManager.get(NAME, state_dict=sd, precision=PREC)
+m = fm.model; m.cuda()
 x = torch.randint(0, 256, (B, H, W, 3), dtype=torch.uint8, device="cuda")
 def step_unfused():  # the reference's split: model.forward returns [B,Q,H,W] probabilities, the processor reads them back
     out = m(x)
@@ -33,19 +39,33 @@ def timed(fn, n=5):
     e1.record(); torch.cuda.synchronize()
     return e0.elapsed_time(e1) / n
 ms_unfused = timed(step_unfused)
-ms = timed(step)
+with SmiSampler() as smi:
+    ms = timed(step)
+extra = {"gpu": smi.summary()}
+LAT = int(os.environ.get("FB200_BENCH_LATENCY", "0"))
+if LAT:  # bs=1 through the public path: preprocess, graph replay, post-processing to host detections
+    img = torch.randint(0, 256, (640, 640, 3), dtype=torch.uint8).numpy()
+    for _ in range(5): fm.infer(img, threshold=0.5)
+    lat = []
+    with SmiSampler() as smi1:
+        for _ in range(LAT):
+            torch.cuda.synchronize(); t0 = time.perf_counter()
+            fm.infer(img, threshold=0.5)
+            torch.cuda.synchronize(); lat.append((time.perf_counter() - t0) * 1e3)
+    lat.sort()
+    extra["bs1_latency_ms"] = {"p50": lat[len(lat) // 2], "p90": lat[int(len(lat) * 0.9)], "n": LAT, "size": 640, "gpu": smi1.summary()}
 tr = ops.enable_trace(True); step(); torch.cuda.synchronize(); ops.enable_trace(False)
 agg = collections.defaultdict(lambda: [0, 0.0])
 for name, note, a, b in tr:
     agg[name][0] += 1; agg[name][1] += a.elapsed_time(b)
 tot = sum(v[1] for v in agg.values())
-print(json.dumps({"workload": f"bisenetformer-l-ade bs={B} {W}x{H} (BASELINE configs[3])", "images_per_s": B / ms * 1e3, "ms_per_step": ms, "unfused_images_per_s": B / ms_unfused * 1e3, "unfused_ms_per_step": ms_unfused, "dtype": {"fp16": "f16", "fp32_tc": "f32 (3x f16 wgmma products)", "fp32": "f32 SIMT"}[PREC], "precision": PREC, "launches": len(tr),
-                  "peak_mem_gb": torch.cuda.max_memory_allocated() / 1e9}))
+print(json.dumps({"workload": f"{NAME} bs={B} {W}x{H}" + (" (BASELINE configs[3])" if NAME == "bisenetformer-l-ade" else ""), "images_per_s": B / ms * 1e3, "ms_per_step": ms, "unfused_images_per_s": B / ms_unfused * 1e3, "unfused_ms_per_step": ms_unfused, "dtype": {"fp16": "f16", "fp32_tc": "f32 (3x f16 wgmma products)", "fp32": "f32 SIMT"}[PREC], "precision": PREC, "launches": len(tr),
+                  "peak_mem_gb": torch.cuda.max_memory_allocated() / 1e9, **extra}))
 for k, (c, t) in sorted(agg.items(), key=lambda kv: -kv[1][1]):
     print(f"{t:9.2f} ms {100*t/tot:5.1f}%  n={c:4d}  {k}")
 if PREC == "fp16" and os.environ.get("FB200_BENCH_PARITY_MODE", "1") == "1":  # the parity-green mode (fp32_tc) of the same workload, in its own process
     import subprocess
-    del m, x
+    del m, fm, x
     torch.cuda.empty_cache()
     r = subprocess.run([sys.executable] + sys.argv, env=dict(os.environ, FB200_BENCH_PRECISION="fp32_tc", FB200_BENCH_PARITY_MODE="0"), capture_output=True, text=True, timeout=280)
     line = next((l for l in r.stdout.splitlines() if l.startswith("{")), None)

@@ -1,15 +1,17 @@
 """Config 3 of BASELINE.json: fai-mf-l-coco-ins, bs=16, 800x800 on one GPU — images/s of FAIMaskFormer.forward (+ GPU part of the
 instance post-process), CUDA events, plus a per-kernel-symbol time breakdown of one eager forward.
     python tools/bench_mf.py [batch] [size]
-FB200_BENCH_MODEL picks another fai_mf registry entry (default fai-mf-l-coco-ins; fai-mf-m-coco-ins, fai-mf-s-coco-ins), FB200_BENCH_PRECISION the precision
+FB200_BENCH_MODEL picks another fai_mf registry entry (default fai-mf-l-coco-ins; fai-mf-m-coco-ins, fai-mf-s-coco-ins, and the semantic fai-mf-l-ade,
+fai-mf-m-ade, whose step ends in the semantic argmax instead of the instance statistics), FB200_BENCH_PRECISION the precision
 (default fp16, which also runs fp32_tc in a second process).  FB200_BENCH_LATENCY=N adds the p50 / p90 of N single-image FocoosModel calls (uint8 image at
 [size]x[size], CUDA graph replay, post-processing included).  The JSON line carries the card, its power limit, and the median SM clock and the throttle
 reasons sampled with nvidia-smi during the timed window."""
-import json, os, sys, collections, statistics, subprocess, threading, time
+import json, os, sys, collections, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from focoos_b200 import ModelManager, ops
 from focoos_b200.utils.seeded_weights import seeded_state_dict
+from tools.smi import SmiSampler
 
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 16
 S = int(sys.argv[2]) if len(sys.argv) > 2 else 800
@@ -22,48 +24,19 @@ fm = ModelManager.get(NAME, state_dict=sd, precision=PREC)
 m = fm.model; m.cuda()
 
 
-class SmiSampler:
-    """nvidia-smi samples (SM clock MHz, active throttle reasons) every 0.2 s while active; card name and power limit read once"""
-
-    Q = "clocks.sm,clocks_throttle_reasons.active"
-
-    def __init__(self):
-        self.samples, self.stop = [], threading.Event()
-        try:
-            self.card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30).stdout.strip()
-        except (OSError, subprocess.TimeoutExpired):
-            self.card = "unknown"
-
-    def _run(self):
-        while not self.stop.is_set():
-            try:
-                out = subprocess.run(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits", "-i", "0"], capture_output=True, text=True, timeout=10).stdout
-                clk, thr = [t.strip() for t in out.strip().split(",")]
-                self.samples.append((float(clk), thr))
-            except (OSError, ValueError, subprocess.TimeoutExpired):
-                pass
-            time.sleep(0.2)
-
-    def __enter__(self):
-        self.t = threading.Thread(target=self._run, daemon=True); self.t.start(); return self
-
-    def __exit__(self, *a):
-        self.stop.set(); self.t.join()
-
-    def summary(self):
-        return {"card": self.card, "sm_clock_mhz_median": statistics.median([c for c, _ in self.samples]) if self.samples else None,
-                "throttle_reasons": sorted({t for _, t in self.samples})}
-
-
 x = torch.randint(0, 256, (B, S, S, 3), dtype=torch.uint8, device="cuda")
+SEMANTIC = m.config.postprocessing_type == "semantic"
 def step_unfused():  # the reference's split: model.forward returns [B,Q,H,W] probabilities, the processor reads them back
     out = m(x)
-    return ops.mask_stats(out.masks, 0.5)
-def step():          # what FocoosModel.__call__ runs: statistics fused into the upsampling (fai_mf.LazyMasks)
+    return ops.mask_argmax(out.masks, out.logits.max(-1).values) if SEMANTIC else ops.mask_stats(out.masks, 0.5)
+def step():          # what FocoosModel.__call__ runs: statistics (instance) or the argmax (semantic) fused into the upsampling (fai_mf.LazyMasks)
     m.lazy_masks = True
     out = m(x)
     m.lazy_masks = False
-    return ops.mask_sigmoid_upsample_stats(out.masks.logits, out.masks.num_queries, out.masks.size, 0.5)
+    lm = out.masks
+    if SEMANTIC:
+        return ops.mask_sigmoid_upsample_argmax(lm.logits, lm.num_queries, lm.size, out.logits.max(-1).values)
+    return ops.mask_sigmoid_upsample_stats(lm.logits, lm.num_queries, lm.size, 0.5)
 def timed(fn, n=5):
     for _ in range(3): fn()
     torch.cuda.synchronize()
