@@ -142,7 +142,8 @@ __device__ __forceinline__ void staging_open(int ct, F&& then) {
   consumer_bar();
 }
 // close: every consumer's writes are made visible to the TMA unit, the consumers meet, and thread 0 stores the chunk at channel n of the tile at
-// (w0, h0, img) - both planes of a pair - as one bulk group; the TMA unit clips ragged tiles and Cout tails
+// (w0, h0, img) - both planes of a pair - as one bulk group; the TMA unit clips ragged tiles, and Cout tails to whole 16-byte pieces (so
+// conv2d_tc_supported takes only Cout that end on one)
 template <typename TOut>
 __device__ __forceinline__ void staging_close(int ct, const uint8_t* stg, const CUtensorMap* tmap_d, const CUtensorMap* tmap_d2, int n, int w0, int h0, int img) {
   fence_proxy_async();
@@ -672,6 +673,9 @@ bool conv2d_tc_supported(const ConvParams& p, int x_dtype, int out_dtype) {
   if ((reinterpret_cast<uintptr_t>(p.x) | reinterpret_cast<uintptr_t>(p.w) | reinterpret_cast<uintptr_t>(p.out)) & 15) return false;
   const int oelt = out_dtype == FB200_F32 ? 4 : 2;   // element size of one stored plane
   if ((p.out_pitch * oelt) % 16 != 0) return false;
+  // a TMA store clips the channel dimension only to whole 16-byte pieces: with a Cout tail inside one (365 fp32, 100 fp16 channels) it would also write
+  // the columns up to the next 16-byte boundary, past the output view into the rest of the pitch.  The row-max epilogue stores nothing.
+  if (!p.rowmax && (p.Cout * oelt) % 16 != 0) return false;
   if (p.res && ((p.res_pitch * oelt) % 16 != 0 || (reinterpret_cast<uintptr_t>(p.res) & 15))) return false;
   if (p.res && out_dtype != FB200_F16PAIR && p.Cout % (128 / oelt) != 0) return false;  // residual is consumed in whole 128-byte row chunks
   if (p.KH != p.KW) return false;

@@ -285,6 +285,17 @@ class _Linear:
         self.w, self.bias, self.w3 = w, bias, None
 
 
+def _pad_rows(lin, mult):
+    """a packed linear with zero output rows (weight, weight triple, bias) up to a multiple of `mult`"""
+    n = -lin.w.shape[0] % mult
+    if not n:
+        return lin
+    pad = lambda t: torch.cat([t, t.new_zeros((n, *t.shape[1:]))])
+    out = _Linear(pad(lin.w), pad(lin.bias))
+    out.w3 = pad(lin.w3)
+    return out
+
+
 def _unpair(t):
     """a Pair as its fp32 values (a torch op: taps and the small 1/32 map of BisenetFormer's context path), any tensor as it is"""
     return t.float() if isinstance(t, ops.Pair) else t
@@ -346,6 +357,10 @@ class DetrEngine:
                     if layer.w3 is None:
                         layer.w3 = _split3_weights(layer.w)
             assert all(layer.w3 is not None for layer in self._pair_layers()), "fp32_tc: a layer of the pair flow has no [W_hi|W_lo|W_hi] weight triple"
+            if isinstance(getattr(self, "dec_score", None), _Linear):
+                # _forward_head_pair writes the class logits into rows padded to 16 bytes (the tensor-core store writes whole 16-byte pieces): zero rows up
+                # to that width make the launch own every column it stores
+                self.dec_score = _pad_rows(self.dec_score, 4)
         self._host_w3 = None
 
     def _pair_layers(self):
@@ -809,8 +824,8 @@ class DetrEngine:
                 taps[f"dec{i}_out"] = tgt
                 taps[f"dec{i}_ref"] = ref
         # class logits on the tensor cores into a 16-byte-padded row (TMA store pitch), then sigmoid into the dense [B,Q,C] scores
-        lbuf = torch.empty((B, nq, (ncls + 3) // 4 * 4), dtype=torch.float32, device=t.device)
-        logits = self._linear(self.dec_score, tgt_p, out=lbuf[..., :ncls])
+        lbuf = torch.empty((B, nq, self.dec_score.w.shape[0]), dtype=torch.float32, device=t.device)  # (ncls + 3) // 4 * 4 rows of the padded head
+        logits = self._linear(self.dec_score, tgt_p, out=lbuf)[..., :ncls]
         if taps is not None:
             taps.update(pred_logits=logits, pred_boxes_cxcywh=ref)
         return ops.sigmoid_rows(logits), ops.box_cxcywh_to_xyxy(ref)

@@ -304,6 +304,10 @@ class MFEngine(DetrEngine):
             # the same GEMM as three fp16 tensor-core products on the mask_features pair and the per-image embeddings as [W_hi | W_lo | W_hi] triples.
             # (On the CUDA-core fp32 kernel this product was a third of the parity-mode step: 16.9 of 50.4 ms at bs=16 800x800.)
             ops.conv2d_per_image(mask_features, _split3_weights(me).reshape(B, Q, 1, 1, 3 * C), out=masks[..., :Q])
+        elif dt == torch.float16 and Qp != Q:
+            # the fp16 tensor-core store writes whole 16-byte pieces (8 channels): the product runs on all Qp columns, zero embeddings past Q, so that
+            # it owns every column it writes
+            ops.conv2d_per_image(mask_features, nn.functional.pad(me, (0, 0, 0, Qp - Q)).reshape(B, Qp, 1, 1, C), out=masks, algo=A)
         else:
             ops.conv2d_per_image(mask_features, me.reshape(B, Q, 1, 1, C), out=masks[..., :Q], algo=A)
         attn = None

@@ -287,3 +287,43 @@ def test_linear_rowmax_pair_matches_fp32():
     ref = (x.reshape(-1, 256).double() @ w.double().t() + b.double()).max(-1).values.float().reshape(3, 1000)
     got = ops.linear_rowmax_pair(ops.Pair(ops.split_pair(x.to(DEV))), _split3_weights(w).to(DEV), b.to(DEV))
     assert float((got.cpu() - ref).abs().max()) <= 2e-5 * float(ref.abs().max())
+
+
+@pytest.mark.parametrize("out_dtype,Cout,pitch", [(torch.float32, 365, 368), (torch.float32, 81, 96), (torch.float16, 100, 104), (torch.float16, 151, 160)],
+                         ids=["f32-365", "f32-81", "f16-100", "f16-151"])
+def test_cout_tail_inside_a_16_byte_piece_leaves_the_pitch_padding(out_dtype, Cout, pitch):
+    """a Cout whose row ends inside a 16-byte piece (the 365-class head, the 100-query fp16 mask product), written into a slice of a wider buffer: the
+    columns past the view keep what they held.  A TMA store clips the channel dimension only to whole 16-byte pieces, so the tensor-core kernel refuses
+    such a Cout and AUTO runs it on the CUDA cores; before, the tensor-core store also wrote the columns up to the next 16-byte boundary."""
+    x = rnd((1, 1, 300, 256), torch.float16, 11)
+    w = rnd((Cout, 1, 1, 256), torch.float16, 12, 1.0 / 16)
+    bi = rnd((Cout,), torch.float32, 13, 0.2)
+    ref = torch.empty((1, 1, 300, Cout), dtype=out_dtype)
+    REF.conv2d(x, w, None, bi, 1, 0, 0, None, ref, 0)
+    buf = torch.full((1, 1, 300, pitch), float("nan"), dtype=out_dtype, device=DEV)
+    with pytest.raises(RuntimeError, match="tensor-core path does not support"):
+        ops.conv2d(x.to(DEV), w.to(DEV), None, bi.to(DEV), out=buf[..., :Cout], algo=ops.ALGO_TCGEN05)
+    ops.conv2d(x.to(DEV), w.to(DEV), None, bi.to(DEV), out=buf[..., :Cout])
+    torch.cuda.synchronize()
+    assert bool(torch.isnan(buf[..., Cout:]).all()), "a column past the output view was written"
+    got = buf[..., :Cout].float().cpu()
+    assert float((got - ref.float()).abs().max()) <= (3e-3 if out_dtype == torch.float16 else 1e-4) * max(1.0, float(ref.abs().max()))
+
+
+def test_conv2d_pair_refuses_a_cout_tail_inside_a_16_byte_piece():
+    """the fp32-accurate conv has no other kernel: a 365-channel fp32 output (1460-byte rows) is refused instead of written to 368 columns; the padded
+    368-row head the DETR pair flow packs writes its whole view"""
+    from focoos_b200.fai_detr import _split3_weights
+
+    x = rnd((1, 1, 300, 256), torch.float32, 21).to(DEV)
+    w = rnd((368, 1, 1, 256), torch.float32, 22, 1.0 / 16).to(DEV)
+    w[365:] = 0
+    buf = torch.full((1, 1, 300, 368), float("nan"), dtype=torch.float32, device=DEV)
+    with pytest.raises(RuntimeError, match="tensor-core path does not support"):
+        ops.conv2d_pair(ops.to_pair(x), _split3_weights(w[:365]), out=buf[..., :365], out_pair=False)
+    torch.cuda.synchronize()
+    assert bool(torch.isnan(buf).all())
+    ops.conv2d_pair(ops.to_pair(x), _split3_weights(w), out=buf, out_pair=False)
+    ref = (x.double().reshape(300, 256) @ w.double().reshape(368, 256).t()).reshape(1, 1, 300, 368)
+    assert float((buf.double() - ref).abs().max()) <= 1e-5 * max(1.0, float(ref.abs().max()))
+    assert float(buf[..., 365:].abs().max()) == 0.0
