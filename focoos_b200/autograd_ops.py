@@ -25,7 +25,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import ops
-from .fai_detr import _split3_weights
+from .engine import _split3_weights
 
 
 # ---- conv through either fp32 engine ----------------------------------------------------------------------------------

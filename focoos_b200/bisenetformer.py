@@ -14,7 +14,6 @@
 """
 from __future__ import annotations
 
-import math
 from dataclasses import dataclass, field, fields
 from typing import List, Optional
 
@@ -22,9 +21,10 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .fai_detr import STDC, ConvX, _bn_fold, _Conv, _CriterionStub, _packed_layers, _unpair
-from .fai_mf import MaskFormerModelOutput, MFEngine, PredictionHeads, _AttnLayer, _ConvBN, _FFNLayer, _SegmentationModel
+from .engine import _packed_layers, _unpair
+from .fai_mf import MaskFormerModelOutput, MFEngine, MultiScaleMaskedTransformerDecoder, _SegmentationModel
 from .ports import ModelOutput, STDCConfig
+from .trunks import STDC, ConvX, build_trunk, pack_trunk
 
 
 @dataclass
@@ -116,45 +116,26 @@ class BiseNet(nn.Module):  # bisenetformer/modelling.py:238
         self.conv_out = ConvX(feat_dim, out_dim, 3)
 
 
-class TransformerDecoder(nn.Module):  # bisenetformer/modelling.py:285 (two feature levels)
-    def __init__(self, in_ch, out_dim, num_classes, d, num_queries, nhead, dff, layers):
-        super().__init__()
-        self.transformer_self_attention_layers = nn.ModuleList([_AttnLayer(d, nhead, "self_attn") for _ in range(layers)])
-        self.transformer_cross_attention_layers = nn.ModuleList([_AttnLayer(d, nhead, "multihead_attn") for _ in range(layers)])
-        self.transformer_ffn_layers = nn.ModuleList([_FFNLayer(d, dff) for _ in range(layers)])
-        self.query_feat, self.query_embed = nn.Embedding(num_queries, d), nn.Embedding(num_queries, d)
-        self.input_proj = nn.ModuleList([_ConvBN(in_ch, d, 1, bias=True, norm=False) for _ in range(2)])
-        self.forward_prediction_heads = PredictionHeads(d, num_classes, out_dim)
-
-
-class BisenetFormerHead(nn.Module):
-    def __init__(self, predictor, num_classes):
-        super().__init__()
-        self.criterion = _CriterionStub(num_classes)
-        self.predictor = predictor
-
-
 class BisenetEngine(MFEngine):
     def _pack(self, sd):
         cfg = self.cfg
         self.nhead, self.d = 8, cfg.transformer_predictor_hidden_dim
-        self._pack_backbone(sd)
+        self.trunk = pack_trunk(self, sd)
         cp, ffm = "pixel_decoder.cp", "pixel_decoder.ffm"
-        self.conv_avg = self._convx(sd, cp + ".conv_avg", 1)
+        convx = lambda p: self._pack_conv(sd, p + ".conv.weight", bn=p + ".bn", act=ops.ACT_RELU)  # ConvBNReLU
+        self.conv_avg = convx(cp + ".conv_avg")
         self.arm = {}
         for name in ("arm32", "arm16"):
             q = f"{cp}.{name}"
-            sa, ba = _bn_fold(sd, q + ".bn_atten")
-            self.arm[name] = {"proj": _Conv(self._to(sd[q + ".proj.weight"].float().permute(0, 2, 3, 1)), None, None, 1, 0, ops.ACT_NONE),
-                              "conv": self._convx(sd, q + ".conv", 1),
-                              "att": _Conv(self._to(sd[q + ".conv_atten.weight"].float().permute(0, 2, 3, 1)), self._f32(sa), self._f32(ba), 1, 0, ops.ACT_SIGMOID)}
-        self.head32, self.head16 = self._convx(sd, cp + ".conv_head32", 1), self._convx(sd, cp + ".conv_head16", 1)
-        self.ffm_p1 = _Conv(self._to(sd[ffm + ".proj1.weight"].float().permute(0, 2, 3, 1)), None, self._f32(sd[ffm + ".proj1.bias"]), 1, 0, ops.ACT_NONE)
-        self.ffm_p2 = _Conv(self._to(sd[ffm + ".proj2.weight"].float().permute(0, 2, 3, 1)), None, self._f32(sd[ffm + ".proj2.bias"]), 1, 0, ops.ACT_NONE)
-        self.ffm_blk = self._convx(sd, ffm + ".convblk", 1)
-        self.ffm_c1 = _Conv(self._to(sd[ffm + ".conv1.weight"].float().permute(0, 2, 3, 1)), None, None, 1, 0, ops.ACT_RELU)
-        self.ffm_c2 = _Conv(self._to(sd[ffm + ".conv2.weight"].float().permute(0, 2, 3, 1)), None, None, 1, 0, ops.ACT_SIGMOID)
-        self.conv_out = self._convx(sd, "pixel_decoder.conv_out", 1)
+            self.arm[name] = {"proj": self._pack_conv(sd, q + ".proj.weight"), "conv": convx(q + ".conv"),
+                              "att": self._pack_conv(sd, q + ".conv_atten.weight", bn=q + ".bn_atten", act=ops.ACT_SIGMOID)}
+        self.head32, self.head16 = convx(cp + ".conv_head32"), convx(cp + ".conv_head16")
+        self.ffm_p1 = self._pack_conv(sd, ffm + ".proj1.weight", bias=ffm + ".proj1.bias")
+        self.ffm_p2 = self._pack_conv(sd, ffm + ".proj2.weight", bias=ffm + ".proj2.bias")
+        self.ffm_blk = convx(ffm + ".convblk")
+        self.ffm_c1 = self._pack_conv(sd, ffm + ".conv1.weight", act=ops.ACT_RELU)
+        self.ffm_c2 = self._pack_conv(sd, ffm + ".conv2.weight", act=ops.ACT_SIGMOID)
+        self.conv_out = convx("pixel_decoder.conv_out")
         self._pack_decoder(sd, 2)
 
     def _pair_layers(self):
@@ -168,14 +149,9 @@ class BisenetEngine(MFEngine):
 
     @torch.no_grad()
     def forward(self, images: torch.Tensor, taps: Optional[dict] = None):
-        cfg = self.cfg
-        if images.dtype == torch.uint8:
-            B, H, W, _ = images.shape
-        else:
-            assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
-            B, _, H, W = images.shape
+        B, H, W = self._input_size(images)
         # any H x W, like the reference (its processor does not resize): odd maps from the stride-2 convs and pools run on the same kernels
-        _, res3, res4, res5 = self._run_backbone(images)
+        _, res3, res4, res5 = self.trunk.run(images)
         res5 = _unpair(res5)  # global average pool + ARM gates work on fp32 (33 M elements at bs=64 1024x512)
         # context path; the convs that read res4 / res3 take a Pair to fp32 themselves
         avg = self._gate(self.conv_avg, ops.global_avgpool(res5))
@@ -203,11 +179,7 @@ class BisenetFormer(_SegmentationModel):
     engine_cls = BisenetEngine
 
     def __init__(self, config: BisenetFormerConfig, precision: str = "fp16"):
-        super().__init__(config, precision)
         c = config
-        self.pixel_decoder = BiseNet(STDC(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim)
-        self.head = BisenetFormerHead(TransformerDecoder(c.pixel_decoder_out_dim, c.transformer_predictor_out_dim, c.num_classes, c.transformer_predictor_hidden_dim,
-                                                         c.num_queries, 8, c.transformer_predictor_dim_feedforward, c.transformer_predictor_dec_layers), c.num_classes)
-        self.register_buffer("pixel_mean", torch.tensor(c.pixel_mean, dtype=torch.float32).view(-1, 1, 1), False)
-        self.register_buffer("pixel_std", torch.tensor(c.pixel_std, dtype=torch.float32).view(-1, 1, 1), False)
-        self.eval()
+        super().__init__(c, precision, BiseNet(build_trunk(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim),
+                         MultiScaleMaskedTransformerDecoder(c.pixel_decoder_out_dim, c.transformer_predictor_out_dim, c.num_classes, c.transformer_predictor_hidden_dim,
+                                                            c.num_queries, 8, c.transformer_predictor_dim_feedforward, c.transformer_predictor_dec_layers, 2))

@@ -22,104 +22,25 @@ from __future__ import annotations
 
 import math
 from collections import OrderedDict
-from typing import Dict, List, Optional
+from typing import Optional
 
 import torch
 import torch.nn as nn
 
 from . import ops
-from .ports import DETRConfig, DETRModelOutput, ResnetConfig, STDCConfig
+from .engine import Engine, _bn_fold, _channels, _Conv, _EngineModel, _Linear, _pad_rows, _packed_layers, _unpair
+from .ports import DETRConfig, DETRModelOutput
+from .trunks import ConvNormLayer, build_trunk, pack_trunk
+# these lived here before engine.py / trunks.py existed; bench.py and code written against that layout import them from this module
+from .engine import _split3_weights  # noqa: F401,E402
+from .trunks import STDC, ResNet  # noqa: F401,E402
 
-RESNET_BLOCKS = {50: [3, 4, 6, 3], 101: [3, 4, 23, 3]}
+NUM_POINTS = 4  # num_decoder_points (modelling.py:1039): sampling points per head and level of the deformable cross-attention
 
 
 # --------------------------------------------------------------------------------------------------
 # parameter containers (names = the reference's state_dict keys)
 # --------------------------------------------------------------------------------------------------
-class ConvNormLayer(nn.Module):  # nn/layers/conv.py:78
-    def __init__(self, ch_in, ch_out, k, stride, act=None):
-        super().__init__()
-        self.conv = nn.Conv2d(ch_in, ch_out, k, stride, padding=(k - 1) // 2, bias=False)
-        self.norm = nn.BatchNorm2d(ch_out)
-        self.act_name, self.stride = act, stride
-
-
-class BottleNeck(nn.Module):  # nn/backbone/resnet.py:72
-    def __init__(self, ch_in, ch_out, stride, shortcut):
-        super().__init__()
-        self.branch2a = ConvNormLayer(ch_in, ch_out, 1, 1, "relu")
-        self.branch2b = ConvNormLayer(ch_out, ch_out, 3, stride, "relu")
-        self.branch2c = ConvNormLayer(ch_out, ch_out * 4, 1, 1)
-        self.shortcut, self.stride = shortcut, stride
-        if not shortcut:
-            if stride == 2:
-                self.short = nn.Sequential(OrderedDict([("pool", nn.AvgPool2d(2, 2, 0, ceil_mode=True)), ("conv", ConvNormLayer(ch_in, ch_out * 4, 1, 1))]))
-            else:
-                self.short = ConvNormLayer(ch_in, ch_out * 4, 1, stride)
-
-
-class Blocks(nn.Module):  # nn/backbone/resnet.py:124
-    def __init__(self, ch_in, ch_out, count, stage_num):
-        super().__init__()
-        self.blocks = nn.ModuleList()
-        for i in range(count):
-            self.blocks.append(BottleNeck(ch_in, ch_out, stride=2 if i == 0 and stage_num != 2 else 1, shortcut=i != 0))
-            if i == 0:
-                ch_in = ch_out * 4
-
-
-class ResNet(nn.Module):  # nn/backbone/resnet.py:164 (variant d, depth >= 50)
-    def __init__(self, cfg: ResnetConfig):
-        super().__init__()
-        assert cfg.variant == "d" and cfg.depth in RESNET_BLOCKS, "focoos_b200 implements ResNet-50/101 vd"
-        self.depth = cfg.depth
-        self.conv1 = nn.Sequential(OrderedDict([
-            ("conv1_1", ConvNormLayer(cfg.in_chans, 32, 3, 2, "relu")),
-            ("conv1_2", ConvNormLayer(32, 32, 3, 1, "relu")),
-            ("conv1_3", ConvNormLayer(32, 64, 3, 1, "relu")),
-        ]))
-        self.res_layers = nn.ModuleList()
-        ch_in = 64
-        for i, (n, ch) in enumerate(zip(RESNET_BLOCKS[cfg.depth], [64, 128, 256, 512])):
-            self.res_layers.append(Blocks(ch_in, ch, n, i + 2))
-            ch_in = ch * 4
-        self.out_channels = [256, 512, 1024, 2048]
-
-
-class ConvX(nn.Module):  # nn/backbone/stdc.py:20 — also ConvBNReLU (bisenetformer/modelling.py:122)
-    def __init__(self, cin, cout, k=3, stride=1):
-        super().__init__()
-        self.conv = nn.Conv2d(cin, cout, k, stride, padding=k // 2, bias=False)
-        self.bn = nn.BatchNorm2d(cout)
-
-
-class CatBottleneck(nn.Module):  # nn/backbone/stdc.py:109
-    def __init__(self, cin, cout, stride):
-        super().__init__()
-        self.stride = stride
-        if stride == 2:
-            self.avd_layer = nn.Sequential(nn.Conv2d(cout // 2, cout // 2, 3, 2, 1, groups=cout // 2, bias=False), nn.BatchNorm2d(cout // 2))
-        self.conv_list = nn.ModuleList([ConvX(cin, cout // 2, 1), ConvX(cout // 2, cout // 4), ConvX(cout // 4, cout // 8), ConvX(cout // 8, cout // 8)])
-
-
-class STDC(nn.Module):  # nn/backbone/stdc.py:189
-    def __init__(self, cfg: STDCConfig):
-        super().__init__()
-        assert cfg.block_type == "cat" and cfg.block_num == 4, "focoos_b200 implements the CatBottleneck STDC (block_num 4)"
-        base, feats = cfg.base, []
-        feats += [ConvX(cfg.in_chans, base // 2, 3, 2), ConvX(base // 2, base, 3, 2)]
-        for i, n in enumerate(cfg.layers):
-            for j in range(n):
-                if i == 0 and j == 0:
-                    feats.append(CatBottleneck(base, base * 4, 2))
-                elif j == 0:
-                    feats.append(CatBottleneck(base * 2 ** (i + 1), base * 2 ** (i + 2), 2))
-                else:
-                    feats.append(CatBottleneck(base * 2 ** (i + 2), base * 2 ** (i + 2), 1))
-        self.features = nn.Sequential(*feats)
-        self.out_channels = [base, base * 4, base * 8, base * 16]
-
-
 class RepVggBlock(nn.Module):  # modelling.py:30
     def __init__(self, ch):
         super().__init__()
@@ -213,23 +134,6 @@ class TransformerPredictor(nn.Module):  # modelling.py:1023
         self.dec_bbox_classifier = nn.ModuleList([MLP(hidden, hidden, 4, 3) for _ in range(dec_layers)])
 
 
-class _CriterionStub(nn.Module):
-    """Holds `head.criterion.empty_weight` (it IS in the weight file, SURVEY Appendix B). Losses: later round."""
-
-    def __init__(self, num_classes):
-        super().__init__()
-        w = torch.ones(num_classes + 1)
-        w[-1] = 0.1
-        self.register_buffer("empty_weight", w)
-
-
-class DETRHead(nn.Module):  # modelling.py:350
-    def __init__(self, predictor, num_classes):
-        super().__init__()
-        self.criterion = _CriterionStub(num_classes)
-        self.predictor = predictor
-
-
 def generate_anchors(spatial_shapes, grid_size=0.05, eps=1e-2):
     """modelling.py:1169-1189 — logit-space anchors [S,4] fp32 and validity [S] (host, once per resolution)."""
     anchors = []
@@ -259,140 +163,20 @@ def aifi_position_embedding(h, w, num_pos_feats=128, temperature=10000.0):
 # --------------------------------------------------------------------------------------------------
 # the fused graph
 # --------------------------------------------------------------------------------------------------
-def _split3_weights(w):
-    """fp32 [..., C] -> fp16 [..., 3C] = [W_hi | W_lo | W_hi] (the weight operand of fb200_conv2d_pair)."""
-    hi = w.half()
-    lo = (w - hi.float()).half()
-    return torch.cat([hi, lo, hi], dim=-1).contiguous()
+class DetrEngine(Engine):
+    """Packs a FAIDetr state_dict and runs the fused forward: trunk, hybrid encoder, query selection, deformable decoder and head."""
 
-
-class _Conv:
-    """Packed conv: weight [Cout,KH,KW,Cin] in activation dtype, fp32 scale/bias (folded BN).
-    `w3` (precision="fp32_tc"): the [W_hi|W_lo|W_hi] fp16 triple of the pair flow's tensor-core products.  Run by DetrEngine._conv."""
-
-    __slots__ = ("w", "scale", "bias", "stride", "pad", "act", "w3")
-
-    def __init__(self, w, scale, bias, stride=1, pad=0, act=ops.ACT_NONE):
-        self.w, self.scale, self.bias, self.stride, self.pad, self.act, self.w3 = w, scale, bias, stride, pad, act, None
-
-
-class _Linear:
-    """Packed linear: weight [N,K] in activation dtype, fp32 bias, `w3` as in _Conv.  Run by DetrEngine._linear."""
-
-    __slots__ = ("w", "bias", "w3")
-
-    def __init__(self, w, bias):
-        self.w, self.bias, self.w3 = w, bias, None
-
-
-def _pad_rows(lin, mult):
-    """a packed linear with zero output rows (weight, weight triple, bias) up to a multiple of `mult`"""
-    n = -lin.w.shape[0] % mult
-    if not n:
-        return lin
-    pad = lambda t: torch.cat([t, t.new_zeros((n, *t.shape[1:]))])
-    out = _Linear(pad(lin.w), pad(lin.bias))
-    out.w3 = pad(lin.w3)
-    return out
-
-
-def _unpair(t):
-    """a Pair as its fp32 values (a torch op: taps and the small 1/32 map of BisenetFormer's context path), any tensor as it is"""
-    return t.float() if isinstance(t, ops.Pair) else t
-
-
-def _channels(t, a, b):
-    """channels [a, b) of an NHWC activation buffer (a tensor view or a Pair slice): concat-free blocks write their branches into them"""
-    return t.slice(a, b) if isinstance(t, ops.Pair) else t[..., a:b]
-
-
-_PAIR_MIN_ROWS = 64  # fp32_tc: an fp32 operand with fewer rows (MaskFormer's 1/32 encoder below ~256x256 input) stays on the CUDA-core fp32 kernel
-
-
-def _packed_layers(obj, seen=None):
-    """every packed layer (_Conv / _Linear) reachable from obj through dicts / lists / tuples, once each"""
-    seen = set() if seen is None else seen
-    if id(obj) in seen:
-        return
-    seen.add(id(obj))
-    if isinstance(obj, (_Conv, _Linear)):
-        yield obj
-    elif isinstance(obj, dict):
-        for v in obj.values():
-            yield from _packed_layers(v, seen)
-    elif isinstance(obj, (list, tuple)):
-        for v in obj:
-            yield from _packed_layers(v, seen)
-
-
-def _bn_fold(sd, p, eps=1e-5):
-    s = sd[p + ".weight"].float() / torch.sqrt(sd[p + ".running_var"].float() + eps)
-    return s, sd[p + ".bias"].float() - sd[p + ".running_mean"].float() * s
-
-
-class DetrEngine:
-    """Packs a state_dict for one (device, precision) and runs the fused forward.  The engines of the other families subclass it and implement `_pack`.
-
-    precision "fp16" / "fp32": activations in that dtype; `algo` goes to every conv / linear (ALGO_SIMT: the CUDA-core kernels).
-    precision "fp32_tc": the pair flow - fp32 storage, every conv / linear of the flow three fp16 tensor-core products on activations kept as fp16 [hi | lo]
-    planes between them; it runs only with the default algorithm choice.  `_conv` / `_linear` pick the kernel of every layer."""
-
-    def __init__(self, sd: Dict[str, torch.Tensor], cfg, device, precision: str = "fp16", algo: int = ops.ALGO_AUTO):
-        assert precision in ("fp32", "fp16", "fp32_tc")
-        if precision == "fp32_tc" and algo != ops.ALGO_AUTO:
-            raise ValueError(f"focoos_b200: precision 'fp32_tc' runs the tensor-core pair flow and takes no other algorithm (got algo={algo})")
-        self.cfg, self.device, self.precision, self.algo = cfg, torch.device(device), precision, algo
-        self.pair = precision == "fp32_tc"
-        self.dt = torch.float16 if precision == "fp16" else torch.float32
-        self._consts = {}  # per-resolution constants (_constants, MFEngine._pos)
-        self._host_w3 = {} if self.pair else None  # id(packed device weight) -> [W_hi|W_lo|W_hi] split on the host in _to()
-        # pack on the HOST (BN folding, re-parameterisation, concatenations are a few hundred tiny tensor ops: as device launches they were ~700 `at::`
-        # kernels in front of the first forward); only the packed tensors travel to the device
-        sd = {k: v.detach().to("cpu") for k, v in sd.items()}
-        self._pack(sd)
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
         if self.pair:
-            for layer in _packed_layers(vars(self)):
-                if layer.w.dtype == torch.float32 and layer.w.shape[-1] % 32 == 0:
-                    layer.w3 = self._host_w3.get(id(layer.w))
-                    if layer.w3 is None:
-                        layer.w3 = _split3_weights(layer.w)
-            assert all(layer.w3 is not None for layer in self._pair_layers()), "fp32_tc: a layer of the pair flow has no [W_hi|W_lo|W_hi] weight triple"
-            if isinstance(getattr(self, "dec_score", None), _Linear):
-                # _forward_head_pair writes the class logits into rows padded to 16 bytes (the tensor-core store writes whole 16-byte pieces): zero rows up
-                # to that width make the launch own every column it stores
-                self.dec_score = _pad_rows(self.dec_score, 4)
-        self._host_w3 = None
+            # _forward_head_pair writes the class logits into rows padded to 16 bytes (the tensor-core store writes whole 16-byte pieces): zero rows up
+            # to that width make the launch own every column it stores
+            self.dec_score = _pad_rows(self.dec_score, 4)
 
     def _pair_layers(self):
-        """the packed layers the fp32_tc flow runs on their weight triples: all but query_pos_head.layers.0 (K = 4), which stays fp32"""
-        return [layer for layer in _packed_layers(vars(self)) if layer is not self.qpos[0]]
-
-    # ---- packing -------------------------------------------------------------------------------
-    def _to(self, t, dtype=None):
-        d = t.to(device=self.device, dtype=dtype or self.dt).contiguous()
-        if self._host_w3 is not None and dtype is None and t.dim() >= 2 and t.shape[-1] % 32 == 0 and not t.is_cuda:
-            self._host_w3[id(d)] = _split3_weights(t.float().contiguous()).to(self.device)
-        return d
-
-    def _f32(self, t):
-        return t.to(device=self.device, dtype=torch.float32).contiguous()
-
-    def _cnl(self, sd, p, act=None, stride=1):
-        """ConvNormLayer -> _Conv with BN in the epilogue."""
-        w = sd[p + ".conv.weight"].float()
-        s, b = _bn_fold(sd, p + ".norm")
-        k = w.shape[-1]
-        return _Conv(self._to(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b), stride, (k - 1) // 2, ops.ACT[act])
-
-    def _seq_conv_bn(self, sd, pc, pn):
-        s, b = _bn_fold(sd, pn)
-        return _Conv(self._to(sd[pc + ".weight"].float().permute(0, 2, 3, 1)), self._f32(s), self._f32(b), 1, 0, ops.ACT_NONE)
-
-    def _lin(self, sd, p, rows=None, dtype=None):
-        w, b = sd[p + ".weight"].float(), sd[p + ".bias"].float()
-        if rows is not None:
-            w, b = w[rows], b[rows]
-        return _Linear(self._to(w, dtype), self._f32(b))
+        """the packed layers the fp32_tc flow runs on their weight triples: all but the trunk's stem (stem_conv) and query_pos_head.layers.0 (K = 4),
+        which stay fp32"""
+        return [layer for layer in _packed_layers(vars(self)) if layer is not self.qpos[0] and layer is not self.trunk.stem]
 
     def _csp(self, sd, p):
         w1, w2 = sd[p + ".conv1.conv.weight"].float(), sd[p + ".conv2.conv.weight"].float()
@@ -410,177 +194,20 @@ class DetrEngine:
             i += 1
         return both, reps
 
-    def _pack_backbone(self, sd, bb="pixel_decoder.backbone"):
-        """the trunk named by cfg.backbone_config.model_type, with folded BN (shared by every model family): ResNet-vd or STDC"""
-        if self.cfg.backbone_config.model_type == "stdc":
-            self._pack_stdc(sd, bb + ".features")
-        else:
-            self._pack_resnet(sd, bb)
-
-    def _pack_resnet(self, sd, bb):
-        """ResNet-vd (nn/backbone/resnet.py:164): stem + bottleneck stages."""
-        w = sd[bb + ".conv1.conv1_1.conv.weight"].float()
-        s, b = _bn_fold(sd, bb + ".conv1.conv1_1.norm")
-        self.stem_w, self.stem_s, self.stem_b = self._f32(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b)
-        self.stem2 = self._cnl(sd, bb + ".conv1.conv1_2", "relu")
-        self.stem3 = self._cnl(sd, bb + ".conv1.conv1_3", "relu")
-        self.stages = []
-        for si, count in enumerate(RESNET_BLOCKS[self.cfg.backbone_config.depth]):
-            blocks = []
-            for bi in range(count):
-                p = f"{bb}.res_layers.{si}.blocks.{bi}"
-                stride = 2 if (bi == 0 and si != 0) else 1
-                blk = {"a": self._cnl(sd, p + ".branch2a", "relu"), "b": self._cnl(sd, p + ".branch2b", "relu", stride),
-                       "c": self._cnl(sd, p + ".branch2c", "relu"), "stride": stride, "short": None}
-                if bi == 0:
-                    blk["short"] = self._cnl(sd, p + (".short.conv" if stride == 2 else ".short"), None)
-                blocks.append(blk)
-            self.stages.append(blocks)
-
-    def _pack_stdc(self, sd, bb):
-        """STDC (nn/backbone/stdc.py:189): two stride-2 ConvX stems + CatBottleneck stages; stride-2 blocks keep the depthwise 3x3/s2 + BN weights fp32 [9, C]."""
-        w = sd[bb + ".0.conv.weight"].float()
-        s, b = _bn_fold(sd, bb + ".0.bn")
-        self.stem_w, self.stem_s, self.stem_b = self._f32(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b)
-        self.stem2 = self._convx(sd, bb + ".1", 2)
-        self.blocks = []
-        idx = 2
-        for n in self.cfg.backbone_config.layers:
-            stage = []
-            for j in range(n):
-                p = f"{bb}.{idx}"
-                stride = 2 if j == 0 else 1
-                blk = {"stride": stride, "convs": [self._convx(sd, f"{p}.conv_list.{i}", 1) for i in range(4)]}
-                if stride == 2:
-                    wd = sd[p + ".avd_layer.0.weight"].float()  # [C,1,3,3]
-                    sa, ba = _bn_fold(sd, p + ".avd_layer.1")
-                    blk["avd"] = (self._f32(wd.reshape(wd.shape[0], 9).t()), self._f32(sa), self._f32(ba))
-                stage.append(blk)
-                idx += 1
-            self.blocks.append(stage)
-
-    def _convx(self, sd, p, stride):
-        w = sd[p + ".conv.weight"].float()
-        s, b = _bn_fold(sd, p + ".bn")
-        return _Conv(self._to(w.permute(0, 2, 3, 1)), self._f32(s), self._f32(b), stride, w.shape[-1] // 2, ops.ACT_RELU)
-
-    def _run_backbone(self, images):
-        """-> [res2, res3, res4, res5] NHWC of the packed trunk (shared by every model family)"""
-        if self.cfg.backbone_config.model_type == "stdc":
-            return self._run_stdc(images)
-        return self._run_resnet(images)
-
-    def _run_resnet(self, images):
-        """nn/backbone/resnet.py:252-266: Pairs under fp32_tc"""
-        cfg = self.cfg
-        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, self.dt, out_pair=self.pair)
-        x = self._conv(self.stem3, self._conv(self.stem2, x, out_pair=True), out_pair=True)
-        x = ops.maxpool3x3s2(x)
-        feats = []
-        for blocks in self.stages:
-            for blk in blocks:
-                y = self._conv(blk["b"], self._conv(blk["a"], x, out_pair=True), out_pair=True)
-                short = x if blk["short"] is None else self._conv(blk["short"], ops.avgpool2x2(x) if blk["stride"] == 2 else x, out_pair=True)
-                x = self._conv(blk["c"], y, residual=short, out_pair=True)
-            feats.append(x)
-        return feats
-
-    def _run_stdc(self, images):
-        """nn/backbone/stdc.py:314: res2 fp32 under fp32_tc; res3-5 are Pairs where the stage's last block runs in the pair format (_pair_block_ok)"""
-        cfg = self.cfg
-        x = ops.stem_conv(images.contiguous(), self.stem_w, self.stem_s, self.stem_b, cfg.pixel_mean, cfg.pixel_std, ops.ACT_RELU, self.dt)
-        x = self._conv(self.stem2, x)  # res2
-        feats = [x]
-        for stage in self.blocks:
-            for blk in stage:
-                x = self._cat_bottleneck(x, blk)
-            feats.append(x)
-        return feats
-
-    def _cat_bottleneck(self, x, blk):
-        """CatBottleneck, concat-free: each conv writes its channel slice of the block's output buffer, which the next conv reads in place.  A block that
-        _pair_block_ok takes keeps the buffer as a Pair (no split pass inside the block); a stride-2 block's first conv reads a Pair input and writes fp32."""
-        c = blk["convs"]
-        half = c[0].w.shape[0]
-        B, H, W, _ = x.shape
-        if blk["stride"] == 2:
-            out1 = self._conv(c[0], x)
-            buf = torch.empty((B, (H - 1) // 2 + 1, (W - 1) // 2 + 1, 2 * half), dtype=self.dt, device=x.device)
-            ops.avgpool3x3s2(out1, out=buf[..., :half])
-            src = ops.dwconv3x3s2(out1, *blk["avd"])
-        else:
-            shape = (B, H, W, 2 * half)
-            buf = ops.Pair.empty(shape, x.device) if self._pair_block_ok(blk, H, W) else torch.empty(shape, dtype=self.dt, device=x.device)
-            src = self._conv(c[0], x, out=_channels(buf, 0, half))
-        o = half
-        for i in (1, 2, 3):
-            w = c[i].w.shape[0]
-            src = self._conv(c[i], src, out=_channels(buf, o, o + w))
-            o += w
-        return buf
-
-    def _pair_block_ok(self, blk, H, W) -> bool:
-        """conv2d_pair takes the block: every conv has its weight triple; a 32-channel 3x3 input needs the halo mode (rows of at least 64 pixels, Cout <= 64)"""
-        if blk["stride"] != 1 or not self.pair:
-            return False
-        for cv in blk["convs"]:
-            cin, cout, k = cv.w.shape[3], cv.w.shape[0], cv.w.shape[1]
-            if cv.w3 is None or cout % 8:
-                return False
-            if cin % 64 and not (cin == 32 and k == 3 and W >= 64 and cout <= 64):
-                return False
-        return True
-
-    # ---- the layer call: the one place that picks a conv / linear kernel from the precision and the operand's format ---------------------------------
-    def _on_pairs(self, layer, x, algo, out_pair):
-        """fp32_tc: whether the layer runs as three fp16 tensor-core products on the pair planes of x (conv2d_pair) rather than on the fp32 CUDA cores.
-        A Pair operand or a Pair result can only take the products.  An fp32 operand with an fp32 result stays on the CUDA cores when the call asks for
-        ALGO_SIMT (the [B,C] gates, the MaskFormer classifier), when the layer has no weight triple, or when it has fewer than _PAIR_MIN_ROWS rows."""
-        if not self.pair:
-            return False
-        if isinstance(x, ops.Pair) or out_pair:
-            return True
-        return algo != ops.ALGO_SIMT and layer.w3 is not None and x.numel() // x.shape[-1] >= _PAIR_MIN_ROWS
-
-    def _conv(self, conv, x, *, act=None, residual=None, out=None, out_dtype=None, algo=None, out_pair=False):
-        """one packed conv.  fp16 / fp32: ops.conv2d on the storage weight with `algo` (default self.algo).  fp32_tc (see _on_pairs): ops.conv2d_pair on
-        the weight triple - x a Pair or split into one - whose result is a Pair with out_pair=True or a Pair `out`, else fp32.  The storage flow ignores
-        out_pair.  The residual has the result's format."""
-        act = conv.act if act is None else act
-        algo = self.algo if algo is None else algo
-        if self._on_pairs(conv, x, algo, out_pair or isinstance(out, ops.Pair)):
-            assert act & 15 not in (ops.ACT_GELU, ops.ACT_SIGMOID), "no layer of the pair flow has a GELU / sigmoid epilogue"
-            return ops.conv2d_pair(ops.to_pair(x), conv.w3, conv.scale, conv.bias, stride=conv.stride, pad=conv.pad, act=act, residual=residual, out=out,
-                                   out_pair=out_pair)
-        return ops.conv2d(x, conv.w, conv.scale, conv.bias, stride=conv.stride, pad=conv.pad, act=act, residual=residual, out=out, out_dtype=out_dtype, algo=algo)
-
-    def _linear(self, lin, x, *, act=ops.ACT_NONE, residual=None, out=None, out_dtype=None, algo=None, out_pair=False):
-        """one packed linear on tokens [..., K]: ops.linear, or under fp32_tc ops.linear_pair, chosen as in _conv.  `out` may be a column slice of a wider
-        fp32 buffer."""
-        algo = self.algo if algo is None else algo
-        if self._on_pairs(lin, x, algo, out_pair):
-            assert act & 15 not in (ops.ACT_GELU, ops.ACT_SIGMOID), "no layer of the pair flow has a GELU / sigmoid epilogue"
-            return ops.linear_pair(ops.to_pair(x), lin.w3, lin.bias, act=act, residual=residual, out=out, out_pair=out_pair)
-        return ops.linear(x, lin.w, lin.bias, act=act, residual=residual, out=out, out_dtype=out_dtype, algo=algo)
-
-    def _empty(self, shape, device):
-        """an activation buffer of the flow: a Pair under fp32_tc, else a tensor in the storage dtype"""
-        return ops.Pair.empty(shape, device) if self.pair else torch.empty(shape, dtype=self.dt, device=device)
-
     def _pack(self, sd):
         cfg = self.cfg
         self.nhead, self.d = cfg.transformer_predictor_nhead, cfg.transformer_predictor_hidden_dim
-        self._pack_backbone(sd)
+        self.trunk = pack_trunk(self, sd)
         pd = "pixel_decoder"
-        self.enc_in = [self._seq_conv_bn(sd, f"{pd}.input_proj.{i}.0", f"{pd}.input_proj.{i}.1") for i in range(3)]
+        self.enc_in = [self._pack_conv(sd, f"{pd}.input_proj.{i}.0.weight", bn=f"{pd}.input_proj.{i}.1") for i in range(3)]
         # the AIFI layer on the 1/32 map (fai-detr-l-*); fai-detr-m-coco has none (pixel_decoder_num_encoder_layers 0)
         self.aifi = self._pack_attn_block(sd, f"{pd}.encoder.0.layers.0", ffn_norms=("norm1", "norm2")) if cfg.pixel_decoder_num_encoder_layers else None
-        self.lateral = [self._cnl(sd, f"{pd}.lateral_convs.{i}", "silu") for i in range(2)]
+        self.lateral = [self._pack_conv(sd, f"{pd}.lateral_convs.{i}.conv.weight", bn=f"{pd}.lateral_convs.{i}.norm", act=ops.ACT_SILU) for i in range(2)]
         self.fpn = [self._csp(sd, f"{pd}.fpn_blocks.{i}") for i in range(2)]
-        self.down = [self._cnl(sd, f"{pd}.downsample_convs.{i}", "silu") for i in range(2)]
+        self.down = [self._pack_conv(sd, f"{pd}.downsample_convs.{i}.conv.weight", bn=f"{pd}.downsample_convs.{i}.norm", act=ops.ACT_SILU) for i in range(2)]
         self.pan = [self._csp(sd, f"{pd}.pan_blocks.{i}") for i in range(2)]
         hp = "head.predictor"
-        self.dec_in = [self._seq_conv_bn(sd, f"{hp}.input_proj.{i}.conv", f"{hp}.input_proj.{i}.norm") for i in range(3)]
+        self.dec_in = [self._pack_conv(sd, f"{hp}.input_proj.{i}.conv.weight", bn=f"{hp}.input_proj.{i}.norm") for i in range(3)]
         self.enc_output = self._lin(sd, hp + ".enc_output.0")
         self.enc_output_ln = (self._f32(sd[hp + ".enc_output.1.weight"]), self._f32(sd[hp + ".enc_output.1.bias"]))
         self.enc_score = self._lin(sd, hp + ".enc_score_classifier")
@@ -602,18 +229,6 @@ class DetrEngine:
             blk["bbox"] = [self._lin(sd, f"{hp}.dec_bbox_classifier.{i}.layers.{j}") for j in range(3)]
             self.dec.append(blk)
         self.dec_score = self._lin(sd, f"{hp}.dec_score_classifier.{L - 1}")
-
-    def _pack_attn_block(self, sd, p, ffn_norms, d=None):
-        """MultiheadAttention (packed in_proj: rows [0,d)=Q, [d,2d)=K, [2d,3d)=V) + FFN + the two LayerNorms around them; d defaults to self.d."""
-        d = self.d if d is None else d
-        w, b = sd[p + ".self_attn.in_proj_weight"].float(), sd[p + ".self_attn.in_proj_bias"].float()
-        n_attn, n_ffn = ffn_norms
-        return {
-            "qk": _Linear(self._to(w[: 2 * d]), self._f32(b[: 2 * d])), "v": _Linear(self._to(w[2 * d:]), self._f32(b[2 * d:])),
-            "out": self._lin(sd, p + ".self_attn.out_proj"), "l1": self._lin(sd, p + ".linear1"), "l2": self._lin(sd, p + ".linear2"),
-            "n_attn": (self._f32(sd[f"{p}.{n_attn}.weight"]), self._f32(sd[f"{p}.{n_attn}.bias"])),
-            "n_ffn": (self._f32(sd[f"{p}.{n_ffn}.weight"]), self._f32(sd[f"{p}.{n_ffn}.bias"])),
-        }
 
     def _constants(self, h32, w32):
         key = (h32, w32)
@@ -670,7 +285,7 @@ class DetrEngine:
     def _trunk(self, images, taps):
         """backbone + hybrid encoder + decoder input projection -> (memory [B,S,d] - a Pair under fp32_tc, else in the storage dtype -, shapes, constants)"""
         cfg = self.cfg
-        _, res3, res4, res5 = self._run_backbone(images)
+        _, res3, res4, res5 = self.trunk.run(images)
         B, h32, w32, _ = res5.shape
         K = self._constants(h32, w32)
         C = cfg.pixel_decoder_feat_dim
@@ -722,13 +337,8 @@ class DetrEngine:
 
     @torch.no_grad()
     def forward(self, images: torch.Tensor, taps: Optional[dict] = None):
-        """images [B,3,H,W] fp32 0..255 (H,W multiples of 32) -> (scores [B,Q,C] fp32, boxes xyxy [B,Q,4] fp32)."""
-        if images.dtype == torch.uint8:  # [B,H,W,3] decoded images straight into the stem kernel
-            assert images.dim() == 4 and images.shape[3] == 3
-            B, H, W, _ = images.shape
-        else:
-            assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
-            B, _, H, W = images.shape
+        """images [B,3,H,W] fp32 0..255 or [B,H,W,3] uint8 (H,W multiples of 32) -> (scores [B,Q,C] fp32, boxes xyxy [B,Q,4] fp32)."""
+        B, H, W = self._input_size(images)
         if H % 32 or W % 32:
             # DETRProcessor resizes to im_size; the encoder buffers, anchors and positional constants are laid out for 1/8 and 1/16 maps of exactly 4x and
             # 2x the 1/32 map, so the engine takes multiples of 32 - resize or pad in the processor (image_size) for other inputs
@@ -767,7 +377,7 @@ class DetrEngine:
             pos = self._linear(self.qpos[1], self._linear(self.qpos[0], ref, act=ops.ACT_RELU, out_dtype=dt, algo=ops.ALGO_SIMT))
             tgt = self._mha(blk, tgt, pos)
             oa = self._linear(blk["oa"], ops.add(tgt, pos), out_dtype=torch.float32)
-            c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, cfg_points(cfg), self.nhead, out_dtype=dt)
+            c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, NUM_POINTS, self.nhead, out_dtype=dt)
             tgt = ops.layernorm(self._linear(blk["cross_out"], c, residual=tgt), *blk["n_cross"])
             tgt = self._ffn(blk, tgt, ops.ACT_RELU)
             bbox = blk["bbox"]
@@ -811,7 +421,7 @@ class DetrEngine:
             y = self._linear(blk["out"], a, residual=tgt)
             tgt, _, tpp = ops.layernorm_ex(y, *blk["n_attn"], pos=pos, want_pair=False, want_pair_pos=True)
             oa = self._linear(blk["oa"], tpp)
-            c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, cfg_points(cfg), self.nhead, out_pair=True)
+            c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, NUM_POINTS, self.nhead, out_pair=True)
             y = self._linear(blk["cross_out"], c, residual=tgt)
             tgt, tgt_p, _ = ops.layernorm_ex(y, *blk["n_cross"])
             y = self._linear(blk["l2"], self._linear(blk["l1"], tgt_p, act=ops.ACT_RELU, out_pair=True), residual=tgt)
@@ -831,51 +441,6 @@ class DetrEngine:
         return ops.sigmoid_rows(logits), ops.box_cxcywh_to_xyxy(ref)
 
 
-def cfg_points(cfg) -> int:
-    return 4  # num_decoder_points (modelling.py:1039)
-
-
-class _EngineModel(nn.Module):
-    """The nn.Module side of every model family: parameters under the reference's state_dict keys, `.device` / `.dtype` from `pixel_mean`, and
-    the `engine_cls` engine packed from the parameters for the current (device, precision, algo) on first use, dropped whenever they may change."""
-
-    engine_cls: type
-
-    def __init__(self, config, precision: str = "fp16"):
-        super().__init__()
-        self.config, self.num_classes, self.precision, self.algo, self._engine = config, config.num_classes, precision, ops.ALGO_AUTO, None
-
-    device = property(lambda self: self.pixel_mean.device)
-    dtype = property(lambda self: self.pixel_mean.dtype)
-
-    def load_state_dict(self, state_dict, strict: bool = False, assign: bool = False):
-        """Shape-tolerant non-strict load like BaseModelNN.load_state_dict (models/base_model.py:98-143); accepts
-        {"model": sd} checkpoints (focoos_model.py:684-685)."""
-        if "model" in state_dict and isinstance(state_dict["model"], dict):
-            state_dict = state_dict["model"]
-        own = self.state_dict()
-        filtered = {k: v for k, v in state_dict.items() if k in own and tuple(own[k].shape) == tuple(v.shape)}
-        res = super().load_state_dict(filtered, strict=False)
-        self._engine = None
-        if strict and (res.missing_keys or len(filtered) != len(state_dict)):
-            raise RuntimeError(f"load_state_dict(strict): missing {res.missing_keys[:5]} / dropped {len(state_dict) - len(filtered)}")
-        return res
-
-    def _apply(self, fn, *a, **k):
-        self._engine = None
-        return super()._apply(fn, *a, **k)
-
-    def engine(self):
-        e = self._engine
-        if e is None or e.device != self.device or e.precision != self.precision or e.algo != self.algo:
-            self._engine = self.engine_cls(self.state_dict(), self.config, self.device, self.precision, self.algo)
-        return self._engine
-
-    def _check_device(self, images):
-        if ops._backend is None and not images.is_cuda:
-            raise RuntimeError(f"focoos_b200.{type(self).__name__} runs on CUDA (sm_90a) only — no CPU fallback; move the model and inputs to the GPU")
-
-
 class FAIDetr(_EngineModel):
     """Drop-in for the reference `FAIDetr(BaseModelNN)` (modelling.py:1273): same constructor argument, same
     state_dict, `forward(images[, targets]) -> DETRModelOutput`."""
@@ -883,16 +448,12 @@ class FAIDetr(_EngineModel):
     engine_cls = DetrEngine
 
     def __init__(self, config: DETRConfig, precision: str = "fp16"):
-        super().__init__(config, precision)
         c = config
-        backbone = STDC(c.backbone_config) if c.backbone_config.model_type == "stdc" else ResNet(c.backbone_config)
-        self.pixel_decoder = Encoder(backbone, c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_nhead,
-                                     c.pixel_decoder_dim_feedforward, c.pixel_decoder_num_encoder_layers)
-        self.head = DETRHead(TransformerPredictor(c.pixel_decoder_out_dim, c.num_classes, c.transformer_predictor_hidden_dim, c.num_queries,
-                                                  c.transformer_predictor_nhead, c.transformer_predictor_dec_layers,
-                                                  c.transformer_predictor_dim_feedforward), c.num_classes)
-        self.register_buffer("pixel_mean", torch.tensor(c.pixel_mean, dtype=torch.float32).view(-1, 1, 1), False)
-        self.register_buffer("pixel_std", torch.tensor(c.pixel_std, dtype=torch.float32).view(-1, 1, 1), False)
+        super().__init__(c, precision,
+                         Encoder(build_trunk(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_nhead,
+                                 c.pixel_decoder_dim_feedforward, c.pixel_decoder_num_encoder_layers),
+                         TransformerPredictor(c.pixel_decoder_out_dim, c.num_classes, c.transformer_predictor_hidden_dim, c.num_queries,
+                                              c.transformer_predictor_nhead, c.transformer_predictor_dec_layers, c.transformer_predictor_dim_feedforward))
         self.train_precision = None  # training arithmetic: None (follow `precision`), "fp32", "fp32_tc" or "amp" (see train_graph)
         self.sync_bn = False    # training: BatchNorm statistics over all data-parallel ranks (torch.nn.SyncBatchNorm, trainer/trainer.py:334); set by the trainer
         self.freeze_bn = False  # training: every BatchNorm as FrozenBatchNorm2d (TrainerArgs.freeze_bn, trainer/trainer.py:330)
@@ -900,7 +461,6 @@ class FAIDetr(_EngineModel):
         freeze_backbone_at(self, getattr(c.backbone_config, "freeze_at", -1), getattr(c.backbone_config, "num_stages", 4))  # resnet.py:221-224
         if getattr(c.backbone_config, "freeze_norm", False):  # resnet.py:226 (the registry configs ship freeze_norm=false)
             freeze_backbone_norm(self)
-        self.eval()
 
     def train(self, mode: bool = True):
         self._engine = None  # packed (BN-folded, re-parameterised) weights are rebuilt from the parameters at the next eval forward

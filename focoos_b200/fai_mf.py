@@ -3,7 +3,7 @@
 Same pattern as `fai_detr.py`: the module tree only holds parameters under the reference's state_dict keys
 (SURVEY Appendix B, 937 entries for fai-mf-l-coco-ins); `FAIMaskFormer.forward` runs `MFEngine`, a fused NHWC graph:
 
-  * ResNet-101-vd backbone (shared kernels / packing with FAIDetr),
+  * ResNet-101-vd or STDC trunk (trunks.py, shared with the other families),
   * TransformerFPN pixel decoder: 1x1 input_proj -> 6 PRE-norm encoder layers with the normalised sine embedding
     (nn/layers/position_encoding.py:45-74) -> final LayerNorm -> 3x3+BN+ReLU; lateral 1x1+BN, nearest x2 upsample + add
     fused in one kernel, 3x3+BN+ReLU; mask_features 3x3 (fai_mf/modelling.py:348-369),
@@ -26,8 +26,10 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .fai_detr import _split3_weights, MLP, STDC, DetrEngine, ResNet, _bn_fold, _Conv, _CriterionStub, _EngineModel, _Linear, _packed_layers
+from .engine import Engine, _EngineModel, _Linear, _packed_layers, _split3_weights
+from .fai_detr import MLP
 from .ports import ModelOutput, ResnetConfig, STDCConfig, backbone_config_from_dict
+from .trunks import STDC, ResNet, build_trunk, pack_trunk
 
 
 @dataclass
@@ -176,22 +178,15 @@ class PredictionHeads(nn.Module):  # fai_mf/modelling.py:28
         self.mask_classifier = MLP(d, d, mask_dim, 3)
 
 
-class MultiScaleMaskedTransformerDecoder(nn.Module):  # fai_mf/modelling.py:372
-    def __init__(self, in_ch, out_dim, num_classes, d, num_queries, nhead, dff, layers):
+class MultiScaleMaskedTransformerDecoder(nn.Module):  # fai_mf/modelling.py:372; bisenetformer/modelling.py:285 (TransformerDecoder, two levels)
+    def __init__(self, in_ch, out_dim, num_classes, d, num_queries, nhead, dff, layers, levels=3):
         super().__init__()
         self.transformer_self_attention_layers = nn.ModuleList([_AttnLayer(d, nhead, "self_attn") for _ in range(layers)])
         self.transformer_cross_attention_layers = nn.ModuleList([_AttnLayer(d, nhead, "multihead_attn") for _ in range(layers)])
         self.transformer_ffn_layers = nn.ModuleList([_FFNLayer(d, dff) for _ in range(layers)])
         self.query_feat, self.query_embed = nn.Embedding(num_queries, d), nn.Embedding(num_queries, d)
-        self.input_proj = nn.ModuleList([_ConvBN(in_ch, d, 1, bias=True, norm=False) for _ in range(3)])
+        self.input_proj = nn.ModuleList([_ConvBN(in_ch, d, 1, bias=True, norm=False) for _ in range(levels)])
         self.forward_prediction_heads = PredictionHeads(d, num_classes, out_dim)
-
-
-class MaskFormerHead(nn.Module):  # fai_mf/modelling.py:563
-    def __init__(self, predictor, num_classes):
-        super().__init__()
-        self.criterion = _CriterionStub(num_classes)
-        self.predictor = predictor
 
 
 def position_embedding_sine_normalized(h, w, num_pos_feats=128, temperature=10000.0):
@@ -209,8 +204,8 @@ def position_embedding_sine_normalized(h, w, num_pos_feats=128, temperature=1000
     return torch.cat((py, px), dim=2).reshape(h * w, -1)
 
 
-class MFEngine(DetrEngine):
-    """Packs a FAIMaskFormer state_dict and runs the fused forward (reuses DetrEngine's packing helpers and backbone)."""
+class MFEngine(Engine):
+    """Packs a FAIMaskFormer state_dict and runs the fused forward: trunk, TransformerFPN pixel decoder, masked transformer decoder and head."""
 
     lazy_masks = False  # True: return LazyMasks instead of the materialised [B,Q,H,W] probabilities
 
@@ -219,36 +214,31 @@ class MFEngine(DetrEngine):
         self.nhead, self.d = 8, cfg.transformer_predictor_hidden_dim  # masked decoder
         # the pixel-decoder encoder has its own width and heads: 256 x 8 heads of 32 channels (fai-mf-l), 128 x 8 heads of 16 channels (fai-mf-m / -s)
         self.pd_d, self.pd_nhead = cfg.pixel_decoder_feat_dim, cfg.pixel_decoder_transformer_nheads
-        self._pack_backbone(sd)
+        self.trunk = pack_trunk(self, sd)
         pd = "pixel_decoder"
         # no encoder (fai-mf-*-ade): no input_proj, no encoder layers, no final LayerNorm - layer_4 reads res5
         self.pd_in = self.enc_norm = None
         self.enc = [self._pack_attn_block(sd, f"{pd}.transformer.encoder.layers.{i}", ffn_norms=("norm1", "norm2"), d=self.pd_d)
                     for i in range(cfg.pixel_decoder_transformer_layers)]
         if self.enc:
-            self.pd_in = self._conv_bias(sd, pd + ".input_proj", 0)
+            self.pd_in = self._pack_conv(sd, pd + ".input_proj.weight", bias=pd + ".input_proj.bias")
             self.enc_norm = (self._f32(sd[pd + ".transformer.encoder.norm.weight"]), self._f32(sd[pd + ".transformer.encoder.norm.bias"]))
-        self.layer = {i: self._conv_bn(sd, f"{pd}.layer_{i}", 1, ops.ACT_RELU) for i in (1, 2, 3, 4)}
-        self.adapter = {i: self._conv_bn(sd, f"{pd}.adapter_{i}", 0, ops.ACT_NONE) for i in (1, 2, 3)}
-        self.mask_features = self._conv_bias(sd, pd + ".mask_features", 1)
+        self.layer = {i: self._pack_conv(sd, f"{pd}.layer_{i}.weight", bn=f"{pd}.layer_{i}.norm", act=ops.ACT_RELU) for i in (1, 2, 3, 4)}
+        self.adapter = {i: self._pack_conv(sd, f"{pd}.adapter_{i}.weight", bn=f"{pd}.adapter_{i}.norm") for i in (1, 2, 3)}
+        self.mask_features = self._pack_conv(sd, pd + ".mask_features.weight", bias=pd + ".mask_features.bias")
         self._pack_decoder(sd, 3)
 
     def _pair_layers(self):
-        """the backbone, the pixel-decoder convs that read its pairs, the 1/4-resolution chain into mask_features, and the decoder linears.
-        ResNet trunk: its stems and bottleneck stages; STDC trunk: its second stem and the CatBottleneck convs (whether a block runs on pairs is
-        _pair_block_ok's call).  res5 is read by input_proj, or without an encoder by layer_4 itself."""
-        if self.cfg.backbone_config.model_type == "stdc":
-            trunk = [self.stem2, [blk["convs"] for stage in self.blocks for blk in stage]]
-        else:
-            trunk = [self.stem2, self.stem3, self.stages]
+        """the trunk's pair layers (on an STDC trunk, whether a block runs on pairs is _pair_block_ok's call), the pixel-decoder convs that read its
+        pairs, the 1/4-resolution chain into mask_features, and the decoder linears.  res5 is read by input_proj, or without an encoder by layer_4 itself."""
         res5_reader = self.pd_in if self.enc else self.layer[4]
-        return list(_packed_layers([trunk, res5_reader, self.adapter, self.layer[1], self.mask_features, self.dec, self.mask_mlp]))
+        return self.trunk.pair_layers() + list(_packed_layers([res5_reader, self.adapter, self.layer[1], self.mask_features, self.dec, self.mask_mlp]))
 
     def _pack_decoder(self, sd, num_levels):
         """head.predictor.* of the masked transformer decoder (same key names in fai_mf and bisenetformer)."""
         cfg = self.cfg
         hp = "head.predictor"
-        self.dec_in = [self._conv_bias(sd, f"{hp}.input_proj.{i}", 0) for i in range(num_levels)]
+        self.dec_in = [self._pack_conv(sd, f"{hp}.input_proj.{i}.weight", bias=f"{hp}.input_proj.{i}.bias") for i in range(num_levels)]
         self.query_feat, self.query_embed = self._to(sd[hp + ".query_feat.weight"].float()), self._to(sd[hp + ".query_embed.weight"].float())
         d = self.d
         self.dec = []
@@ -268,13 +258,6 @@ class MFEngine(DetrEngine):
         self.head_norm = (self._f32(sd[h + ".decoder_norm.weight"]), self._f32(sd[h + ".decoder_norm.bias"]))
         self.classifier = self._lin(sd, h + ".classifier")
         self.mask_mlp = [self._lin(sd, f"{h}.mask_classifier.layers.{j}") for j in range(3)]
-
-    def _conv_bias(self, sd, p, pad):
-        return _Conv(self._to(sd[p + ".weight"].float().permute(0, 2, 3, 1)), None, self._f32(sd[p + ".bias"]), 1, pad, ops.ACT_NONE)
-
-    def _conv_bn(self, sd, p, pad, act):
-        s, b = _bn_fold(sd, p + ".norm")
-        return _Conv(self._to(sd[p + ".weight"].float().permute(0, 2, 3, 1)), self._f32(s), self._f32(b), 1, pad, act)
 
     def _pos(self, h, w, d=None):
         """the normalised sine embedding of an h x w map for a d-wide sequence (default: the decoder width self.d)"""
@@ -318,15 +301,11 @@ class MFEngine(DetrEngine):
 
     @torch.no_grad()
     def forward(self, images: torch.Tensor, taps: Optional[dict] = None):
-        if images.dtype == torch.uint8:
-            B, H, W, _ = images.shape
-        else:
-            assert images.dim() == 4 and images.shape[1] == 3 and images.dtype == torch.float32
-            B, _, H, W = images.shape
+        B, H, W = self._input_size(images)
         # any H x W, like the reference (its processor does not resize): odd maps from the stride-2 convs and ceil-mode pools run on the same kernels
         # fp32_tc: the backbone keeps its activations as fp16 [hi | lo] planes between convs (no split pass in front of every conv); the four pixel-decoder
         # convs that consume res2..res5 read the pairs and write the fp32 tensors the transformer / FPN arithmetic below works on
-        res2, res3, res4, res5 = self._run_backbone(images)
+        res2, res3, res4, res5 = self.trunk.run(images)
         d, nh = self.pd_d, self.pd_nhead
         scale = 1.0 / math.sqrt(d // nh)
         # ---- pixel decoder (TransformerFPN.forward_features)
@@ -447,16 +426,11 @@ class FAIMaskFormer(_SegmentationModel):
     engine_cls = MFEngine
 
     def __init__(self, config: MaskFormerConfig, precision: str = "fp16"):
-        super().__init__(config, precision)
         c = config
         if c.postprocessing_type not in ("semantic", "instance"):
             raise ValueError(f"Invalid postprocessing type: {c.postprocessing_type}. Must be one of: ['semantic', 'instance']")
-        backbone = STDC(c.backbone_config) if c.backbone_config.model_type == "stdc" else ResNet(c.backbone_config)
-        self.pixel_decoder = TransformerFPN(backbone, c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_transformer_layers,
-                                            c.pixel_decoder_transformer_nheads, c.pixel_decoder_transformer_dim_feedforward)
-        self.head = MaskFormerHead(MultiScaleMaskedTransformerDecoder(c.pixel_decoder_out_dim, c.transformer_predictor_out_dim, c.num_classes,
-                                                                      c.transformer_predictor_hidden_dim, c.num_queries, 8,
-                                                                      c.transformer_predictor_dim_feedforward, c.transformer_predictor_dec_layers), c.num_classes)
-        self.register_buffer("pixel_mean", torch.tensor(c.pixel_mean, dtype=torch.float32).view(-1, 1, 1), False)
-        self.register_buffer("pixel_std", torch.tensor(c.pixel_std, dtype=torch.float32).view(-1, 1, 1), False)
-        self.eval()
+        super().__init__(c, precision,
+                         TransformerFPN(build_trunk(c.backbone_config), c.pixel_decoder_feat_dim, c.pixel_decoder_out_dim, c.pixel_decoder_transformer_layers,
+                                        c.pixel_decoder_transformer_nheads, c.pixel_decoder_transformer_dim_feedforward),
+                         MultiScaleMaskedTransformerDecoder(c.pixel_decoder_out_dim, c.transformer_predictor_out_dim, c.num_classes, c.transformer_predictor_hidden_dim,
+                                                            c.num_queries, 8, c.transformer_predictor_dim_feedforward, c.transformer_predictor_dec_layers))

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from focoos_b200 import ModelManager, ops
-from focoos_b200.fai_detr import _split3_weights
+from focoos_b200.engine import _split3_weights
 from focoos_b200.processor import MaskFormerProcessor
 from focoos_b200.utils.seeded_weights import seeded_state_dict
 from oracle.gen_golden import synth_images

@@ -16,7 +16,7 @@ import torch.nn.functional as F
 
 from focoos_b200 import ops
 from focoos_b200.bisenetformer import BisenetFormer, BisenetFormerConfig
-from focoos_b200.fai_detr import _split3_weights
+from focoos_b200.engine import _split3_weights
 from focoos_b200.fai_mf import FAIMaskFormer, MaskFormerConfig
 from focoos_b200.processor import MaskFormerProcessor
 from focoos_b200.utils.seeded_weights import seeded_state_dict

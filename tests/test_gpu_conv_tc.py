@@ -98,7 +98,7 @@ def test_conv_cin32_swizzle64(H, W, Cin, Cout, k):
                                                           (3, 20, 20, 512, 2048, 1, 1, True), (2, 80, 80, 256, 256, 3, 2, False)])  # pair + residual (2-stage ring), stride-2 pair
 def test_split_precision_conv_matches_fp32(B, H, W, Cin, Cout, k, stride, res):
     """precision="fp32_tc": fp32 tensors, three fp16 tensor-core products (hi*hi + hi*lo + lo*hi) -> fp32-level agreement."""
-    from focoos_b200.fai_detr import _split3_weights
+    from focoos_b200.engine import _split3_weights
 
     x = rnd((B, H, W, Cin), torch.float32, 1, 3.0)
     w = rnd((Cout, k, k, Cin), torch.float32, 2, 1.0 / math.sqrt(k * k * Cin))
@@ -121,7 +121,7 @@ def test_split_precision_conv_matches_fp32(B, H, W, Cin, Cout, k, stride, res):
 def test_split_precision_conv_has_no_fp16_output():
     """a split-precision conv writes fp32 or the pair: an fp16 output is refused on the host, before any launch, and fp32 is the default.  ops.conv2d with
     ALGO_TCGEN05_SPLIT3 on the dense [hi|lo] tensor is conv2d_pair with a plain output, bit for bit."""
-    from focoos_b200.fai_detr import _split3_weights
+    from focoos_b200.engine import _split3_weights
 
     xp = ops.split_pair(rnd((2, 20, 20, 64), torch.float32, 1).to(DEV))
     w3 = _split3_weights(rnd((64, 3, 3, 64), torch.float32, 2, 0.04)).to(DEV)
@@ -217,7 +217,7 @@ def _pair_from(x32):
                                                           (3, 20, 20, 512, 2048, 1, 1, True), (1, 1, 1000, 256, 512, 1, 1, False), (2, 7, 9, 64, 128, 3, 1, True)])
 def test_conv2d_pair_output_and_residual(B, H, W, Cin, Cout, k, stride, res):
     """out = Pair: hi + lo reproduce the fp32 reference conv to split precision; the pair residual is read back as hi + lo"""
-    from focoos_b200.fai_detr import _split3_weights
+    from focoos_b200.engine import _split3_weights
     x = rnd((B, H, W, Cin), torch.float32, 1, 3.0)
     w = rnd((Cout, k, k, Cin), torch.float32, 2, 1.0 / math.sqrt(k * k * Cin))
     bi, sc = rnd((Cout,), torch.float32, 3, 0.2), torch.rand(Cout) + 0.5
@@ -241,7 +241,7 @@ def test_conv2d_pair_output_and_residual(B, H, W, Cin, Cout, k, stride, res):
 
 def test_conv2d_pair_channel_slices_of_a_wider_pair_buffer():
     """CSP pattern: input = channels [0, C) of a 2C pair buffer, residual = channels [C, 2C), output = a slice of another pair buffer"""
-    from focoos_b200.fai_detr import _split3_weights
+    from focoos_b200.engine import _split3_weights
     C = 128
     y12 = rnd((2, 20, 24, 2 * C), torch.float32, 11, 2.0)
     w = rnd((C, 3, 3, C), torch.float32, 12, 0.03)
@@ -280,7 +280,7 @@ def test_stem_conv_pair_output():
 
 def test_linear_rowmax_pair_matches_fp32():
     """query-selection scores of the fp32-accurate mode: max over the 365 class logits per row, straight from the tensor-core epilogue"""
-    from focoos_b200.fai_detr import _split3_weights
+    from focoos_b200.engine import _split3_weights
     x = rnd((3, 1000, 256), torch.float32, 1, 2.0)
     w = rnd((365, 256), torch.float32, 2, 0.08)
     b = rnd((365,), torch.float32, 3, 0.5)
@@ -313,7 +313,7 @@ def test_cout_tail_inside_a_16_byte_piece_leaves_the_pitch_padding(out_dtype, Co
 def test_conv2d_pair_refuses_a_cout_tail_inside_a_16_byte_piece():
     """the fp32-accurate conv has no other kernel: a 365-channel fp32 output (1460-byte rows) is refused instead of written to 368 columns; the padded
     368-row head the DETR pair flow packs writes its whole view"""
-    from focoos_b200.fai_detr import _split3_weights
+    from focoos_b200.engine import _split3_weights
 
     x = rnd((1, 1, 300, 256), torch.float32, 21).to(DEV)
     w = rnd((368, 1, 1, 256), torch.float32, 22, 1.0 / 16).to(DEV)

@@ -13,7 +13,7 @@ import pytest
 import torch
 
 from focoos_b200 import ops
-from focoos_b200.fai_detr import _split3_weights
+from focoos_b200.engine import _split3_weights
 from oracle.ops_ref import RefBackend
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]

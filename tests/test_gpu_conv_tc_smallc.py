@@ -12,7 +12,7 @@ import torch
 import torch.nn.functional as F
 
 from focoos_b200 import ops
-from focoos_b200.fai_detr import _split3_weights
+from focoos_b200.engine import _split3_weights
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(180)]
 DEV = "cuda"

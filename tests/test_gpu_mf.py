@@ -91,7 +91,7 @@ def test_masked_attention_split_precision(hw, Q):
 def test_per_image_mask_product_split_precision(B, h, w, C, Q):
     """einsum("bqc,bchw->bqhw") with per-image weights on the fp32-accurate tensor-core path (fb200_conv2d_pair with a weight batch stride: x = the Pair of
     mask_features, w = per-image [W_hi|W_lo|W_hi] triples) vs fp64, into the first Q columns of a padded NHWC buffer like MFEngine._heads does."""
-    from focoos_b200.fai_detr import _split3_weights
+    from focoos_b200.engine import _split3_weights
     x, me = rnd((B, h, w, C), torch.float32, 11), rnd((B, Q, C), torch.float32, 12, 0.5)
     ref = torch.einsum("bqc,bhwc->bhwq", me.double(), x.double())
     Qp = (Q + 7) // 8 * 8

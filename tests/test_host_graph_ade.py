@@ -12,7 +12,7 @@ import torch
 from focoos_b200 import FAIMaskFormer, ModelManager, ops
 from focoos_b200.bisenetformer import BisenetFormer
 from focoos_b200.export import _rebuild, make_meta
-from focoos_b200.fai_detr import STDC, ResNet
+from focoos_b200.trunks import STDC, ResNet
 from focoos_b200.fai_mf import MaskFormerConfig
 from focoos_b200.ports import ResnetConfig, STDCConfig
 from focoos_b200.processor import MaskFormerProcessor
@@ -171,7 +171,7 @@ def test_mf_l_ade_pair_flow_runs_trunk_and_layer_4_as_pair_convs(ref_backend):
     m, _ = _model("fai-mf-l-ade", "fp32_tc")
     eng = m.engine()
     assert eng.pd_in is None and eng.enc == [] and eng.enc_norm is None
-    layers = [eng.stem2, eng.stem3, *[blk[k] for st in eng.stages for blk in st for k in ("a", "b", "c", "short") if blk[k] is not None], eng.layer[4]]
+    layers = [eng.trunk.stem2, eng.trunk.stem3, *[blk[k] for st in eng.trunk.stages for blk in st for k in ("a", "b", "c", "short") if blk[k] is not None], eng.layer[4]]
     assert all(any(layer is p for p in eng._pair_layers()) for layer in layers)
     ops._backend = calls = ConvCalls(ops._backend)
     m(torch.from_numpy(synth_images(5, [(96, 128)])[0]).permute(2, 0, 1).float()[None])
@@ -186,7 +186,7 @@ def test_mf_m_ade_pair_layers_name_the_stdc_trunk():
     m, _ = _model("fai-mf-m-ade", "fp32_tc")
     eng = m.engine()
     pl = eng._pair_layers()
-    stdc = [eng.stem2, *[c for st in eng.blocks for blk in st for c in blk["convs"]], eng.layer[4]]
+    stdc = [eng.trunk.stem2, *[c for st in eng.trunk.blocks for blk in st for c in blk["convs"]], eng.layer[4]]
     assert all(any(layer is p for p in pl) for layer in stdc) and all(layer.w3 is not None for layer in pl)
 
 

@@ -76,14 +76,14 @@ def test_bisenet_pair_blocks_run_as_pair_convs(ref_backend):
     m.load_state_dict(seeded_state_dict(manifest_template("bisenetformer_l_ade"), 0), strict=True)
     eng = m.engine()
     H, W = (int(v) for v in g["sizes"][0])
-    taken = [eng._pair_block_ok(blk, H // (8 << si), W // (8 << si)) for si, stage in enumerate(eng.blocks) for blk in stage]
-    assert sum(taken) >= 6 and not any(t for t, blk in zip(taken, [b for st in eng.blocks for b in st]) if blk["stride"] == 2)
+    taken = [eng.trunk._pair_block_ok(blk, H // (8 << si), W // (8 << si)) for si, stage in enumerate(eng.trunk.blocks) for blk in stage]
+    assert sum(taken) >= 6 and not any(t for t, blk in zip(taken, [b for st in eng.trunk.blocks for b in st]) if blk["stride"] == 2)
     imgs = synth_images(4, [tuple(s) for s in g["sizes"].tolist()])
     x = torch.stack([torch.from_numpy(im).permute(2, 0, 1).float() for im in imgs])
     taps = {}
     ops._backend = calls = ConvCalls(ops._backend)
     out = m(x, taps=taps)
-    pair_convs = [c for t, blk in zip(taken, [b for st in eng.blocks for b in st]) if t for c in blk["convs"]]
+    pair_convs = [c for t, blk in zip(taken, [b for st in eng.trunk.blocks for b in st]) if t for c in blk["convs"]]
     paired = {id(w) for w in calls.w["conv2d_pair"]}
     assert all(id(c.w3) in paired for c in pair_convs)
     assert not any(c.w is w or c.w3 is w for c in pair_convs for w in calls.w["conv2d"])

@@ -10,7 +10,7 @@ import torch
 
 from focoos_b200 import FAIDetr, DETRConfig, DETRProcessor, ops
 from focoos_b200.export import _rebuild, make_meta
-from focoos_b200.fai_detr import STDC
+from focoos_b200.trunks import STDC
 from focoos_b200.model_manager import _REGISTRY, ModelManager
 from focoos_b200.ports import ResnetConfig, STDCConfig
 from focoos_b200.trainer import TrainerArgs, run_train_entry
@@ -116,7 +116,7 @@ def test_fp32_tc_runs_only_pair_convs_and_matches_golden(ref_backend):
     ops._backend = calls.be
     assert not calls.w["conv2d"] and calls.w["conv2d_pair"]
     eng = m.engine()
-    assert any(eng._pair_block_ok(blk, 640 // (8 << si), 640 // (8 << si)) for si, stage in enumerate(eng.blocks) for blk in stage)
+    assert any(eng.trunk._pair_block_ok(blk, 640 // (8 << si), 640 // (8 << si)) for si, stage in enumerate(eng.trunk.blocks) for blk in stage)
     _check_backbone_taps(g, taps)
     ds, db = compare_queries(g["scores"], g["boxes"], g["enc_topk_ind"], out.logits.numpy(), out.boxes.numpy(), taps["topk_ind"].numpy())
     assert ds < 2e-4 and db < 2e-4, (ds, db)

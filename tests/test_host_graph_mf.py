@@ -74,7 +74,7 @@ def test_mf_fused_graph_matches_golden(ref_backend):
 
 
 def test_mf_pair_backbone_runs_as_pair_convs(ref_backend):
-    """precision="fp32_tc": the ResNet backbone runs in the pair format (fp16 hi/lo planes between convs, DetrEngine._run_backbone) and the four pixel-decoder
+    """precision="fp32_tc": the ResNet backbone runs in the pair format (fp16 hi/lo planes between convs, ResNetTrunk.run) and the four pixel-decoder
     convs read the pairs - host-side bookkeeping on the CPU references: same outputs as the fp32 graph up to the pair rounding (2^-22 relative per activation)."""
     g = load_golden("mf_l_coco_ins_b2_320x416")
     m = FAIMaskFormer(MaskFormerConfig(), precision="fp32_tc")
@@ -85,7 +85,7 @@ def test_mf_pair_backbone_runs_as_pair_convs(ref_backend):
     ops._backend = calls = ConvCalls(ops._backend)
     out = m(x, taps=taps)
     eng = m.engine()
-    backbone = [eng.stem2, eng.stem3] + [blk[k] for st in eng.stages for blk in st for k in ("a", "b", "c", "short") if blk[k] is not None]
+    backbone = [eng.trunk.stem2, eng.trunk.stem3] + [blk[k] for st in eng.trunk.stages for blk in st for k in ("a", "b", "c", "short") if blk[k] is not None]
     paired = {id(w) for w in calls.w["conv2d_pair"]}
     assert all(id(c.w3) in paired for c in backbone + [eng.pd_in, *eng.adapter.values(), eng.layer[1], eng.mask_features])
     assert not any(c.w is w or c.w3 is w for c in backbone for w in calls.w["conv2d"])

@@ -11,7 +11,7 @@ import numpy as np
 import torch
 from bench import measured_peaks
 from focoos_b200 import ops
-from focoos_b200.fai_detr import _split3_weights
+from focoos_b200.engine import _split3_weights
 
 B = 32
 SHAPES = [("conv1_2", 320, 320, 32, 32), ("conv1_3", 320, 320, 32, 64), ("res2_branch2b", 160, 160, 64, 64)]

@@ -6,7 +6,7 @@ import hashlib, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from focoos_b200 import ops
-from focoos_b200.fai_detr import _split3_weights
+from focoos_b200.engine import _split3_weights
 
 if not torch.cuda.is_available():
     sys.exit("conv_tc_digest: needs a CUDA device")
