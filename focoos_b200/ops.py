@@ -441,6 +441,17 @@ class CudaBackend:
         self._call("fb200_label_resize_bbox", _p(labels), labels.shape[1], labels.shape[2], _p(bq), bq.shape[0], _p(out_masks), out_masks.shape[1], out_masks.shape[2],
                    _p(out_bbox), _stream())
 
+    def _mask_png(self, masks, bbox, lengths):
+        """-> uint8 buffer holding the PNG files of the crops back to back (its capacity bounds them; `lengths` says how many bytes each has).
+        Not one of the per-operator methods the CPU reference backend mirrors: the encoding has no place in the tests' host graphs, and its CPU
+        restatement (oracle/png_ref.py) is compared with this one directly."""
+        self._cuda(masks, bbox, lengths)
+        n, H, W = masks.shape
+        out = torch.empty((n * self.lib.fb200_mask_png_bound(H, W),), dtype=torch.uint8, device=masks.device)
+        ws = _ws(self.lib.fb200_mask_png_workspace_bytes(n, H, W), masks.device)
+        self._call("fb200_mask_png", _p(masks), n, H, W, _p(bbox), _p(out), _p(lengths), _p(ws), _stream())
+        return out
+
     # ---- backward / training-mode kernels (autograd_ops.py) ------------------------------------------------------------
     def conv_wgrad(self, x, dy, KH, KW, stride, pad, dw):
         self._cuda(x, dy, dw)
@@ -652,13 +663,15 @@ class Pair:
 _cuda_backend = None
 
 
-def _be():
+def _cuda_be() -> CudaBackend:
     global _cuda_backend
-    if _backend is not None:
-        return _backend
     if _cuda_backend is None:
         _cuda_backend = CudaBackend()
     return _cuda_backend
+
+
+def _be():
+    return _backend if _backend is not None else _cuda_be()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1209,3 +1222,20 @@ def label_resize_bbox(labels, bq_i32, size):
     if n:
         _be().label_resize_bbox(labels.contiguous(), bq_i32.contiguous(), om, ob)
     return om, ob
+
+
+def mask_png(masks_u8, boxes):
+    """PNG files of the crops masks_u8[i][y1:min(y2,H), x1:min(x2,W)] (boxes [n,4] int32 xyxy, as mask_resize_bbox / label_resize_bbox return them), byte
+    for byte what `cv2.imencode(".png", crop * 255)` writes, encoded on the device in one launch sequence.
+    -> (bytes uint8 [sum(lengths)] on the device: the files back to back, lengths int32 [n] on the host: 0 for a crop without rows or columns).
+    Reading the lengths is the one synchronisation; the masks themselves never leave the device."""
+    assert masks_u8.dtype == torch.uint8 and masks_u8.dim() == 3 and boxes.shape == (masks_u8.shape[0], 4)
+    n = masks_u8.shape[0]
+    lengths = torch.zeros((n,), dtype=torch.int32, device=masks_u8.device)
+    if n == 0:
+        return torch.empty((0,), dtype=torch.uint8, device=masks_u8.device), lengths.cpu()
+    out = _cuda_be()._mask_png(masks_u8.contiguous(), boxes.to(torch.int32).contiguous(), lengths)
+    lens = lengths.cpu()
+    if bool((lens < 0).any()):
+        raise RuntimeError(f"focoos_b200.mask_png: masks {torch.nonzero(lens < 0).flatten().tolist()} have a negative box corner or need a stored deflate block")
+    return out[: int(lens.sum())], lens

@@ -8,6 +8,7 @@ replacing the reference's per-image Python loop with 3 `.cpu().tolist()` syncs e
 """
 from __future__ import annotations
 
+import base64
 from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -220,7 +221,7 @@ class MaskFormerProcessor(DETRProcessor):
     """preprocess as the base Processor; postprocess = the reference's tensor pipeline as GPU reductions + one compaction:
     per (image, query): pixel count and probability mass of `prob >= mask_threshold` (ONE pass over the [B,Q,H,W] tensor),
     class score x mask score, threshold, then only the KEPT masks are binarised / resized to the original image size and
-    boxed on the device and copied to the host for PNG encoding.  Works for any batch size (the reference raises IndexError
+    boxed and PNG-encoded on the device; only the PNG files travel to the host, for base64.  Works for any batch size (the reference raises IndexError
     for B >= 2, SURVEY A.25): the batched result equals the concatenation of the reference's per-image results."""
 
     def __init__(self, config, image_size=None):
@@ -277,6 +278,26 @@ class MaskFormerProcessor(DETRProcessor):
             res.append((nz[keep].astype(np.int32), s[keep].astype(np.float32), labels[nz][keep].astype(np.int32)))
         return res
 
+    @staticmethod
+    def _crops_to_base64(m, box):
+        """(boxes as a host array, base64 PNG of every crop m[i][y1:min(y2,H), x1:min(x2,W)]) - trim_mask + binary_mask_to_base64, utils/vision.py:264-293.
+        Device masks are encoded on the device (ops.mask_png): only the files and their lengths reach the host.  Host masks come only from the CPU
+        reference backend of the tests (every product op refuses host tensors) and are encoded by binary_mask_to_base64 itself."""
+        H, W = m.shape[1:]
+        if not m.is_cuda:
+            mh, box_h = m.numpy().astype(bool), box.numpy()
+            return box_h, [binary_mask_to_base64(mh[i][y1:min(y2, H), x1:min(x2, W)]) for i, (x1, y1, x2, y2) in enumerate(box_h.tolist())]
+        png, lens = ops.mask_png(m, box)
+        box_h, data = box.cpu().numpy(), png.cpu().numpy().tobytes()
+        out, off = [], 0
+        for (x1, y1, x2, y2), n in zip(box_h.tolist(), lens.tolist()):
+            if n:
+                out.append(base64.b64encode(data[off:off + n]).decode("utf-8"))
+                off += n
+            else:  # a crop with no rows or no columns: whatever binary_mask_to_base64 does with it
+                out.append(binary_mask_to_base64(np.zeros((max(0, min(y2, H) - y1), max(0, min(x2, W) - x1)), dtype=bool)))
+        return box_h, out
+
     def postprocess(self, output, inputs, class_names=(), top_k=None, threshold=None, use_mask_score=None, predict_all_pixels=None):
         image_sizes = get_image_sizes(inputs)
         B = output.logits.shape[0]
@@ -298,12 +319,11 @@ class MaskFormerProcessor(DETRProcessor):
                     m, box = ops.mask_resize_bbox(planes, idx, float(self.mask_threshold), image_sizes[b])
                 else:
                     m, box = ops.mask_resize_bbox(self._masks, bq, float(self.mask_threshold), image_sizes[b])
-            m, box = m.cpu().numpy().astype(bool), box.cpu().numpy()
+            box_h, masks_b64 = self._crops_to_base64(m, box)
             dets = []
             for i in range(len(q)):
-                x1, y1, x2, y2 = (int(v) for v in box[i])
-                crop = m[i][y1:min(y2, m[i].shape[0]), x1:min(x2, m[i].shape[1])]  # trim_mask (utils/vision.py:264-267)
-                dets.append(FocoosDet(bbox=[x1, y1, x2, y2], conf=float(s[i]), cls_id=int(l[i]), mask=binary_mask_to_base64(crop),
+                x1, y1, x2, y2 = (int(v) for v in box_h[i])
+                dets.append(FocoosDet(bbox=[x1, y1, x2, y2], conf=float(s[i]), cls_id=int(l[i]), mask=masks_b64[i],
                                       label=class_names[int(l[i])] if class_names else None))
             results.append(FocoosDetections(detections=dets))
         return results

@@ -273,6 +273,16 @@ int fb200_mask_argmax(const float* masks, const float* scores, int B, int Q, int
 /* kept one-hot masks -> original image size + boxes: pair i = (b,q): (labels[b] == q) -> bilinear resize -> != 0 (processor.py:275-283). */
 int fb200_label_resize_bbox(const uint8_t* labels, int H, int W, const int* bq, int n, uint8_t* out, int Ho, int Wo, int* bbox, void* stream);
 
+/* PNG files of the kept mask crops (trim_mask + binary_mask_to_base64, utils/vision.py:264-293; fai_mf/processor.py:275-304): for mask i of
+ * masks [n,H,W] uint8 (non-zero = set) and bbox[i] = (x1,y1,x2,y2) from fb200_mask_resize_bbox / fb200_label_resize_bbox, the crop
+ * masks[i][y1:min(y2,H), x1:min(x2,W)] encoded byte for byte as cv2.imencode(".png", crop * 255) encodes it (SUB-filtered rows, zlib
+ * Z_RLE deflate, 8192-byte IDAT chunks).  out receives the files back to back (mask i at the sum of the lengths before it) and must hold
+ * n * fb200_mask_png_bound(H, W) bytes; lengths [n] i32: bytes of each file, 0 for a crop with no rows or no columns, -1 for a crop zlib
+ * would store uncompressed (not produced by any 0/255 mask seen) or a negative x1 / y1.  workspace: fb200_mask_png_workspace_bytes. */
+int fb200_mask_png_bound(int H, int W);
+int64_t fb200_mask_png_workspace_bytes(int n, int H, int W);
+int fb200_mask_png(const uint8_t* masks, int n, int H, int W, const int* bbox, uint8_t* out, int* lengths, void* workspace, void* stream);
+
 /* ---- training criterion (SURVEY 8 a20) ---------------------------------------------------------------------
  * Replaces BoxHungarianMatcher.forward (focoos/models/fai_detr/modelling.py:693-758) and SetCriterion.forward with
  * loss_labels_vfl / loss_boxes (:464-531, :553-612) for all L supervised layers at once.
