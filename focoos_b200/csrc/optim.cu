@@ -41,8 +41,8 @@ __global__ void __launch_bounds__(256) grad_stats_kernel(const float* __restrict
 
 // ctrl words: see include/focoos_b200.h (FB200_CTRL_*)
 __global__ void optim_finalize_kernel(const double* __restrict__ partial, const int* __restrict__ flags, int nblk, float* __restrict__ ctrl, float max_norm,
-                                      int clip_passes, float inv_world, int use_scaler, float growth, float backoff, int growth_interval, float beta1,
-                                      float beta2) {
+                                      int clip_passes, float inv_world, int use_scaler, float growth, float backoff, int growth_interval,
+                                      float one_minus_beta1, float one_minus_beta2) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   int* ictrl = reinterpret_cast<int*>(ctrl);
   double s = 0.0;
@@ -66,8 +66,8 @@ __global__ void optim_finalize_kernel(const double* __restrict__ partial, const 
   if (!bad) {
     const int step = ictrl[5] + 1;
     ictrl[5] = step;
-    ctrl[6] = (float)(1.0 - pow((double)beta1, (double)step));
-    ctrl[7] = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+    ctrl[6] = (float)(1.0 - pow(1.0 - (double)one_minus_beta1, (double)step));
+    ctrl[7] = (float)sqrt(1.0 - pow(1.0 - (double)one_minus_beta2, (double)step));
   }
   if (use_scaler) {                                       // GradScaler.update (torch/amp/grad_scaler.py: _amp_update_scale_)
     if (bad) { ctrl[0] = scale * backoff; ictrl[1] = 0; }
@@ -81,10 +81,12 @@ __global__ void optim_finalize_kernel(const double* __restrict__ partial, const 
 
 // torch.optim.AdamW (single-tensor path, torch/optim/adam.py): p *= 1 - lr*wd; m = lerp(m, g, 1-b1); v = b2*v + (1-b2)*g*g;
 // p -= (lr / bc1) * m / (sqrt(v) / sqrt(bc2) + eps).   One CTA per chunk; a chunk never straddles two tensors.
+// omb1 / omb2 = 1 - beta as the caller formed it before rounding to fp32, as torch's scalars are (1 - fp32(0.999) is 1.3e-5 smaller than
+// fp32(0.001)).
 __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                                                      const int64_t* __restrict__ chunk_start, const int* __restrict__ chunk_len, const int* __restrict__ chunk_seg,
                                                      const float* __restrict__ seg_lr, const float* __restrict__ seg_wd, const int* __restrict__ seg_active, float lr_factor,
-                                                     float beta1, float beta2, float eps, const float* __restrict__ ctrl) {
+                                                     float omb1, float beta2, float omb2, float eps, const float* __restrict__ ctrl) {
   if (reinterpret_cast<const int*>(ctrl)[2]) return;      // non-finite gradients: the step is skipped (GradScaler.step)
   const float gmul = ctrl[4], bc1 = ctrl[6], bc2s = ctrl[7];
   const int c = blockIdx.x;
@@ -100,8 +102,8 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const
   auto upd = [&](float& pp, float gg, float& mm, float& vv) {
     gg *= gmul;
     pp *= decay;
-    mm = mm + (gg - mm) * (1.f - beta1);
-    vv = vv * beta2 + (1.f - beta2) * (gg * gg);
+    mm = mm + (gg - mm) * omb1;
+    vv = vv * beta2 + omb2 * (gg * gg);
     pp -= step_size * (mm / (sqrtf(vv) / bc2s + eps));
   };
   for (int i = threadIdx.x; i < (len >> 2); i += blockDim.x) {
@@ -130,23 +132,23 @@ extern "C" int fb200_grad_stats(const float* grads, int64_t n, void* workspace, 
 }
 
 extern "C" int fb200_optim_finalize(const void* workspace, float* ctrl, float max_norm, int clip_passes, float inv_world, int use_scaler, float growth,
-                                    float backoff, int growth_interval, float beta1, float beta2, void* stream) {
+                                    float backoff, int growth_interval, float one_minus_beta1, float one_minus_beta2, void* stream) {
   FB_CHECK_ARG(workspace && ctrl && inv_world > 0.f && clip_passes >= 0, "optim_finalize: bad arguments");
   const double* partial = reinterpret_cast<const double*>(workspace);
   const int* flags = reinterpret_cast<const int*>(partial + STATS_BLOCKS);
   optim_finalize_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(partial, flags, STATS_BLOCKS, ctrl, max_norm, clip_passes, inv_world, use_scaler, growth, backoff,
-                                                            growth_interval, beta1, beta2);
+                                                            growth_interval, one_minus_beta1, one_minus_beta2);
   FB_CHECK_LAUNCH("optim_finalize");
   return FB200_OK;
 }
 
 extern "C" int fb200_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const int64_t* chunk_start, const int* chunk_len,
-                                const int* chunk_seg, int nchunks, const float* seg_lr, const float* seg_wd, const int* seg_active, float lr_factor, float beta1,
-                                float beta2, float eps, const float* ctrl, void* stream) {
+                                const int* chunk_seg, int nchunks, const float* seg_lr, const float* seg_wd, const int* seg_active, float lr_factor,
+                                float one_minus_beta1, float one_minus_beta2, float eps, const float* ctrl, void* stream) {
   FB_CHECK_ARG(params && grads && exp_avg && exp_avg_sq && chunk_start && chunk_len && chunk_seg && seg_lr && seg_wd && ctrl && nchunks > 0,
                "adamw_step: bad arguments");
   adamw_kernel<<<nchunks, 256, 0, (cudaStream_t)stream>>>(params, grads, exp_avg, exp_avg_sq, chunk_start, chunk_len, chunk_seg, seg_lr, seg_wd, seg_active, lr_factor,
-                                                          beta1, beta2, eps, ctrl);
+                                                          one_minus_beta1, 1.f - one_minus_beta2, one_minus_beta2, eps, ctrl);
   FB_CHECK_LAUNCH("adamw_step");
   return FB200_OK;
 }

@@ -603,12 +603,12 @@ class CudaBackend:
     def optim_finalize(self, ws, ctrl, max_norm, clip_passes, inv_world, use_scaler, growth, backoff, growth_interval, beta1, beta2):
         self._cuda(ws, ctrl)
         self._call("fb200_optim_finalize", _p(ws), _p(ctrl), max_norm, int(clip_passes), inv_world, int(use_scaler),
-                   growth, backoff, int(growth_interval), beta1, beta2, _stream())
+                   growth, backoff, int(growth_interval), 1.0 - beta1, 1.0 - beta2, _stream())   # 1 - beta in double, then fp32: torch's scalars
 
     def adamw_step(self, params, grads, m, v, chunk_start, chunk_len, chunk_seg, seg_lr, seg_wd, seg_active, lr_factor, beta1, beta2, eps, ctrl):
         self._cuda(params, grads, m, v, chunk_start, chunk_len, chunk_seg, seg_lr, seg_wd, ctrl)
         self._call("fb200_adamw_step", _p(params), _p(grads), _p(m), _p(v), _p(chunk_start), _p(chunk_len), _p(chunk_seg), chunk_len.shape[0], _p(seg_lr), _p(seg_wd), _p(seg_active),
-                   lr_factor, beta1, beta2, eps, _p(ctrl), _stream())
+                   lr_factor, 1.0 - beta1, 1.0 - beta2, eps, _p(ctrl), _stream())
 
 
 class Pair:

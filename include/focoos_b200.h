@@ -322,14 +322,17 @@ int fb200_detr_loss(const float* logits, const float* boxes, const int* tgt_labe
 int64_t fb200_optim_workspace_bytes(void);
 /* sum of squares + non-finite flag of the flat gradient buffer (per-block partials, reduced in a fixed order) */
 int fb200_grad_stats(const float* grads, int64_t n, void* workspace, void* stream);
-/* one thread: norm, `clip_passes` successive clip_grad_norm_(max_norm) coefficients, loss-scale update, bias corrections */
+/* one thread: norm, `clip_passes` successive clip_grad_norm_(max_norm) coefficients, loss-scale update, bias corrections 1 - beta^step with
+ * beta = 1 - one_minus_beta in double (fp32(0.001) puts 1 - beta2 within 5e-8 relative of torch's) */
 int fb200_optim_finalize(const void* workspace, float* ctrl, float max_norm, int clip_passes, float inv_world, int use_scaler, float growth,
-                         float backoff, int growth_interval, float beta1, float beta2, void* stream);
+                         float backoff, int growth_interval, float one_minus_beta1, float one_minus_beta2, void* stream);
 /* AdamW over chunks (chunk c covers [chunk_start[c], +chunk_len[c]) of tensor chunk_seg[c]; lr = seg_lr[seg]*lr_factor).
- * seg_active: NULL, or one int per tensor, 0 = the tensor received no gradient this step and is skipped (torch: p.grad is None). */
+ * seg_active: NULL, or one int per tensor, 0 = the tensor received no gradient this step and is skipped (torch: p.grad is None).
+ * The Adam betas arrive as 1 - beta, formed by the caller before the rounding to fp32 as torch forms its scalars: 1 - fp32(0.999) would be
+ * 1.3e-5 smaller than fp32(1 - 0.999).  fp32(1 - fp32(1 - beta)) rounds back to fp32(beta) for the betas in use (0.9, 0.999). */
 int fb200_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const int64_t* chunk_start, const int* chunk_len,
-                     const int* chunk_seg, int nchunks, const float* seg_lr, const float* seg_wd, const int* seg_active, float lr_factor, float beta1,
-                     float beta2, float eps, const float* ctrl, void* stream);
+                     const int* chunk_seg, int nchunks, const float* seg_lr, const float* seg_wd, const int* seg_active, float lr_factor,
+                     float one_minus_beta1, float one_minus_beta2, float eps, const float* ctrl, void* stream);
 
 /* ---- backward / training-mode kernels (SURVEY 8 a21: what autograd executes under TrainerLoop.run_step, trainer/trainer.py:757) ----
  * fp32, NHWC, caller-owned workspaces.  Each replaces the aten backward of the torch call the reference makes at the cited site. */
