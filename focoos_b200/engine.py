@@ -188,6 +188,33 @@ class Engine:
             return ops.linear_pair(ops.to_pair(x), lin.w3, lin.bias, act=act, residual=residual, out=out, out_pair=out_pair)
         return ops.linear(x, lin.w, lin.bias, act=act, residual=residual, out=out, out_dtype=out_dtype, algo=algo)
 
+    # ---- the row glue between two linears of the transformer layers: the one place that picks it from the precision --------------------------------------
+    # fp32_tc: the fused glue kernels (csrc/head_fused.cu) - LayerNorm, positional add, GELU - write the Pair operand of the next tensor-core linear
+    # themselves, so no separate split / add launch sits between two linears.  fp16 / fp32: ops.layernorm / ops.add in the storage dtype.
+    def _operand(self, x):
+        """x as a linear operand of the flow: its Pair under fp32_tc (one split launch), else x"""
+        return ops.to_pair(x) if self.pair else x
+
+    def _with_pos(self, x, pos, want_op=False):
+        """(x as an operand if want_op else None, x + pos as an operand); fp32_tc writes both in one launch"""
+        if self.pair:
+            return ops.split_pair_ex(x, pos=pos, want_pair=want_op, want_pair_pos=True)
+        return (x if want_op else None), ops.add(x, pos)
+
+    def _norm(self, y, ln, *, pos=None, want_f32=True, want_op=True):
+        """x = LayerNorm(y) with ln = (gamma, beta) -> (x, x as an operand, x + pos as an operand or None without pos); fp32_tc writes them in one launch.
+        want_f32 / want_op let fp32_tc skip an output no one reads (None in its place); the storage flow returns its one tensor in both places."""
+        if self.pair:
+            return ops.layernorm_ex(y, *ln, pos=pos, want_f32=want_f32, want_pair=want_op, want_pair_pos=pos is not None)
+        x = ops.layernorm(y, *ln)
+        return x, x, (None if pos is None else ops.add(x, pos))
+
+    def _mlp(self, layers, x, out_dtype=None):
+        """packed linears with ReLU between them; under fp32_tc the hidden activations stay Pairs"""
+        for lin in layers[:-1]:
+            x = self._linear(lin, x, act=ops.ACT_RELU, out_pair=True)
+        return self._linear(layers[-1], x, out_dtype=out_dtype)
+
     def _empty(self, shape, device):
         """an activation buffer of the flow: a Pair under fp32_tc, else a tensor in the storage dtype"""
         return ops.Pair.empty(shape, device) if self.pair else torch.empty(shape, dtype=self.dt, device=device)

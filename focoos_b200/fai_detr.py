@@ -169,8 +169,8 @@ class DetrEngine(Engine):
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)
         if self.pair:
-            # _forward_head_pair writes the class logits into rows padded to 16 bytes (the tensor-core store writes whole 16-byte pieces): zero rows up
-            # to that width make the launch own every column it stores
+            # the pair flow's score head (_forward_head) writes the class logits into rows padded to 16 bytes (the tensor-core store writes whole
+            # 16-byte pieces): zero rows up to that width make the launch own every column it stores
             self.dec_score = _pad_rows(self.dec_score, 4)
 
     def _pair_layers(self):
@@ -252,34 +252,19 @@ class DetrEngine(Engine):
                            out_pair=True)
         return x
 
-    def _mha(self, blk, x, pos):
-        """post-norm self-attention block: LN(x + out_proj(attn(q=k=x+pos, v=x)))."""
-        B, L, d = x.shape
-        qk = self._linear(blk["qk"], ops.add(x, pos))
-        v = self._linear(blk["v"], x)
-        a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, 1.0 / math.sqrt(d // self.nhead))
-        y = self._linear(blk["out"], a, residual=x)
-        return ops.layernorm(y, *blk["n_attn"])
-
-    def _ffn(self, blk, x, act):
-        f = self._linear(blk["l2"], self._linear(blk["l1"], x, act=act), residual=x)
-        return ops.layernorm(f, *blk["n_ffn"])
-
-    # fused row glue (csrc/head_fused.cu): LayerNorm / positional add / GELU / gather / mask kernels write the pair operand of the next tensor-core linear themselves
-    # (and attention / deformable attention write pair rows), so no split_f32_pair / add / row_select launch remains in the AIFI, selection and decoder chains
-    def _aifi_pair(self, src, pos):
-        """AIFI encoder layer (nn/layers/transformer.py:583-601, post-norm, GELU) on fp32 tokens [B,L,d] -> (fp32 tokens, their Pair)"""
+    def _aifi(self, src, pos):
+        """AIFI encoder layer (nn/layers/transformer.py:583-601, post-norm, GELU) on tokens [B,L,d] (fp32 under fp32_tc) -> (tokens, their operand)"""
         blk, d = self.aifi, src.shape[-1]
-        sp, spp = ops.split_pair_ex(src, pos=pos, want_pair=True, want_pair_pos=True)
+        sp, spp = self._with_pos(src, pos, want_op=True)
         qk = self._linear(blk["qk"], spp)
         v = self._linear(blk["v"], sp)
-        a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, 1.0 / math.sqrt(d // self.nhead), split=True, out_pair=True)
-        y = self._linear(blk["out"], a, residual=src)
-        x1, x1p, _ = ops.layernorm_ex(y, *blk["n_attn"])
-        h = self._linear(blk["l1"], x1p)
-        hp, _ = ops.split_pair_ex(h, act=ops.ACT_GELU)
-        y = self._linear(blk["l2"], hp, residual=x1)
-        x2, x2p, _ = ops.layernorm_ex(y, *blk["n_ffn"])
+        a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, 1.0 / math.sqrt(d // self.nhead), split=self.pair, out_pair=self.pair)
+        x1, x1p, _ = self._norm(self._linear(blk["out"], a, residual=src), blk["n_attn"])
+        if self.pair:  # no layer of the pair flow has a GELU epilogue: the split that writes linear2's operand applies it
+            h, _ = ops.split_pair_ex(self._linear(blk["l1"], x1p), act=ops.ACT_GELU)
+        else:
+            h = self._linear(blk["l1"], x1p, act=ops.ACT_GELU)
+        x2, x2p, _ = self._norm(self._linear(blk["l2"], h, residual=x1), blk["n_ffn"])
         return x2, x2p
 
     def _trunk(self, images, taps):
@@ -301,10 +286,7 @@ class DetrEngine(Engine):
         else:
             src = self._conv(self.enc_in[2], res5).reshape(B, h32 * w32, C)  # tokens for the AIFI block: fp32 in the pair flow (LayerNorm / attention work on fp32)
             # AIFI (modelling.py:315-324)
-            if self.pair:
-                src, src_p = self._aifi_pair(src, K["pos"])
-            else:
-                src = self._ffn(self.aifi, self._mha(self.aifi, src, K["pos"]), ops.ACT_GELU)
+            src, src_p = self._aifi(src, K["pos"])
             p5 = src.reshape(B, h32, w32, C)
             lat_in = ops.Pair(src_p.buf.reshape(B, h32, w32, 2 * C)) if self.pair else p5  # the pair flow's conv reads the pair its LayerNorm wrote
             if taps is not None:
@@ -347,98 +329,75 @@ class DetrEngine(Engine):
         value_all = self._linear(self.value_all, memory)  # [B,S,6*d], layer i uses columns [i*d,(i+1)*d)
         # query selection (modelling.py:1191-1232)
         t = self._linear(self.enc_output, memory)
-        head = self._forward_head_pair if self.pair else self._forward_head
-        return head(t, value_all, memory, shapes, K, B, memory.shape[1], taps)
+        return self._forward_head(t, value_all, memory, shapes, K, B, memory.shape[1], taps)
 
     def _forward_head(self, t, value_all, memory, shapes, K, B, S, taps):
-        """query selection + decoder + head on the encoder memory of the fp16 / fp32 flow (fp32_tc runs _forward_head_pair)"""
-        cfg, dt, A, d = self.cfg, self.dt, self.algo, self.d
-        dev = t.device
-        t = ops.row_select(t, K["valid"], self.enc_output.bias)
-        output_memory = ops.layernorm(t, *self.enc_output_ln)
-        ncls = cfg.num_classes
-        if self.precision == "fp16" and A == ops.ALGO_AUTO:
-            # only the per-anchor maximum is ever used in eval (modelling.py:1210-1214): the [B,S,365] fp32 logits (395 MB at bs=32) are never materialised
-            scores = ops.linear_rowmax(output_memory, self.enc_score.w, self.enc_score.bias)
-        else:
-            cls_buf = torch.empty((B, S, (ncls + 7) // 8 * 8), dtype=torch.float32, device=dev)
-            self._linear(self.enc_score, output_memory, out=cls_buf[..., :ncls])
-            scores = ops.rowmax(cls_buf[..., :ncls])
-        _, topk_ind = ops.topk(scores, cfg.num_queries)
-        tgt = ops.gather_rows(output_memory, topk_ind)
-        bb = self._linear(self.enc_bbox[2], self._linear(self.enc_bbox[1], self._linear(self.enc_bbox[0], tgt, act=ops.ACT_RELU), act=ops.ACT_RELU),
-                          out_dtype=torch.float32)
-        ref_unact = ops.box_add_anchors(bb, K["anchors"], topk_ind)
-        ref = ops.box_sigmoid(ref_unact)
-        if taps is not None:
-            taps.update(memory=memory, enc_scores=scores, topk_ind=topk_ind, target=tgt, ref_unact=ref_unact)
-        # decoder (modelling.py:969-1020, eval: logits only from the last layer)
-        for i, blk in enumerate(self.dec):
-            pos = self._linear(self.qpos[1], self._linear(self.qpos[0], ref, act=ops.ACT_RELU, out_dtype=dt, algo=ops.ALGO_SIMT))
-            tgt = self._mha(blk, tgt, pos)
-            oa = self._linear(blk["oa"], ops.add(tgt, pos), out_dtype=torch.float32)
-            c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, NUM_POINTS, self.nhead, out_dtype=dt)
-            tgt = ops.layernorm(self._linear(blk["cross_out"], c, residual=tgt), *blk["n_cross"])
-            tgt = self._ffn(blk, tgt, ops.ACT_RELU)
-            bbox = blk["bbox"]
-            delta = self._linear(bbox[2], self._linear(bbox[1], self._linear(bbox[0], tgt, act=ops.ACT_RELU), act=ops.ACT_RELU), out_dtype=torch.float32)
-            ref = ops.box_refine(delta, ref)
-            if taps is not None:
-                taps[f"dec{i}_out"] = tgt
-                taps[f"dec{i}_ref"] = ref
-        logits = self._linear(self.dec_score, tgt, out_dtype=torch.float32, algo=ops.ALGO_SIMT)  # [B,Q,C] contiguous
-        if taps is not None:
-            taps.update(pred_logits=logits, pred_boxes_cxcywh=ref)
-        return ops.box_sigmoid(logits), ops.box_cxcywh_to_xyxy(ref)
-
-    def _forward_head_pair(self, t, value_all, memory, shapes, K, B, S, taps):
-        """query selection + decoder + head of the fp32-accurate mode with the fused row glue: the same operators and arithmetic as _forward_head, ~18 launches per
-        decoder layer instead of 31.  t = enc_output.0(memory) BEFORE the valid-mask fill (modelling.py:1202-1207); memory: the Pair."""
+        """query selection + decoder + head on the encoder memory (a Pair under fp32_tc).  t = enc_output.0(memory) BEFORE the valid-mask fill
+        (modelling.py:1202-1207)."""
         cfg, d = self.cfg, self.d
         nq, ncls = cfg.num_queries, cfg.num_classes
         ln_w, ln_b = self.enc_output_ln
-        # output_memory = LayerNorm(where(valid, t, bias)) only ever feeds the score head (as a pair) and the 300 gathered rows (recomputed below from t: same arithmetic)
-        _, om_pair, _ = ops.layernorm_ex(t, ln_w, ln_b, valid=K["valid"], fill=self.enc_output.bias, want_f32=False)
-        scores = ops.linear_rowmax_pair(om_pair, self.enc_score.w3, self.enc_score.bias)
-        _, topk_ind = ops.topk(scores, nq)
-        tgt, tgt_p, _ = ops.layernorm_ex(t, ln_w, ln_b, gather=topk_ind, valid=K["valid"], fill=self.enc_output.bias)
-        h = self._linear(self.enc_bbox[1], self._linear(self.enc_bbox[0], tgt_p, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True)
-        bb = self._linear(self.enc_bbox[2], h)
-        ref_unact = ops.box_add_anchors(bb, K["anchors"], topk_ind)
+        if self.pair:
+            # output_memory = LayerNorm(where(valid, t, bias)) only ever feeds the score head (as a pair) and the gathered rows (recomputed from t:
+            # same arithmetic)
+            _, om_pair, _ = ops.layernorm_ex(t, ln_w, ln_b, valid=K["valid"], fill=self.enc_output.bias, want_f32=False)
+            scores = ops.linear_rowmax_pair(om_pair, self.enc_score.w3, self.enc_score.bias)
+            _, topk_ind = ops.topk(scores, nq)
+            tgt, tgt_op, _ = ops.layernorm_ex(t, ln_w, ln_b, gather=topk_ind, valid=K["valid"], fill=self.enc_output.bias)
+        else:
+            output_memory = ops.layernorm(ops.row_select(t, K["valid"], self.enc_output.bias), ln_w, ln_b)
+            if self.precision == "fp16" and self.algo == ops.ALGO_AUTO:
+                # only the per-anchor maximum is ever used in eval (modelling.py:1210-1214): the [B,S,365] fp32 logits (395 MB at bs=32) are never materialised
+                scores = ops.linear_rowmax(output_memory, self.enc_score.w, self.enc_score.bias)
+            else:
+                cls_buf = torch.empty((B, S, (ncls + 7) // 8 * 8), dtype=torch.float32, device=t.device)
+                self._linear(self.enc_score, output_memory, out=cls_buf[..., :ncls])
+                scores = ops.rowmax(cls_buf[..., :ncls])
+            _, topk_ind = ops.topk(scores, nq)
+            tgt = tgt_op = ops.gather_rows(output_memory, topk_ind)
+        ref_unact = ops.box_add_anchors(self._mlp(self.enc_bbox, tgt_op, out_dtype=torch.float32), K["anchors"], topk_ind)
         ref = ops.box_sigmoid(ref_unact)
         if taps is not None:
-            taps.update(memory=memory.float(), enc_scores=scores, topk_ind=topk_ind, target=tgt, ref_unact=ref_unact)
-        q0w, q0b = self.qpos[0].w, self.qpos[0].bias   # query_pos_head layer 0: fp32 [2d, 4]
-        _, qp = ops.box_refine_qpos(None, ref, q0w, q0b)
+            taps.update(memory=_unpair(memory), enc_scores=scores, topk_ind=topk_ind, target=tgt, ref_unact=ref_unact)
+        _, qp = self._refine(None, ref, False)
         scale = 1.0 / math.sqrt(d // self.nhead)
         L = len(self.dec)
+        # decoder (modelling.py:969-1020, eval: logits only from the last layer)
         for i, blk in enumerate(self.dec):
             pos = self._linear(self.qpos[1], qp)
-            _, tpp = ops.split_pair_ex(tgt, pos=pos, want_pair=False, want_pair_pos=True)
+            _, tpp = self._with_pos(tgt, pos)
             qk = self._linear(blk["qk"], tpp)
-            v = self._linear(blk["v"], tgt_p)
-            a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, scale, split=True, out_pair=True)
-            y = self._linear(blk["out"], a, residual=tgt)
-            tgt, _, tpp = ops.layernorm_ex(y, *blk["n_attn"], pos=pos, want_pair=False, want_pair_pos=True)
-            oa = self._linear(blk["oa"], tpp)
-            c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, NUM_POINTS, self.nhead, out_pair=True)
-            y = self._linear(blk["cross_out"], c, residual=tgt)
-            tgt, tgt_p, _ = ops.layernorm_ex(y, *blk["n_cross"])
-            y = self._linear(blk["l2"], self._linear(blk["l1"], tgt_p, act=ops.ACT_RELU, out_pair=True), residual=tgt)
-            tgt, tgt_p, _ = ops.layernorm_ex(y, *blk["n_ffn"])
-            h = self._linear(blk["bbox"][1], self._linear(blk["bbox"][0], tgt_p, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True)
-            delta = self._linear(blk["bbox"][2], h)
-            last = i == L - 1
-            ref, qp = ops.box_refine_qpos(delta, ref, None if last else q0w, None if last else q0b)
+            v = self._linear(blk["v"], tgt_op)
+            a = ops.attention(qk[..., :d], qk[..., d:], v, self.nhead, scale, split=self.pair, out_pair=self.pair)
+            tgt, _, tpp = self._norm(self._linear(blk["out"], a, residual=tgt), blk["n_attn"], pos=pos, want_op=False)
+            oa = self._linear(blk["oa"], tpp, out_dtype=torch.float32)
+            c = ops.msda(value_all[..., i * d:(i + 1) * d], oa, ref, shapes, NUM_POINTS, self.nhead, out_dtype=self.dt, out_pair=self.pair)
+            tgt, tgt_op, _ = self._norm(self._linear(blk["cross_out"], c, residual=tgt), blk["n_cross"])
+            y = self._linear(blk["l2"], self._linear(blk["l1"], tgt_op, act=ops.ACT_RELU, out_pair=True), residual=tgt)
+            tgt, tgt_op, _ = self._norm(y, blk["n_ffn"])
+            ref, qp = self._refine(self._mlp(blk["bbox"], tgt_op, out_dtype=torch.float32), ref, i == L - 1)
             if taps is not None:
                 taps[f"dec{i}_out"] = tgt
                 taps[f"dec{i}_ref"] = ref
-        # class logits on the tensor cores into a 16-byte-padded row (TMA store pitch), then sigmoid into the dense [B,Q,C] scores
-        lbuf = torch.empty((B, nq, self.dec_score.w.shape[0]), dtype=torch.float32, device=t.device)  # (ncls + 3) // 4 * 4 rows of the padded head
-        logits = self._linear(self.dec_score, tgt_p, out=lbuf)[..., :ncls]
+        if self.pair:
+            # class logits on the tensor cores into a 16-byte-padded row (TMA store pitch), then sigmoid into the dense [B,Q,C] scores
+            lbuf = torch.empty((B, nq, self.dec_score.w.shape[0]), dtype=torch.float32, device=t.device)  # (ncls + 3) // 4 * 4 rows of the padded head
+            logits = self._linear(self.dec_score, tgt_op, out=lbuf)[..., :ncls]
+            scores = ops.sigmoid_rows(logits)
+        else:
+            logits = self._linear(self.dec_score, tgt, out_dtype=torch.float32, algo=ops.ALGO_SIMT)  # [B,Q,C] contiguous
+            scores = ops.box_sigmoid(logits)
         if taps is not None:
             taps.update(pred_logits=logits, pred_boxes_cxcywh=ref)
-        return ops.sigmoid_rows(logits), ops.box_cxcywh_to_xyxy(ref)
+        return scores, ops.box_cxcywh_to_xyxy(ref)
+
+    def _refine(self, delta, ref, last):
+        """(ref refined by delta, or ref itself for delta None; query_pos_head.layers.0 on those boxes, None when last).  fp32_tc writes both in one
+        launch, the second as the Pair operand of query_pos_head.layers.1; fp16 / fp32 run the layer on the CUDA cores (K = 4)."""
+        if self.pair:
+            return ops.box_refine_qpos(delta, ref, None if last else self.qpos[0].w, None if last else self.qpos[0].bias)
+        ref = ref if delta is None else ops.box_refine(delta, ref)
+        return ref, None if last else self._linear(self.qpos[0], ref, act=ops.ACT_RELU, out_dtype=self.dt, algo=ops.ALGO_SIMT)
 
 
 class FAIDetr(_EngineModel):

@@ -272,13 +272,9 @@ class MFEngine(Engine):
         mask_features: a Pair under fp32_tc (see _run_decoder)."""
         A, dt = self.algo, self.dt
         B, Q, d = out.shape
-        if self.pair:  # LayerNorm writes the pair operand of the mask MLP, whose hidden layers stay in the pair format
-            dn, dnp, _ = ops.layernorm_ex(out, *self.head_norm, want_f32=want_class)
-        else:
-            dn = dnp = ops.layernorm(out, *self.head_norm)
+        dn, dnp, _ = self._norm(out, self.head_norm, want_f32=want_class)
         cls = self._linear(self.classifier, dn, out_dtype=torch.float32, algo=ops.ALGO_SIMT) if want_class else None
-        mlp = self.mask_mlp
-        me = self._linear(mlp[2], self._linear(mlp[1], self._linear(mlp[0], dnp, act=ops.ACT_RELU, out_pair=True), act=ops.ACT_RELU, out_pair=True))  # [B,Q,256]
+        me = self._mlp(self.mask_mlp, dnp)  # [B,Q,256]
         _, h4, w4, C = mask_features.shape
         Qp = (Q + 7) // 8 * 8
         masks = torch.zeros((B, h4, w4, Qp), dtype=dt, device=out.device)
@@ -363,36 +359,21 @@ class MFEngine(Engine):
         qpos = self.query_embed
         L = len(self.dec)
         cls = None
-        if self.pair:
-            # masked cross-attention on the tensor cores (fb200_attention_masked_split): the per-level key / value inputs are split ONCE (they are the same for
-            # the layers of a level) and the K / V projections run pair -> pair.  Fused row glue (csrc/head_fused.cu, the kernels of the fai-detr head): every
-            # LayerNorm writes the pair operand(s) of the linears behind it - LN(x) and LN(x) + query_pos in one launch - and the FFN / mask-MLP hidden layers
-            # stay in the pair format: no add / split launches between two tensor-core linears
-            kpos_p, srcs_p = [ops.to_pair(t) for t in kpos], [ops.to_pair(t) for t in srcs]
+        # fp32_tc: the per-level key / value inputs are split once (every layer of a level reads the same ones), the K / V projections run pair -> pair
+        kpos, srcs = [self._operand(t) for t in kpos], [self._operand(t) for t in srcs]
         _, masks, attn = self._heads(out, mask_features, sizes[0], False)
         for i, blk in enumerate(self.dec):
             lvl = i % nl
-            if self.pair:
-                _, _, tq = ops.layernorm_ex(out, *blk["cn"], pos=qpos, want_f32=False, want_pair=False, want_pair_pos=True)
-                q = self._linear(blk["cq"], tq)
-                kk, vv = self._linear(blk["ck"], kpos_p[lvl], out_pair=True), self._linear(blk["cv"], srcs_p[lvl], out_pair=True)
-                a = ops.attention_masked(q, kk, vv, attn[0], attn[1], nh, scale, split=True)
-                out = self._linear(blk["cout"], ops.to_pair(a), residual=out)
-                _, t2p, t2pp = ops.layernorm_ex(out, *blk["sn"], pos=qpos, want_f32=False, want_pair=True, want_pair_pos=True)
-                qk = self._linear(blk["sqk"], t2pp)
-                a = ops.attention(qk[..., :d], qk[..., d:], self._linear(blk["sv"], t2p), nh, scale, split=True, out_pair=True)
-                out = self._linear(blk["sout"], a, residual=out)
-                _, ffn_in, _ = ops.layernorm_ex(out, *blk["fn"], want_f32=False)
-            else:
-                t2 = ops.layernorm(out, *blk["cn"])
-                q = self._linear(blk["cq"], ops.add(t2, qpos))
-                a = ops.attention_masked(q, self._linear(blk["ck"], kpos[lvl]), self._linear(blk["cv"], srcs[lvl]), attn[0], attn[1], nh, scale)
-                out = self._linear(blk["cout"], a, residual=out)
-                t2 = ops.layernorm(out, *blk["sn"])
-                qk = self._linear(blk["sqk"], ops.add(t2, qpos))
-                a = ops.attention(qk[..., :d], qk[..., d:], self._linear(blk["sv"], t2), nh, scale)
-                out = self._linear(blk["sout"], a, residual=out)
-                ffn_in = ops.layernorm(out, *blk["fn"])
+            _, _, tq = self._norm(out, blk["cn"], pos=qpos, want_f32=False, want_op=False)
+            q = self._linear(blk["cq"], tq)
+            kk, vv = self._linear(blk["ck"], kpos[lvl], out_pair=True), self._linear(blk["cv"], srcs[lvl], out_pair=True)
+            a = ops.attention_masked(q, kk, vv, attn[0], attn[1], nh, scale, split=self.pair)
+            out = self._linear(blk["cout"], self._operand(a), residual=out)
+            _, t2, t2p = self._norm(out, blk["sn"], pos=qpos, want_f32=False)
+            qk = self._linear(blk["sqk"], t2p)
+            a = ops.attention(qk[..., :d], qk[..., d:], self._linear(blk["sv"], t2), nh, scale, split=self.pair, out_pair=self.pair)
+            out = self._linear(blk["sout"], a, residual=out)
+            _, ffn_in, _ = self._norm(out, blk["fn"], want_f32=False)
             out = self._linear(blk["l2"], self._linear(blk["l1"], ffn_in, act=ops.ACT_RELU, out_pair=True), residual=out)
             last = i == L - 1
             cls, masks, attn = self._heads(out, mask_features, None if last else sizes[(i + 1) % nl], last)

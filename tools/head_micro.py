@@ -62,7 +62,7 @@ with torch.no_grad():
         mem, shapes, K = state["mem"], state["shapes"], state["K"]
         value_all = eng._linear(eng.value_all, mem)
         t = eng._linear(eng.enc_output, mem)
-        return eng._forward_head_pair(t, value_all, mem, shapes, K, B, mem.shape[1], None)
+        return eng._forward_head(t, value_all, mem, shapes, K, B, mem.shape[1], None)
 
     l0 = ops.launch_count()
     trunk()
