@@ -252,7 +252,8 @@ class FocoosModel:
         return run_train_entry(self, args, data_train, data_val)
 
     def eval(self, args, data_test, save_json: bool = True):
-        """focoos_model.py:276-310: `inference_on_dataset` with `processor.eval_postprocess` and the detection evaluator; returns the metrics dict."""
+        """focoos_model.py:276-310: `inference_on_dataset` with `processor.eval_postprocess` and the processor's evaluator (box AP for fai-detr, mIoU for semantic
+        segmenters); returns the metrics dict."""
         from .trainer import run_eval_entry
         return run_eval_entry(self, args, data_test, save_json)
 

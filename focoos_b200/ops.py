@@ -400,6 +400,24 @@ class CudaBackend:
         _, h, w, Qp = x.shape
         self._call("fb200_mask_sigmoid_upsample_select", _p(x), _dt(x), h, w, Qp, _p(bq), bq.shape[0], _p(out), out.shape[1], out.shape[2], _stream())
 
+    # ---- semantic evaluation (processor.MaskFormerProcessor.eval_postprocess, trainer.SemSegEvaluator) ----------------------------------------------
+    # Not among the per-operator methods the CPU reference backend mirrors: their CPU restatement is oracle/sem_seg_ref.py (SemSegRefBackend, a RefBackend
+    # with these two methods), which the tests install to run the evaluation's host logic without a GPU.
+    def _mask_sigmoid_upsample_nhwc(self, x, Q, out):
+        """out: fp32 / fp16 [B,H,W,Qo], or a Pair [B,H,W,Qo]"""
+        buf = out.buf if isinstance(out, Pair) else out
+        self._cuda(x, buf)
+        B, h, w, Qp = x.shape
+        _, H, W, Qo = out.shape
+        self._call("fb200_mask_sigmoid_upsample_nhwc", _p(x), _dt(x), B, h, w, Qp, Q, _p(buf), F16PAIR if isinstance(out, Pair) else _dt(out), Qo, H, W, _stream())
+
+    def _sem_seg_confusion(self, scores, labels, C, ignore_label, conf, invalid):
+        self._cuda(scores, labels, conf, invalid)
+        B, H, W, _ = scores.shape
+        pitch = _pitch(scores, True)
+        self._call("fb200_sem_seg_confusion", _p(scores), B, H, W, C, pitch, scores.stride(0) if B > 1 else H * W * pitch, _p(labels), labels.element_size(),
+                   ignore_label, _p(conf), _p(invalid), _stream())
+
     def mask_stats(self, masks, thr, count, psum):
         self._cuda(masks, count, psum)
         B, Q, H, W = masks.shape
@@ -1148,6 +1166,30 @@ def mask_sigmoid_upsample_select(mask_logits_nhwc, bq_i32, size):
     if n:
         _be().mask_sigmoid_upsample_select(mask_logits_nhwc.contiguous(), bq_i32.contiguous(), out)
     return out
+
+
+def mask_sigmoid_upsample_nhwc(mask_logits_nhwc, num_queries: int, size, channels: int, fmt: str = "fp32"):
+    """[B,h,w,Qp] logits -> the probabilities of mask_sigmoid_upsample in NHWC [B,H,W,channels] (channels >= num_queries, the ones past it zero), as
+    fmt "fp32" / "fp16" tensors or a "pair" (Pair): the activation operand of the per-image class x mask product."""
+    B = mask_logits_nhwc.shape[0]
+    shape = (B, int(size[0]), int(size[1]), int(channels))
+    if fmt == "pair":
+        out = Pair.empty(shape, mask_logits_nhwc.device)
+    else:
+        out = torch.empty(shape, dtype=torch.float16 if fmt == "fp16" else torch.float32, device=mask_logits_nhwc.device)
+    _be()._mask_sigmoid_upsample_nhwc(mask_logits_nhwc.contiguous(), num_queries, out)
+    return out
+
+
+def sem_seg_confusion(scores, labels, num_classes: int, ignore_label: int, conf, invalid):
+    """conf[(C+1) * argmax_c(scores) + gt] += 1 over every pixel (the first maximum over c < C wins, a NaN is the maximum; gt = C where labels == ignore_label):
+    scores fp32 NHWC [B,H,W,>=C] (a channel slice of a wider buffer is fine), labels uint8 / int32 [B,H,W], conf int64 [(C+1),(C+1)] and invalid int64 [1]
+    (pixels whose label is neither in [0, C] nor ignore_label) on the device, both added into."""
+    assert scores.dtype == torch.float32 and scores.dim() == 4 and scores.shape[-1] >= num_classes, (scores.dtype, tuple(scores.shape))
+    assert labels.dtype in (torch.uint8, torch.int32) and tuple(labels.shape) == tuple(scores.shape[:3]), (labels.dtype, tuple(labels.shape))
+    assert conf.dtype == torch.int64 and tuple(conf.shape) == (num_classes + 1, num_classes + 1) and conf.is_contiguous()
+    assert invalid.dtype == torch.int64 and invalid.numel() == 1
+    _be()._sem_seg_confusion(scores, labels.contiguous(), int(num_classes), int(ignore_label), conf, invalid)
 
 
 def mask_stats(masks, thr: float):

@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .engine import _split3_weights
 from .ports import Boxes, DETRConfig, DETRModelOutput, FocoosDet, FocoosDetections, Instances
 
 
@@ -217,6 +218,13 @@ def base64_to_binary_mask(b64: str) -> np.ndarray:
     return np.array(Image.open(io.BytesIO(base64.b64decode(b64)))) > 0
 
 
+_SEM_FMT = {"fp32": "fp32", "fp16": "fp16", "fp32_tc": "pair"}  # model precision -> operand format of the class x mask product
+
+
+def _entry_get(e, name):
+    return e[name] if isinstance(e, dict) else getattr(e, name)
+
+
 class MaskFormerProcessor(DETRProcessor):
     """preprocess as the base Processor; postprocess = the reference's tensor pipeline as GPU reductions + one compaction:
     per (image, query): pixel count and probability mass of `prob >= mask_threshold` (ONE pass over the [B,Q,H,W] tensor),
@@ -230,6 +238,46 @@ class MaskFormerProcessor(DETRProcessor):
         self.top_k, self.threshold = config.top_k, config.threshold
         self.mask_threshold, self.use_mask_score, self.predict_all_pixels = config.mask_threshold, config.use_mask_score, config.predict_all_pixels
         self.training = False
+
+    def eval_postprocess(self, output, batched_inputs, top_k: Optional[int] = None, precision: str = "fp32"):
+        """fai_mf/processor.py:142-166 for semantic configs (BisenetFormer's processor is the same): per image the mask probabilities at the entry's
+        (height, width) and sem_seg = einsum("qc,qhw->chw", logits, probs) (semantic_inference, :99-105) -> [{"sem_seg": [C,height,width] fp32}].
+        `output.masks` must be the model's LazyMasks (`lazy_masks = True`).  Per run of entries with the same (height, width), three launches and no
+        torch arithmetic: the NHWC probabilities [g,height,width,Qk] (mask_sigmoid_upsample_nhwc, then resize_bilinear when (height, width) is not the
+        input size), and the product as a 1x1 conv with per-image weights W_b = logits[b]^T (C padded to Cp, Q to Qk with zeros) writing NHWC scores
+        [g,height,width,Cp].  Each "sem_seg" is a [C,H,W] view of that buffer (a permute, channels >= C sliced off).  The reference's crop to the
+        augmented size is a no-op here: the masks are at the input size, so its output stride is 1.  The product's arithmetic follows `precision`:
+        CUDA-core fp32 ("fp32"), three fp16 tensor-core products on the [hi | lo] pair ("fp32_tc"), one fp16 product with fp32 accumulation ("fp16")."""
+        if self.config.postprocessing_type != "semantic":
+            raise NotImplementedError("focoos_b200: evaluation of instance-segmentation models (mask AP) is not built; only semantic configs can be evaluated")
+        if precision not in _SEM_FMT:
+            raise ValueError(f"precision must be one of {sorted(_SEM_FMT)} (got {precision!r})")
+        lazy = output.masks
+        if not hasattr(lazy, "materialize"):
+            raise TypeError("MaskFormerProcessor.eval_postprocess reads the low-resolution mask logits: run the model with `lazy_masks = True`")
+        logits = output.logits
+        B, Q, C = logits.shape
+        assert len(batched_inputs) == B, (len(batched_inputs), B)
+        fmt = _SEM_FMT[precision]
+        Qk, Cp = -(-Q // 32) * 32, -(-C // 8) * 8  # the tensor-core product takes channels in 32-wide chunks; fp32 rows of 8 channels are 32-byte aligned
+        w = torch.zeros((B, Cp, Qk), dtype=torch.float32, device=logits.device)
+        w[:, :C, :Q] = logits.transpose(1, 2)
+        w = _split3_weights(w) if fmt == "pair" else w.to(torch.float16 if fmt == "fp16" else torch.float32)
+        w = w.reshape(B, Cp, 1, 1, w.shape[-1])
+        sizes = [(int(_entry_get(e, "height")), int(_entry_get(e, "width"))) for e in batched_inputs]
+        results = []
+        i = 0
+        while i < B:
+            j = i + 1
+            while j < B and sizes[j] == sizes[i]:
+                j += 1
+            probs = ops.mask_sigmoid_upsample_nhwc(lazy.logits[i:j], Q, lazy.size, Qk, fmt)
+            if sizes[i] != tuple(lazy.size):  # interpolate_image(mask, (height, width))
+                probs = ops.resize_bilinear(probs, sizes[i])
+            scores = ops.conv2d_per_image(probs, w[i:j], out_dtype=torch.float32)
+            results += [{"sem_seg": scores[k, ..., :C].permute(2, 0, 1)} for k in range(j - i)]
+            i = j
+        return results
 
     def export_postprocess(self, output, inputs, class_names=(), top_k=None, threshold: float = 0.5):
         """fai_mf/processor.py:308-337: output = (masks, logits) of an exported graph."""

@@ -262,11 +262,16 @@ class BoxAPEvaluator:
 
 
 @torch.no_grad()
-def inference_on_dataset(fm, dataset, batch_size: int = 16, evaluator: Optional[BoxAPEvaluator] = None, top_k: Optional[int] = None):
+def inference_on_dataset(fm, dataset, batch_size: int = 16, evaluator=None, top_k: Optional[int] = None):
     """evaluator.py:115-238: run the model over `dataset` in batches (the reference uses batch 1 per GPU), `processor.eval_postprocess`, `evaluator.process`;
-    each rank takes a contiguous shard and rank 0 evaluates its own (single-process evaluation is the tested path)."""
+    each rank takes a contiguous shard and rank 0 evaluates its own (single-process evaluation is the tested path).  The evaluator follows the processor:
+    BoxAPEvaluator for DETRProcessor, SemSegEvaluator for MaskFormerProcessor, whose batches hold consecutive entries of one image size and run the model
+    with `lazy_masks = True` (as FocoosModel.__call__ does)."""
+    from .processor import MaskFormerProcessor
     model, proc = fm.model, fm.processor
     model.eval()
+    if isinstance(proc, MaskFormerProcessor):
+        return _sem_seg_inference(fm, dataset, batch_size, evaluator)
     evaluator = evaluator or BoxAPEvaluator(model.config.num_classes)
     evaluator.reset()
     lo, hi = D.shard_range(len(dataset))
@@ -275,6 +280,34 @@ def inference_on_dataset(fm, dataset, batch_size: int = 16, evaluator: Optional[
         x = torch.stack([torch.as_tensor(_get(e, "image")) for e in entries]).to(model.device).float()
         out = model(x)
         evaluator.process(entries, proc.eval_postprocess(out, entries, top_k))
+    return evaluator.evaluate()
+
+
+def _sem_seg_inference(fm, dataset, batch_size, evaluator):
+    model, proc = fm.model, fm.processor
+    if evaluator is None:
+        meta = getattr(dataset, "metadata", None)
+        ignore = getattr(meta, "ignore_label", None)
+        evaluator = SemSegEvaluator(model.config.num_classes, fm.model_info.classes, 255 if ignore is None else int(ignore))
+    evaluator.reset()
+    lo, hi = D.shard_range(len(dataset))
+    s = lo
+    while s < hi:
+        entries = [dataset[s]]
+        shape = tuple(torch.as_tensor(_get(entries[0], "image")).shape)
+        while s + len(entries) < hi and len(entries) < batch_size:
+            e = dataset[s + len(entries)]
+            if tuple(torch.as_tensor(_get(e, "image")).shape) != shape:
+                break
+            entries.append(e)
+        s += len(entries)
+        x = torch.stack([torch.as_tensor(_get(e, "image")) for e in entries]).to(model.device).float()
+        model.lazy_masks = True
+        try:
+            out = fm._forward(x)
+        finally:
+            model.lazy_masks = False
+        evaluator.process(entries, proc.eval_postprocess(out, entries, precision=model.precision))
     return evaluator.evaluate()
 
 
@@ -288,6 +321,83 @@ def run_eval_entry(fm, args: TrainerArgs, data_test, save_json: bool = True):
         with open(os.path.join(out_dir, "eval_metrics.json"), "w") as f:
             json.dump(metrics, f, indent=1)
     return metrics
+
+
+def _sem_seg_gt(e) -> np.ndarray:
+    """the entry's ground-truth label map [H,W]: `sem_seg` (array / tensor), or `sem_seg_file_name` read as load_image_into_numpy_array does
+    (sem_seg_evaluation.py:28-34)"""
+    if (isinstance(e, dict) and e.get("sem_seg") is not None) or getattr(e, "sem_seg", None) is not None:
+        gt = _get(e, "sem_seg")
+        return gt.cpu().numpy() if torch.is_tensor(gt) else np.asarray(gt)
+    from PIL import Image
+    with open(_get(e, "sem_seg_file_name"), "rb") as f:
+        return np.array(Image.open(f))
+
+
+class SemSegEvaluator:
+    """SemSegEvaluator of trainer/evaluation/sem_seg_evaluation.py:37-163 with the reset / process / evaluate shape of BoxAPEvaluator.  `process` adds
+    every image into a (C+1) x (C+1) int64 confusion matrix (row = predicted class, column = ground truth, ignore_label -> C) with one kernel launch
+    (ops.sem_seg_confusion: argmax over the classes folded into the histogram); the matrix stays on the device until `evaluate`, which is the
+    reference's numpy arithmetic -> {"sem_seg": {mIoU, fwIoU, IoU-<class>, mACC, pACC, ACC-<class>}}, non-finite values as None.  Class names are
+    `class_names` when it names every class, the class indices otherwise."""
+
+    def __init__(self, num_classes: int, class_names: Sequence[str] = (), ignore_label: int = 255):
+        self.num_classes, self.ignore_label = num_classes, ignore_label
+        self.class_names = list(class_names) if len(class_names) == num_classes else [str(i) for i in range(num_classes)]
+        self.reset()
+
+    def reset(self):
+        self._conf = self._invalid = None  # allocated on the device of the first prediction
+
+    def process(self, inputs, outputs):
+        C = self.num_classes
+        for e, o in zip(inputs, outputs):
+            hwc = o["sem_seg"].permute(1, 2, 0)  # the NHWC score buffer eval_postprocess wrote
+            if hwc.stride(-1) != 1:  # a [C,H,W] tensor that is not such a view
+                hwc = hwc.contiguous()
+            gt = _sem_seg_gt(e)
+            assert gt.shape == tuple(hwc.shape[:2]), f"ground truth {gt.shape} vs prediction {tuple(hwc.shape[:2])}"
+            if gt.dtype != np.uint8:  # int32 for the kernel; values beyond it stay out of [0, C] and are reported by evaluate()
+                gt = np.clip(gt.astype(np.int64), -1, np.iinfo(np.int32).max).astype(np.int32)
+            if self._conf is None:
+                self._conf = torch.zeros((C + 1, C + 1), dtype=torch.int64, device=hwc.device)
+                self._invalid = torch.zeros((1,), dtype=torch.int64, device=hwc.device)
+            ops.sem_seg_confusion(hwc.unsqueeze(0), torch.from_numpy(np.ascontiguousarray(gt)).to(hwc.device, non_blocking=True).unsqueeze(0), C,
+                                  self.ignore_label, self._conf, self._invalid)
+
+    def confusion_matrix(self) -> np.ndarray:
+        C = self.num_classes
+        return np.zeros((C + 1, C + 1), dtype=np.int64) if self._conf is None else self._conf.cpu().numpy()
+
+    def evaluate(self):
+        if self._invalid is not None and int(self._invalid.item()):
+            raise ValueError(f"{int(self._invalid.item())} ground-truth pixels are neither in [0, {self.num_classes}] nor ignore_label={self.ignore_label}")
+        conf = self.confusion_matrix()
+        n = self.num_classes
+        acc = np.full(n, np.nan, dtype=float)
+        iou = np.full(n, np.nan, dtype=float)
+        tp = conf.diagonal()[:-1].astype(float)
+        pos_gt = np.sum(conf[:-1, :-1], axis=0).astype(float)
+        with np.errstate(divide="ignore", invalid="ignore"):  # an empty matrix gives NaN metrics (None), as in the reference
+            class_weights = pos_gt / np.sum(pos_gt)
+            pos_pred = np.sum(conf[:-1, :-1], axis=1).astype(float)
+            acc_valid = pos_gt > 0
+            acc[acc_valid] = tp[acc_valid] / pos_gt[acc_valid]
+            union = pos_gt + pos_pred - tp
+            iou_valid = np.logical_and(acc_valid, union > 0)
+            iou[iou_valid] = tp[iou_valid] / union[iou_valid]
+            macc = np.sum(acc[acc_valid]) / np.sum(acc_valid)
+            miou = np.sum(iou[iou_valid]) / np.sum(iou_valid)
+            fiou = np.sum(iou[iou_valid] * class_weights[iou_valid])
+            pacc = np.sum(tp) / np.sum(pos_gt)
+        res = {"mIoU": 100 * miou, "fwIoU": 100 * fiou}
+        for i, name in enumerate(self.class_names):
+            res[f"IoU-{name}"] = 100 * iou[i]
+        res["mACC"] = 100 * macc
+        res["pACC"] = 100 * pacc
+        for i, name in enumerate(self.class_names):
+            res[f"ACC-{name}"] = 100 * acc[i]
+        return {"sem_seg": {k: (float(v) if np.isfinite(v) else None) for k, v in res.items()}}
 
 
 class SyntheticDetectionDataset:
@@ -308,3 +418,26 @@ class SyntheticDetectionDataset:
         img = torch.randint(0, 256, (3, self.size, self.size), generator=g, dtype=torch.uint8)
         return {"image": img, "height": self.size, "width": self.size,
                 "instances": Instances((self.size, self.size), boxes=Boxes(box), classes=torch.randint(0, self.num_classes, (k,), generator=g))}
+
+
+class SyntheticSemSegDataset:
+    """ADE20K-shaped synthetic semantic-segmentation entries: seeded uint8 images [3,H,W] and label maps `sem_seg` [H,W] uint8 made of class blocks on an
+    8x8 grid with about 5% of the pixels set to ignore_label.  The entries take the `sizes` in turn, in consecutive runs (default: two non-square sizes that
+    are not multiples of 32).  `metadata.ignore_label` is what inference_on_dataset hands to SemSegEvaluator."""
+
+    def __init__(self, n: int = 8, sizes=((357, 483), (250, 333)), num_classes: int = 150, ignore_label: int = 255, seed: int = 7):
+        from types import SimpleNamespace
+        self.n, self.sizes, self.num_classes, self.seed = n, [tuple(s) for s in sizes], num_classes, seed
+        self.metadata = SimpleNamespace(ignore_label=ignore_label)
+
+    def __len__(self):
+        return self.n
+
+    def __getitem__(self, i):
+        g = torch.Generator().manual_seed(self.seed * 100003 + i)
+        H, W = self.sizes[i * len(self.sizes) // self.n]
+        img = torch.randint(0, 256, (3, H, W), generator=g, dtype=torch.uint8)
+        blocks = torch.randint(0, self.num_classes, (8, 8), generator=g, dtype=torch.uint8)
+        gt = blocks[(torch.arange(H) * 8 // H)[:, None], (torch.arange(W) * 8 // W)[None, :]]
+        gt[torch.rand((H, W), generator=g) < 0.05] = self.metadata.ignore_label
+        return {"image": img, "height": H, "width": W, "sem_seg": gt}

@@ -244,6 +244,18 @@ int fb200_mask_sigmoid_upsample_argmax(const void* x, int dtype, int B, int h, i
  * straight from the low-resolution logits; and the upsampled probabilities of only the n kept (b,q) pairs (bq [n,2] i32 -> out [n,H,W] f32). */
 int fb200_mask_sigmoid_upsample_stats(const void* x, int dtype, int B, int h, int w, int Qp, int Q, int H, int W, float thr, int* count, float* psum, void* stream);
 int fb200_mask_sigmoid_upsample_select(const void* x, int dtype, int h, int w, int Qp, const int* bq, int n, float* out, int H, int W, void* stream);
+/* The probabilities of fb200_mask_sigmoid_upsample (same values) in NHWC, as the operand of the class x mask product of semantic evaluation
+ * (fai_mf/processor.py:99-105,142-166): out [B,H,W,Qo] with channels Q..Qo-1 zero, Qo % 4 == 0.  out_dtype FB200_F32 / FB200_F16: one plane;
+ * FB200_F16PAIR: per pixel [hi(Qo) | lo(Qo)] fp16, the operand of fb200_conv2d_pair. */
+int fb200_mask_sigmoid_upsample_nhwc(const void* x, int dtype, int B, int h, int w, int Qp, int Q, void* out, int out_dtype, int Qo, int H, int W, void* stream);
+
+/* SemSegEvaluator.process (trainer/evaluation/sem_seg_evaluation.py:86-107): conf[(C+1) * pred + gt] += 1 for every pixel of scores [B,H,W,*] fp32 NHWC
+ * (pixel pitch `pitch`, `batch_stride` elements between images; only channels 0..C-1 count), pred = argmax over c < C with the FIRST maximum winning
+ * and a NaN counting as the maximum (the first NaN wins), as torch.argmax on the CPU; gt = labels[b,y,x] (uint8 or int32: label_bytes 1 / 4), mapped
+ * to C when it equals ignore_label.  conf: (C+1) x (C+1) int64 on the device, added into (row = prediction, column = ground truth).  A label outside
+ * [0, C] that is not ignore_label is not counted; `invalid` (one int64) is incremented instead (the reference's bincount raises on it). */
+int fb200_sem_seg_confusion(const float* scores, int B, int H, int W, int C, int pitch, int64_t batch_stride, const void* labels, int label_bytes,
+                            int ignore_label, int64_t* conf, int64_t* invalid, void* stream);
 
 /* MaskFormerProcessor.postprocess reductions (fai_mf/processor.py:222-257): per plane of masks [planes, hw] fp32:
  * count = #(p >= thr), psum = sum of those p. */
