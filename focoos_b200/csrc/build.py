@@ -11,7 +11,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-SOURCES = ["conv_simt.cu", "conv_tc.cu", "pool_resize.cu", "norm_attn.cu", "msda.cu", "select.cu", "head_fused.cu", "mf_ops.cu", "bisenet_ops.cu", "criterion.cu", "optim.cu", "bwd_conv_norm.cu", "bwd_attn.cu", "wgrad_tc.cu", "mask_png.cu", "sem_seg.cu"]
+SOURCES = ["conv_simt.cu", "conv_tc.cu", "pool_resize.cu", "norm_attn.cu", "msda.cu", "select.cu", "head_fused.cu", "mf_ops.cu", "bisenet_ops.cu", "criterion.cu", "optim.cu", "bwd_conv_norm.cu", "bwd_attn.cu", "wgrad_tc.cu", "mask_png.cu", "sem_seg.cu", "box_ap.cu"]
 HEADERS = ["common.cuh", "tma.cuh", "wgmma.cuh", os.path.join(ROOT, "include", "focoos_b200.h")]
 LIB_DIR = os.path.join(os.path.dirname(HERE), "lib")
 LIB = os.path.join(LIB_DIR, "libfocoos_b200.so")

@@ -2,8 +2,8 @@
 
 Images are independent units, so the path shards with NO data-path collective (SURVEY.md §8e): one process per GPU,
 each with a full model replica, the batch split evenly on the host.  `torch.distributed` (NCCL on GPUs, gloo in the CPU
-tests) is used only to agree on the wall/devices timing (barrier + max over ranks) and to gather per-rank detection
-counts for reporting.  Mirrors the role of `focoos/utils/distributed/{dist,comm}.py` for inference
+tests) is used only to agree on the wall/devices timing (barrier + max over ranks), to gather per-rank detection
+counts for reporting, and to combine the evaluators' state (box-AP records, confusion matrix) on rank 0.  Mirrors the role of `focoos/utils/distributed/{dist,comm}.py` for inference
 (`comm.get_rank/get_world_size/synchronize/all_gather`), minus DDP (fine-tuning is a later round).
 """
 from __future__ import annotations
@@ -68,3 +68,32 @@ def gather_counts(count: int, device: torch.device | str = "cpu") -> List[int]:
     out = [torch.zeros_like(t) for _ in range(get_world_size())]
     dist.all_gather(out, t)
     return [int(o.item()) for o in out]
+
+
+def collective_device() -> torch.device:
+    """where the default group's collectives take their tensors: the current GPU under NCCL, the host otherwise (gloo)"""
+    if get_world_size() > 1 and dist.get_backend() == "nccl":
+        return torch.device("cuda", torch.cuda.current_device())
+    return torch.device("cpu")
+
+
+def all_gather_rows(t: torch.Tensor) -> List[torch.Tensor]:
+    """all_gather of a [n, ...] tensor whose n differs between ranks (evaluation records): padded to the largest n, trimmed after -> one tensor per rank,
+    in rank order, on collective_device()"""
+    t = t.to(collective_device())
+    if get_world_size() == 1:
+        return [t]
+    n = gather_counts(t.shape[0], t.device)
+    pad = t.new_zeros((max(n),) + tuple(t.shape[1:]))
+    pad[: t.shape[0]] = t
+    out = [torch.empty_like(pad) for _ in n]
+    dist.all_gather(out, pad)
+    return [o[:k] for o, k in zip(out, n)]
+
+
+def all_reduce_sum(t: torch.Tensor) -> torch.Tensor:
+    """SUM over the ranks of a copy of `t`, on collective_device() (`t` itself is left as it is)"""
+    t = t.to(collective_device(), copy=True)
+    if get_world_size() > 1:
+        dist.all_reduce(t, op=dist.ReduceOp.SUM)
+    return t

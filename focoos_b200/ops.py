@@ -418,6 +418,15 @@ class CudaBackend:
         self._call("fb200_sem_seg_confusion", _p(scores), B, H, W, C, pitch, scores.stride(0) if B > 1 else H * W * pitch, _p(labels), labels.element_size(),
                    ignore_label, _p(conf), _p(invalid), _stream())
 
+    # ---- box-AP evaluation (trainer.DeviceBoxAPEvaluator) --------------------------------------------------------------------------------------------
+    # Private for the same reason: its CPU restatement is oracle/box_ap_ref.py (BoxAPRefBackend).
+    def _box_ap_match(self, scores, classes, boxes, counts, gt_boxes, gt_classes, gt_offsets, gt_offsets_host, thresholds_host, C, tp, gt_count):
+        self._cuda(scores, classes, boxes, counts, gt_boxes, gt_classes, gt_offsets, tp, gt_count)
+        B, K = scores.shape
+        self._call("fb200_box_ap_match", _p(scores), _p(classes), _p(boxes), _p(counts), B, K, _p(gt_boxes), int(gt_boxes.dtype == torch.float64),
+                   _p(gt_classes), _p(gt_offsets), _p(gt_offsets_host), gt_boxes.shape[0], _p(thresholds_host), thresholds_host.numel(), C, _p(tp),
+                   _p(gt_count), _stream())
+
     def mask_stats(self, masks, thr, count, psum):
         self._cuda(masks, count, psum)
         B, Q, H, W = masks.shape
@@ -1190,6 +1199,27 @@ def sem_seg_confusion(scores, labels, num_classes: int, ignore_label: int, conf,
     assert conf.dtype == torch.int64 and tuple(conf.shape) == (num_classes + 1, num_classes + 1) and conf.is_contiguous()
     assert invalid.dtype == torch.int64 and invalid.numel() == 1
     _be()._sem_seg_confusion(scores, labels.contiguous(), int(num_classes), int(ignore_label), conf, invalid)
+
+
+def box_ap_match(scores, classes, boxes, counts, gt_boxes, gt_classes, gt_offsets, thresholds, num_classes: int, gt_count):
+    """The greedy matching of BoxAPEvaluator.evaluate for a batch of images, bit for bit, in one launch -> tp int16 [B,K]: bit t set when detection
+    (b, k) is a true positive at thresholds[t].  Detections as DETRProcessor.eval_postprocess leaves them: scores fp32 [B,K], classes int32 [B,K],
+    boxes fp32 [B,K,4] absolute xyxy, counts int32 [B] (the first counts[b] of row b are valid).  Ground truth: boxes fp32 / fp64 [G,4] (the IoU runs
+    in that precision, as numpy promotes), classes int32 [G], offsets int32 [B+1] on the HOST (image b owns rows offsets[b]..offsets[b+1]-1; checked
+    before the launch).  thresholds: fp64 values on the host (at most 16).  gt_count int64 [num_classes] on the device is added the ground truths of
+    each class in [0, num_classes)."""
+    B, K = scores.shape
+    assert scores.dtype == torch.float32 and classes.dtype == torch.int32 and tuple(classes.shape) == (B, K), (scores.dtype, classes.dtype, tuple(classes.shape))
+    assert boxes.dtype == torch.float32 and tuple(boxes.shape) == (B, K, 4) and counts.dtype == torch.int32 and counts.numel() == B
+    assert gt_boxes.dtype in (torch.float32, torch.float64) and gt_boxes.dim() == 2 and gt_boxes.shape[1] == 4, (gt_boxes.dtype, tuple(gt_boxes.shape))
+    assert gt_classes.dtype == torch.int32 and gt_classes.numel() == gt_boxes.shape[0] and gt_offsets.dtype == torch.int32 and gt_offsets.numel() == B + 1
+    assert gt_count.dtype == torch.int64 and gt_count.numel() == num_classes and gt_count.is_contiguous()
+    off_host = gt_offsets.cpu().contiguous()
+    thr = torch.as_tensor(np.asarray(thresholds, dtype=np.float64)).contiguous()
+    tp = torch.empty((B, K), dtype=torch.int16, device=scores.device)
+    _be()._box_ap_match(scores.contiguous(), classes.contiguous(), boxes.contiguous(), counts.contiguous(), gt_boxes.contiguous(), gt_classes.contiguous(),
+                        off_host.to(scores.device, non_blocking=True), off_host, thr, int(num_classes), tp, gt_count)
+    return tp
 
 
 def mask_stats(masks, thr: float):

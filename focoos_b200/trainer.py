@@ -143,10 +143,14 @@ def _train_worker(rank: int, world: int, fm, args: TrainerArgs, data_train, data
             history.append({"iter": it, "total_loss": tot, **opt.stats()})
             if rank == 0:
                 print(f"[focoos_b200.train] iter {it}: total_loss {tot:.4f} lr_factor {lr_factor(it, args.max_iters, args.scheduler, args.scheduler_extra):.3g} scale {history[-1]['scale']:.0f}", flush=True)
+        # EvalHook.after_step (trainer/hooks/hook.py:539-545): every eval_period iterations; the one after the last iteration is the final evaluation
+        if data_val is not None and args.eval_period > 0 and (it + 1) % args.eval_period == 0 and it + 1 != args.max_iters:
+            history.append({"iter": it, "val_metrics": _evaluate_while_training(fm, data_val, args.batch_size, dev)})
     metrics = None
-    if data_val is not None and rank == 0:
-        model.eval()
-        metrics = inference_on_dataset(fm, data_val, batch_size=args.batch_size)
+    if data_val is not None:  # every rank evaluates its shard; rank 0 gets the metrics of all of data_val
+        metrics = _evaluate_while_training(fm, data_val, args.batch_size, dev)
+        if args.eval_period > 0:  # EvalHook.after_train
+            history.append({"iter": args.max_iters - 1, "val_metrics": metrics})
     if rank == 0:
         os.makedirs(out_dir, exist_ok=True)
         torch.save({"model": {k: v.detach().cpu() for k, v in model.state_dict().items()}}, os.path.join(out_dir, "model_final.pth"))  # ArtifactName.WEIGHTS
@@ -158,6 +162,19 @@ def _train_worker(rank: int, world: int, fm, args: TrainerArgs, data_train, data
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def _evaluate_while_training(fm, data_val, batch_size: int, dev) -> dict:
+    """inference_on_dataset between training iterations, leaving training as it was: no gradients flow (no_grad), the parameters, optimiser state and
+    BatchNorm running statistics are only read (the eval forward packs its own copy of the weights), the global RNG state is restored, and the model
+    returns to train mode.  {} on ranks other than 0."""
+    model = fm.model
+    with torch.random.fork_rng(devices=[dev] if dev.type == "cuda" else []):
+        model.eval()
+        try:
+            return inference_on_dataset(fm, data_val, batch_size=batch_size)
+        finally:
+            model.train()
 
 
 def run_train_entry(fm, args: TrainerArgs, data_train, data_val=None):
@@ -261,18 +278,132 @@ class BoxAPEvaluator:
                 "num_detections": len(self.dets), "num_images": self._img}
 
 
+class DeviceBoxAPEvaluator(BoxAPEvaluator):
+    """BoxAPEvaluator with the matching on the device and the ranks combined; `evaluate` returns the dict BoxAPEvaluator returns for the same images.
+    `process` runs the greedy matching of a whole batch in one launch (ops.box_ap_match) and keeps one record per detection on the device: score,
+    class, true-positive bits per IoU threshold, image and detection index.  `evaluate` gathers the records of every rank (images numbered in rank
+    order, as the contiguous shards of inference_on_dataset lie in the dataset), sums the ground-truth counts, and on rank 0 accumulates precision /
+    recall per class in numpy: one stable sort by (class, -score, image, detection), cumulative sums, the precision envelope and the 101 recall points,
+    with BoxAPEvaluator's arithmetic.  Other ranks return {} (as the reference's evaluators do)."""
+
+    THRESHOLDS = np.arange(0.5, 0.96, 0.05)
+
+    def reset(self):
+        self._rec: List[torch.Tensor] = []  # int32 [n,5] per batch: score bits, class, tp bits, image (this rank), detection index
+        self._npos = None                   # int64 [C] ground truths per class, on the device of the first batch
+        self._img = 0
+        self._ndet = 0
+
+    @staticmethod
+    def _gt(e):
+        """(boxes [n,4] as the entry holds them, classes [n] int64) of an entry, as BoxAPEvaluator.process reads them"""
+        gi = _get(e, "instances") if (isinstance(e, dict) and "instances" in e) or hasattr(e, "instances") else None
+        if gi is None:
+            return np.zeros((0, 4), np.float32), np.zeros((0,), np.int64)
+        gb = _get(gi, "boxes")
+        gb = (gb.tensor if hasattr(gb, "tensor") else torch.as_tensor(gb)).cpu().numpy().reshape(-1, 4)
+        return gb, np.asarray(torch.as_tensor(_get(gi, "classes")).cpu().numpy(), dtype=np.int64).reshape(-1)
+
+    def process(self, inputs, outputs):
+        pairs = list(zip(inputs, outputs))
+        if not pairs:
+            return
+        insts = [o["instances"] for _, o in pairs]
+        dev = insts[0].scores.device
+        B, C = len(pairs), self.num_classes
+        counts = [int(i.scores.shape[0]) for i in insts]
+        K = max(max(counts), 1)
+        scores = torch.zeros((B, K), dtype=torch.float32, device=dev)
+        classes = torch.full((B, K), -1, dtype=torch.int32, device=dev)
+        boxes = torch.zeros((B, K, 4), dtype=torch.float32, device=dev)
+        for b, (inst, n) in enumerate(zip(insts, counts)):
+            scores[b, :n] = inst.scores
+            classes[b, :n] = inst.classes
+            boxes[b, :n] = inst.boxes.tensor
+        gts = [self._gt(e) for e, _ in pairs]
+        # numpy promotes the IoU of fp32 detections to fp64 for fp64 (or integer) ground truth: one launch per precision present in the batch
+        fp64 = [np.result_type(np.float32, gb.dtype) == np.float64 for gb, _ in gts]
+        if self._npos is None:
+            self._npos = torch.zeros((C,), dtype=torch.int64, device=dev)
+        tp = torch.zeros((B, K), dtype=torch.int16, device=dev)
+        for prec in sorted(set(fp64)):
+            sel = [b for b in range(B) if fp64[b] == prec]
+            off = np.concatenate([[0], np.cumsum([len(gts[b][1]) for b in sel])]).astype(np.int32)
+            gb = np.concatenate([gts[b][0] for b in sel]).astype(np.float64 if prec else np.float32).reshape(-1, 4)
+            gc = np.clip(np.concatenate([gts[b][1] for b in sel]), -1, np.iinfo(np.int32).max).astype(np.int32)
+            rows = slice(None) if len(sel) == B else torch.tensor(sel, device=dev)
+            cnt = torch.tensor([counts[b] for b in sel], dtype=torch.int32).to(dev, non_blocking=True)
+            t = ops.box_ap_match(scores[rows], classes[rows], boxes[rows], cnt, torch.from_numpy(gb).to(dev), torch.from_numpy(gc).to(dev),
+                                 torch.from_numpy(off), self.THRESHOLDS, C, self._npos)
+            tp[rows] = t
+        rec = torch.stack([scores.view(torch.int32), classes, tp.to(torch.int32) & 0xFFFF,
+                           (self._img + torch.arange(B, dtype=torch.int32, device=dev))[:, None].expand(B, K),
+                           torch.arange(K, dtype=torch.int32, device=dev)[None, :].expand(B, K)], -1).reshape(B * K, 5)
+        keep = np.concatenate([b * K + np.arange(n) for b, n in enumerate(counts)]).astype(np.int64)
+        self._rec.append(rec.index_select(0, torch.from_numpy(keep).to(dev, non_blocking=True)))
+        self._img += B
+        self._ndet += sum(counts)
+
+    def evaluate(self):
+        C, T = self.num_classes, len(self.THRESHOLDS)
+        rec = torch.cat(self._rec) if self._rec else torch.zeros((0, 5), dtype=torch.int32)
+        parts = D.all_gather_rows(rec)
+        imgs = D.gather_counts(self._img, D.collective_device())
+        npos_t = torch.zeros((C,), dtype=torch.int64) if self._npos is None else self._npos
+        npos = D.all_reduce_sum(npos_t).cpu().numpy()
+        ndet = sum(D.gather_counts(self._ndet, D.collective_device()))
+        if D.get_rank() != 0:
+            return {}
+        first = np.concatenate([[0], np.cumsum(imgs)[:-1]])
+        R = np.concatenate([p.cpu().numpy() for p in parts]) if parts else np.zeros((0, 5), np.int32)
+        img = R[:, 3].astype(np.int64) + np.repeat(first, [p.shape[0] for p in parts])
+        score = np.ascontiguousarray(R[:, 0]).view(np.float32)
+        cls, bits = R[:, 1], R[:, 2]
+        order = np.lexsort((R[:, 4], img, -score.astype(np.float64), cls))
+        cls, bits = cls[order], bits[order]
+        aps = np.zeros((T, C))
+        has = npos > 0
+        rs = np.linspace(0, 1, 101)
+        lo = np.searchsorted(cls, np.arange(C), side="left")
+        hi = np.searchsorted(cls, np.arange(C), side="right")
+        for c in np.nonzero(has)[0]:
+            n = int(hi[c] - lo[c])
+            if n == 0:
+                continue
+            tp = ((bits[lo[c]:hi[c]][None, :] >> np.arange(T)[:, None]) & 1).astype(np.float64)
+            ctp = np.cumsum(tp, axis=1)
+            recall = ctp / int(npos[c])
+            prec = ctp / np.maximum(np.arange(1, n + 1), 1)
+            prec = np.maximum.accumulate(prec[:, ::-1], axis=1)[:, ::-1]
+            for ti in range(T):
+                idx = np.searchsorted(recall[ti], rs, side="left")
+                aps[ti, c] = np.mean(np.where(idx < n, prec[ti][np.minimum(idx, n - 1)], 0.0))
+        if not has.any():
+            return {"bbox": {"AP": float("nan"), "AP50": float("nan"), "AP75": float("nan")}, "num_detections": ndet}
+        return {"bbox": {"AP": float(aps[:, has].mean() * 100), "AP50": float(aps[0, has].mean() * 100), "AP75": float(aps[5, has].mean() * 100)},
+                "num_detections": ndet, "num_images": sum(imgs)}
+
+
+def _box_ap_evaluator(num_classes: int) -> BoxAPEvaluator:
+    """DeviceBoxAPEvaluator.  The host BoxAPEvaluator only when a test installs a CPU reference backend that does not restate the matching kernel
+    (`ops._backend`; product code never sets it)."""
+    if ops._backend is not None and not hasattr(ops._backend, "_box_ap_match"):
+        return BoxAPEvaluator(num_classes)
+    return DeviceBoxAPEvaluator(num_classes)
+
+
 @torch.no_grad()
 def inference_on_dataset(fm, dataset, batch_size: int = 16, evaluator=None, top_k: Optional[int] = None):
     """evaluator.py:115-238: run the model over `dataset` in batches (the reference uses batch 1 per GPU), `processor.eval_postprocess`, `evaluator.process`;
-    each rank takes a contiguous shard and rank 0 evaluates its own (single-process evaluation is the tested path).  The evaluator follows the processor:
-    BoxAPEvaluator for DETRProcessor, SemSegEvaluator for MaskFormerProcessor, whose batches hold consecutive entries of one image size and run the model
-    with `lazy_masks = True` (as FocoosModel.__call__ does)."""
+    each rank of an initialised process group takes a contiguous shard and the evaluator combines the ranks: rank 0 returns the metrics of the whole
+    dataset, the other ranks {}.  The evaluator follows the processor: DeviceBoxAPEvaluator for DETRProcessor, SemSegEvaluator for MaskFormerProcessor,
+    whose batches hold consecutive entries of one image size and run the model with `lazy_masks = True` (as FocoosModel.__call__ does)."""
     from .processor import MaskFormerProcessor
     model, proc = fm.model, fm.processor
     model.eval()
     if isinstance(proc, MaskFormerProcessor):
         return _sem_seg_inference(fm, dataset, batch_size, evaluator)
-    evaluator = evaluator or BoxAPEvaluator(model.config.num_classes)
+    evaluator = evaluator or _box_ap_evaluator(model.config.num_classes)
     evaluator.reset()
     lo, hi = D.shard_range(len(dataset))
     for s in range(lo, hi, batch_size):
@@ -311,9 +442,41 @@ def _sem_seg_inference(fm, dataset, batch_size, evaluator):
     return evaluator.evaluate()
 
 
-def run_eval_entry(fm, args: TrainerArgs, data_test, save_json: bool = True):
-    assert args.num_gpus, "Testing without GPUs is not supported. num_gpus must be greater than 0"  # focoos_model.py:300
+def _eval_worker(rank: int, world: int, fm, args: TrainerArgs, data_test, result_path: str):
+    """one rank of a multi-GPU model.eval: its shard through inference_on_dataset; rank 0 writes the metrics of the whole dataset to `result_path`"""
+    os.environ.update(RANK=str(rank), LOCAL_RANK=str(rank), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(args.master_port))
+    torch.cuda.set_device(rank)
+    D.init_from_env("nccl", torch.device("cuda", rank))
+    fm.model.cuda(rank)
     metrics = inference_on_dataset(fm, data_test, batch_size=args.batch_size)
+    if rank == 0:
+        with open(result_path, "w") as f:
+            json.dump(metrics, f)
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def run_eval_entry(fm, args: TrainerArgs, data_test, save_json: bool = True):
+    """focoos_model.py:276-310: one process (num_gpus = 1) or one per GPU, each evaluating a contiguous shard, combined by the evaluator; the metrics of the
+    whole dataset are returned, kept in model_info.val_metrics and written to <output_dir>/<run_name>/eval_metrics.json when `save_json`."""
+    assert args.num_gpus, "Testing without GPUs is not supported. num_gpus must be greater than 0"  # focoos_model.py:300
+    if args.num_gpus > 1:
+        import tempfile
+
+        import torch.multiprocessing as mp
+        fm.model.cpu()
+        fm._graphs.clear()
+        fm._pipe = None
+        with tempfile.TemporaryDirectory() as tmp:
+            path = os.path.join(tmp, "metrics.json")
+            try:
+                mp.start_processes(_eval_worker, args=(args.num_gpus, fm, args, data_test, path), nprocs=args.num_gpus, join=True, start_method="spawn")
+            finally:
+                fm.model.cuda()
+            with open(path) as f:
+                metrics = json.load(f)  # JSON keeps every float bit for bit (repr round trip), NaN included
+    else:
+        metrics = inference_on_dataset(fm, data_test, batch_size=args.batch_size)
     fm.model_info.val_metrics = metrics
     if save_json:
         out_dir = os.path.join(args.output_dir, args.run_name)
@@ -370,9 +533,20 @@ class SemSegEvaluator:
         return np.zeros((C + 1, C + 1), dtype=np.int64) if self._conf is None else self._conf.cpu().numpy()
 
     def evaluate(self):
-        if self._invalid is not None and int(self._invalid.item()):
-            raise ValueError(f"{int(self._invalid.item())} ground-truth pixels are neither in [0, {self.num_classes}] nor ignore_label={self.ignore_label}")
-        conf = self.confusion_matrix()
+        """the metrics of this rank's matrix, or with a process group of several ranks, of the matrices summed over the ranks (on rank 0; {} elsewhere)"""
+        if D.get_world_size() > 1:  # one SUM of [matrix | invalid count]; every rank raises on invalid labels
+            C = self.num_classes
+            local = torch.zeros(((C + 1) ** 2 + 1,), dtype=torch.int64)
+            if self._conf is not None:
+                local = torch.cat([self._conf.reshape(-1), self._invalid])
+            tot = D.all_reduce_sum(local).cpu().numpy()
+            conf, invalid = tot[:-1].reshape(C + 1, C + 1), int(tot[-1])
+        else:
+            conf, invalid = self.confusion_matrix(), 0 if self._invalid is None else int(self._invalid.item())
+        if invalid:
+            raise ValueError(f"{invalid} ground-truth pixels are neither in [0, {self.num_classes}] nor ignore_label={self.ignore_label}")
+        if D.get_rank() != 0:
+            return {}
         n = self.num_classes
         acc = np.full(n, np.nan, dtype=float)
         iou = np.full(n, np.nan, dtype=float)

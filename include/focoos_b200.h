@@ -257,6 +257,19 @@ int fb200_mask_sigmoid_upsample_nhwc(const void* x, int dtype, int B, int h, int
 int fb200_sem_seg_confusion(const float* scores, int B, int H, int W, int C, int pitch, int64_t batch_stride, const void* labels, int label_bytes,
                             int ignore_label, int64_t* conf, int64_t* invalid, void* stream);
 
+/* The greedy matching of box AP (trainer.BoxAPEvaluator.evaluate) for a batch of B images, bit for bit: per image, its detections of one class are
+ * visited in (score descending, detection index ascending) order; at threshold t a detection takes the FIRST unmatched same-class ground truth of
+ * maximum IoU and is a true positive iff that IoU >= thresholds_host[t] (compared as double; used ground truths count as IoU -1, a NaN IoU as the
+ * maximum).  The IoU is numpy's arithmetic of trainer._iou_matrix, without contraction: fp32 when gt_fp64 == 0, fp64 (detections widened) otherwise.
+ * Detections as DETRProcessor.eval_postprocess leaves them: scores [B,K] fp32, classes [B,K] int32, boxes [B,K,4] fp32 absolute xyxy, the first
+ * counts[b] of row b valid.  Ground truth: boxes [G,4] fp32 / fp64, classes [G] int32, image b owns rows gt_offsets[b] .. gt_offsets[b+1]-1
+ * (gt_offsets [B+1] on the device, gt_offsets_host the same values on the host: checked to be monotonic, to start at 0 and end at G).
+ * Out: tp [B,K] (bit t of tp[b,k]: true positive at threshold t; 0 past counts[b]); gt_count [C] int64 += the ground truths of each class in [0, C).
+ * Limits: K <= 1024, at most 1024 ground truths per image, 1 <= T <= 16 thresholds. */
+int fb200_box_ap_match(const float* scores, const int* classes, const float* boxes, const int* counts, int B, int K, const void* gt_boxes, int gt_fp64,
+                       const int* gt_classes, const int* gt_offsets, const int* gt_offsets_host, int G, const double* thresholds_host, int T, int C,
+                       uint16_t* tp, int64_t* gt_count, void* stream);
+
 /* MaskFormerProcessor.postprocess reductions (fai_mf/processor.py:222-257): per plane of masks [planes, hw] fp32:
  * count = #(p >= thr), psum = sum of those p. */
 int fb200_mask_stats(const float* masks, int64_t planes, int64_t hw, float thr, int* count, float* psum, void* stream);
