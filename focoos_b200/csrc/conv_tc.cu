@@ -17,8 +17,9 @@
 //                  chunks) layout wgmma reads through its shared-memory descriptors.  After a tile's last k-block the producer loads
 //                  the tile's residual (if any) into the next ring entries, so it is in flight while the consumers finish the previous tile.
 //   warp-groups 1-2  consumers: group g owns tile rows 64g..64g+63.  Per k-block it issues BLOCK_K/16 x wgmma.m64nBLOCK_Nk16
-//                  (three per step in the fp32-accurate fused-split mode) into its register accumulator and releases the ring stage
-//                  one k-block later (wgmma.wait_group 1).  The epilogue of its rows follows: folded-BN scale/bias, residual (before
+//                  into its register accumulator and releases the ring stage once they have retired (wgmma.wait_group 1 in the next
+//                  k-block).  In the fp32-accurate fused-split mode a step is three products; at BLOCK_N = 128 they take A from registers
+//                  (A_hi and A_lo loaded by ldmatrix), one wgmma group per step.  The epilogue of its rows follows: folded-BN scale/bias, residual (before
 //                  or after the activation), ReLU/SiLU/GELU -> fp16/fp32/pair -> swizzled smem staging (double buffered, shared by
 //                  both groups) -> TMA store (clips ragged tiles / Cout tails).  The producer keeps filling the ring with the next
 //                  tile's operands meanwhile.
@@ -163,6 +164,32 @@ template <int BLOCK_N, int STAGES, int BLOCK_K, int NSTG, bool FS> constexpr int
   return STAGES * (a_stage_bytes<BLOCK_K, FS>() + b_stage_bytes<BLOCK_N, BLOCK_K, FS>()) + NSTG * STAGING_BYTES + (2 * STAGES + 1) * 8 + 1024 /*align slack*/;
 }
 
+// The FS products of the N = 128 configurations take A from registers: each warp loads A_hi and A_lo of its 16 rows once per 16-channel step with ldmatrix
+// and feeds both A_hi products from the same fragment, where descriptors would have the tensor pipe read A_hi from shared memory twice.
+// Byte offset of the row this lane hands ldmatrix_x4 for the A fragment of rows row0 .. row0 + 15, channels 16k .. 16k + 15, inside an operand tile of
+// BLOCK_K channels.  The ring's tiles have the staging tiles' swizzles (64 channels: 128-byte rows like fp16 staging; 32 channels: 64-byte rows like a pair
+// plane), and every tile starts on a multiple of the swizzle's repeat.
+template <int BLOCK_K>
+__device__ __forceinline__ uint32_t a_frag_offset(int row0, int k, int lane) {
+  typedef std::conditional_t<BLOCK_K == 64, __half, PairOut> Layout;
+  return (uint32_t)staging_offset<Layout>(row0 + (lane & 15), 16 * k + 8 * (lane >> 4));
+}
+
+// One 16-channel FS step as one wgmma group: ldmatrix A_hi and A_lo at a_hi / a_lo into fr, then hi x W_hi, hi x W_lo, lo x W_hi.  Callers alternate two
+// fragment buffers; the wait retires the previous step's group, so the other buffer may be reloaded while this step's products run.
+template <int BLOCK_N>
+__device__ __forceinline__ void fs_step(float (&acc)[BLOCK_N / 2], uint32_t (&fr)[2][4], uint32_t a_hi, uint32_t a_lo, uint64_t db_hi, uint64_t db_lo,
+                                        uint32_t scale_d) {
+  ldmatrix_x4(fr[0], a_hi);
+  ldmatrix_x4(fr[1], a_lo);
+  wgmma_fence();
+  WgmmaRS<BLOCK_N>::mma(acc, fr[0], db_hi, scale_d);
+  WgmmaRS<BLOCK_N>::mma(acc, fr[0], db_lo, 1u);
+  WgmmaRS<BLOCK_N>::mma(acc, fr[1], db_hi, 1u);
+  wgmma_commit();
+  wgmma_wait<1>();
+}
+
 // ---------------------------------------------------------------------------------------------- kernel
 template <int BLOCK_N, int STAGES, typename TOut, int BLOCK_K, int NSTG, bool GELU, bool FS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -294,6 +321,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   const bool post = (p.act & FB200_ACT_RESIDUAL_AFTER) != 0;
   const bool has_res = p.res != nullptr;
   float acc[NACC];
+  // The fused-split products take A from registers at N = 128 only.  At N = 64 a step's products are too short for it: the register form gained nothing on
+  // those convs (-1% to +4% in five sessions, H100 80GB HBM3, 700 W), and it slowed the small-channel kernel's N = 32 / 64 products.
+  constexpr bool RS = FS && BLOCK_N == 128;
+  uint32_t frag[2][2][4];  // RS: two buffers of this warp's (A_hi, A_lo) fragments
   int stage = 0;
   uint32_t phase = 0, res_phase = 0, chunk_ctr = 0;
   for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
@@ -303,22 +334,35 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       mbar_wait(&full_bar[stage], phase);
       const uint32_t sa = smem_u32(smem_a + stage * A_STAGE_BYTES) + (uint32_t)(th.g * 64 * BLOCK_K * 2);
       const uint32_t sb = smem_u32(smem_b + stage * B_STAGE_BYTES);
-      const uint64_t da = make_smem_desc<BLOCK_K>(sa), db = make_smem_desc<BLOCK_K>(sb);
-      wgmma_fence();
+      const uint64_t db = make_smem_desc<BLOCK_K>(sb);
+      if constexpr (RS) {  // hi x W_hi, hi x W_lo, lo x W_hi into the same fp32 accumulator, one group per step
+        const uint64_t db_lo = make_smem_desc<BLOCK_K>(sb + B_HALF);
+        const int row0 = ((th.ct & 127) >> 5) * 16;
 #pragma unroll
-      for (int k = 0; k < BLOCK_K / 16; ++k) {
-        // advance 16 halves = 32 B inside the swizzle row: +2 in 16-byte units
-        const uint64_t ko = (uint64_t)(k * 2);
-        Wgmma<BLOCK_N, 0>::mma(acc, da + ko, db + ko, (kb > 0 || k > 0) ? 1u : 0u);
-        if constexpr (FS) {  // hi x W_lo, lo x W_hi into the same fp32 accumulator
-          const uint64_t da_lo = make_smem_desc<BLOCK_K>(sa + A_HALF), db_lo = make_smem_desc<BLOCK_K>(sb + B_HALF);
-          Wgmma<BLOCK_N, 0>::mma(acc, da + ko, db_lo + ko, 1u);
-          Wgmma<BLOCK_N, 0>::mma(acc, da_lo + ko, db + ko, 1u);
+        for (int k = 0; k < BLOCK_K / 16; ++k) {  // an even number of steps: step 0 of the next k-block takes buffer 0 again
+          const uint32_t ao = a_frag_offset<BLOCK_K>(row0, k, lane);
+          fs_step<BLOCK_N>(acc, frag[k & 1], sa + ao, sa + A_HALF + ao, db + (uint64_t)(k * 2), db_lo + (uint64_t)(k * 2), (kb > 0 || k > 0) ? 1u : 0u);
+          // at k = 0 the previous k-block's last group has retired: its stage may be refilled
+          if (k == 0 && prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
         }
+      } else {
+        const uint64_t da = make_smem_desc<BLOCK_K>(sa);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / 16; ++k) {
+          // advance 16 halves = 32 B inside the swizzle row: +2 in 16-byte units
+          const uint64_t ko = (uint64_t)(k * 2);
+          Wgmma<BLOCK_N, 0>::mma(acc, da + ko, db + ko, (kb > 0 || k > 0) ? 1u : 0u);
+          if constexpr (FS) {  // hi x W_lo, lo x W_hi into the same fp32 accumulator
+            const uint64_t da_lo = make_smem_desc<BLOCK_K>(sa + A_HALF), db_lo = make_smem_desc<BLOCK_K>(sb + B_HALF);
+            Wgmma<BLOCK_N, 0>::mma(acc, da + ko, db_lo + ko, 1u);
+            Wgmma<BLOCK_N, 0>::mma(acc, da_lo + ko, db + ko, 1u);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's products are done: its stage may be refilled
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-      wgmma_commit();
-      wgmma_wait<1>();  // the previous k-block's products are done: its stage may be refilled
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
@@ -437,6 +481,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 // 512-byte repeat of the 64-byte swizzle, so the usual descriptors address it.  That is 3 x 160 instead of 9 x 128 A rows per tile and no weights in the
 // stream.  Products run in the general kernel's order (tap, 16-channel step, then hi x W_hi, hi x W_lo, lo x W_hi) with N = Cout, so the outputs are the
 // same bits.  Same warp roles and epilogue (folded BN, activation, fp32 or pair output through TMA stores) without residual or row-max.
+// A stays in shared memory, as in the general kernel's N = 64 configurations: the register form (with two or four fragment buffers) made conv1_2 and
+// conv1_3 4-11% slower (H100 80GB HBM3, 700 W).
 constexpr int SC_BW = 16, SC_BH = 8;                 // output tile: 16 x 8 pixels = BLOCK_M rows
 constexpr int SC_BOX_ROWS = SC_BW * (SC_BH + 2);     // one kw-shifted input box
 constexpr int SC_BOX_BYTES = SC_BOX_ROWS * 64;       // 32 channels of fp16: 64-byte rows, 64-byte swizzle
