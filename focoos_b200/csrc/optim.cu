@@ -114,10 +114,58 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const
   }
 }
 
+// Model EMA (focoos/trainer/solver/ema.py:112-140), one launch per step.  Blocks [0, arena_blocks) stride over the EMA arena, which has the
+// layout of the flat parameter buffer: torch._foreach_mul_(ema, d) then torch._foreach_add_(ema, p, alpha=omd).  torch's foreach add is
+// `a + alpha * b` in fp32 and nvcc contracts it into one FMA, so the update is fma(omd, p, fl(ema * d)) - two roundings, as on the device.
+// Every further block owns one chunk of the table {src address, EMA address, length, kind}: the entries outside the flat buffer (frozen
+// parameters, BatchNorm buffers).  Kind 1 is an int64 entry, updated as `ema.copy_(ema * decay + val * (1.0 - decay))` is: both products
+// in fp32 (the int64 values converted to fp32), an fp32 sum, truncation back to int64.
+__global__ void __launch_bounds__(256) ema_kernel(float* __restrict__ ema, const float* __restrict__ p, int64_t n4, int arena_blocks,
+                                                  const int64_t* __restrict__ chunks, float d, float omd) {
+  if ((int)blockIdx.x < arena_blocks) {
+    float4* e4 = reinterpret_cast<float4*>(ema);
+    const float4* p4 = reinterpret_cast<const float4*>(p);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)arena_blocks * blockDim.x) {
+      float4 E = e4[i];
+      const float4 P = p4[i];
+      E.x = __fmaf_rn(omd, P.x, __fmul_rn(E.x, d));
+      E.y = __fmaf_rn(omd, P.y, __fmul_rn(E.y, d));
+      E.z = __fmaf_rn(omd, P.z, __fmul_rn(E.z, d));
+      E.w = __fmaf_rn(omd, P.w, __fmul_rn(E.w, d));
+      e4[i] = E;
+    }
+    return;
+  }
+  const int64_t* c = chunks + 4 * (int64_t)(blockIdx.x - arena_blocks);
+  const int64_t len = c[2];
+  if (c[3] == 1) {
+    const long long* s = reinterpret_cast<const long long*>(c[0]);
+    long long* e = reinterpret_cast<long long*>(c[1]);
+    for (int64_t i = threadIdx.x; i < len; i += blockDim.x)
+      e[i] = (long long)__fadd_rn(__fmul_rn(__ll2float_rn(e[i]), d), __fmul_rn(__ll2float_rn(s[i]), omd));
+  } else {
+    const float* s = reinterpret_cast<const float*>(c[0]);
+    float* e = reinterpret_cast<float*>(c[1]);
+    for (int64_t i = threadIdx.x; i < len; i += blockDim.x) e[i] = __fmaf_rn(omd, s[i], __fmul_rn(e[i], d));
+  }
+}
+
 }  // namespace
 }  // namespace fb200
 
 using namespace fb200;
+
+extern "C" int fb200_ema_update(float* ema, const float* params, int64_t n, const int64_t* chunks, int nchunks, float decay, float one_minus_decay,
+                                void* stream) {
+  FB_CHECK_ARG(n >= 0 && (n & 3) == 0 && nchunks >= 0 && (n > 0 || nchunks > 0) && (n == 0 || (ema && params)) && (nchunks == 0 || chunks),
+               "ema_update: bad arguments");
+  FB_CHECK_ARG(((reinterpret_cast<uintptr_t>(ema) | reinterpret_cast<uintptr_t>(params)) & 15) == 0, "ema_update: arena and parameters must be 16-byte aligned");
+  const int64_t n4 = n >> 2;
+  const int arena_blocks = (int)std::min<int64_t>((n4 + 255) / 256, (int64_t)kNumSMs * 8);
+  ema_kernel<<<arena_blocks + nchunks, 256, 0, (cudaStream_t)stream>>>(ema, params, n4, arena_blocks, chunks, decay, one_minus_decay);
+  FB_CHECK_LAUNCH("ema_update");
+  return FB200_OK;
+}
 
 extern "C" int64_t fb200_optim_workspace_bytes(void) { return (int64_t)STATS_BLOCKS * (8 + 4) + 64; }
 

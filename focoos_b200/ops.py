@@ -637,6 +637,10 @@ class CudaBackend:
         self._call("fb200_adamw_step", _p(params), _p(grads), _p(m), _p(v), _p(chunk_start), _p(chunk_len), _p(chunk_seg), chunk_len.shape[0], _p(seg_lr), _p(seg_wd), _p(seg_active),
                    lr_factor, 1.0 - beta1, 1.0 - beta2, eps, _p(ctrl), _stream())
 
+    def _ema_update(self, ema, params, chunks, decay, one_minus_decay):
+        self._cuda(ema, params, chunks)
+        self._call("fb200_ema_update", _p(ema), _p(params), ema.numel(), _p(chunks), chunks.shape[0], decay, one_minus_decay, _stream())
+
 
 class Pair:
     """An fp32 NHWC activation stored as TWO fp16 planes (hi = fp16(v), lo = fp16(v - hi), exact to ~2^-22) inside one buffer `buf` [..., 2 * Ctot]:
@@ -1199,6 +1203,15 @@ def sem_seg_confusion(scores, labels, num_classes: int, ignore_label: int, conf,
     assert conf.dtype == torch.int64 and tuple(conf.shape) == (num_classes + 1, num_classes + 1) and conf.is_contiguous()
     assert invalid.dtype == torch.int64 and invalid.numel() == 1
     _be()._sem_seg_confusion(scores, labels.contiguous(), int(num_classes), int(ignore_label), conf, invalid)
+
+
+def ema_update(ema, params, chunks, decay: float, one_minus_decay: float):
+    """One model-EMA update (train_step.ModelEMA.update) in one launch: the fp32 arena `ema` follows the flat parameter buffer `params` (same length, a
+    multiple of 4) as fma(one_minus_decay, p, ema * decay); `chunks` (int64 [n, 4] on the device: source address, EMA address, element count, kind 0 fp32 /
+    1 int64) covers the entries outside that buffer.  decay and one_minus_decay are Python floats (formed in double), rounded to fp32 for the kernel."""
+    assert ema.dtype == params.dtype == torch.float32 and ema.numel() == params.numel() and ema.numel() % 4 == 0, (ema.dtype, params.dtype, ema.numel())
+    assert ema.is_contiguous() and params.is_contiguous() and chunks.dtype == torch.int64 and chunks.dim() == 2 and chunks.shape[1] == 4 and chunks.is_contiguous()
+    _be()._ema_update(ema, params, chunks, float(decay), float(one_minus_decay))
 
 
 def box_ap_match(scores, classes, boxes, counts, gt_boxes, gt_classes, gt_offsets, thresholds, num_classes: int, gt_count):

@@ -12,6 +12,9 @@ bucket by bucket (reverse parameter order, as the backward pass produces them) f
 """
 from __future__ import annotations
 
+import itertools
+import math
+from contextlib import contextmanager
 from typing import Dict, Iterable, List, Optional, Sequence
 
 import torch
@@ -185,6 +188,77 @@ class FlatAdamW:
         self.ctrl.copy_(sd["ctrl"])
 
 
+class ModelEMA:
+    """Model EMA of the reference trainer (EMAState / EMAUpdater / EMAHook, trainer/solver/ema.py:14-140,203-228): an averaged copy of every
+    parameter and buffer (model.named_parameters() then model.named_buffers(), frozen parameters and BatchNorm statistics included), taken at
+    construction (EMAHook.before_train) and updated by `update()` after every optimiser step, skipped steps too.
+
+    The trainable parameters average in `arena`, laid out like `opt.flat_params` (same offsets and padding); every other entry (fp32 or int64)
+    has its own EMA tensor, listed in `chunks` (int64 [n, 4]: source address, EMA address, length, kind) in pieces of at most `chunk_elems`.
+    One ops.ema_update launch per update covers both.  The table holds addresses: the model's tensors must stay where they are, as the
+    trainer's in-place updates keep them."""
+
+    KIND_FP32, KIND_INT64 = 0, 1
+
+    def __init__(self, model: nn.Module, opt: FlatAdamW, decay: float = 0.999, warmup: int = 2000, chunk_elems: int = 1 << 16):
+        self.model, self.opt, self.decay, self.warmup, self.updates = model, opt, float(decay), int(warmup), 0
+        dev = opt.flat_params.device
+        flat = {id(p): i for i, p in enumerate(opt.params)}
+        self.entries: Dict[int, torch.Tensor] = {}  # id(model tensor) -> its EMA tensor
+        self.side: List[tuple] = []                 # (model tensor, EMA tensor) outside the flat buffer
+        with torch.no_grad():
+            self.arena = opt.flat_params.clone()
+            rows = []
+            for name, t in itertools.chain(model.named_parameters(), model.named_buffers()):
+                if id(t) in flat:
+                    o = opt.offsets[flat[id(t)]]
+                    self.entries[id(t)] = self.arena[o:o + t.numel()].view_as(t)
+                    continue
+                if t.dtype not in (torch.float32, torch.int64) or t.device != dev or not t.is_contiguous():
+                    raise NotImplementedError(f"ModelEMA: {name} is {t.dtype} on {t.device}; the EMA covers contiguous fp32 / int64 tensors on {dev}")
+                e = t.detach().clone()
+                self.entries[id(t)] = e
+                self.side.append((t, e))
+                kind = self.KIND_INT64 if t.dtype == torch.int64 else self.KIND_FP32
+                for s in range(0, t.numel(), chunk_elems):
+                    rows.append([t.data_ptr() + s * t.element_size(), e.data_ptr() + s * e.element_size(), min(chunk_elems, t.numel() - s), kind])
+        self.chunks = torch.tensor(rows, dtype=torch.int64).reshape(-1, 4).to(dev)
+
+    def decay_at(self, updates: int) -> float:
+        """EMAUpdater.decay_fn, in double"""
+        return self.decay * (1 - math.exp(-updates / self.warmup)) if self.warmup > 0 else self.decay
+
+    def update(self) -> None:
+        self.updates += 1
+        d = self.decay_at(self.updates)
+        ops.ema_update(self.arena, self.opt.flat_params, self.chunks, d, 1 - d)
+
+    @torch.no_grad()
+    def _load(self, flat: torch.Tensor, side: Sequence[torch.Tensor]) -> None:
+        self.opt.flat_params.copy_(flat)
+        for (t, _), v in zip(self.side, side):
+            t.copy_(v)
+
+    @contextmanager
+    def applied(self):
+        """apply_model_ema_and_restore (ema.py:188-200): the model holds the EMA inside the block and its training values, bit for bit, after it.
+        The copies go through opt.flat_params, whose views the parameters are."""
+        saved = (self.opt.flat_params.clone(), [t.detach().clone() for t, _ in self.side])
+        self._load(self.arena, [e for _, e in self.side])
+        try:
+            yield
+        finally:
+            self._load(*saved)
+
+    def apply(self) -> None:
+        """apply_model_ema (ema.py:171-185): copy the EMA into the model, for good"""
+        self._load(self.arena, [e for _, e in self.side])
+
+    def state_dict(self) -> Dict[str, torch.Tensor]:
+        """the EMA under model.state_dict()'s keys (what the model's state_dict is after apply())"""
+        return {k: self.entries.get(id(v), v).detach().clone() for k, v in self.model.state_dict(keep_vars=True).items()}
+
+
 class GradBucketReducer:
     """Data-parallel gradient exchange (what DistributedDataParallel does for the reference, dist.py:152): SUM all-reduce of
     contiguous slices of the flat gradient buffer.  Buckets follow reverse parameter order (the order backward fills them) and
@@ -278,8 +352,8 @@ class GradBucketReducer:
 class TrainStep:
     """TrainerLoop.run_step (trainer.py:723-773) for one already-preprocessed batch."""
 
-    def __init__(self, model: nn.Module, opt: FlatAdamW, reducer: Optional[GradBucketReducer] = None):
-        self.model, self.opt, self.reducer = model, opt, reducer
+    def __init__(self, model: nn.Module, opt: FlatAdamW, reducer: Optional[GradBucketReducer] = None, ema: Optional[ModelEMA] = None):
+        self.model, self.opt, self.reducer, self.ema = model, opt, reducer, ema
 
     def __call__(self, images, targets, lr_factor: float = 1.0) -> Dict[str, torch.Tensor]:
         self.opt.zero_grad()
@@ -299,4 +373,6 @@ class TrainStep:
         if self.reducer is not None:
             self.reducer.finish()
         self.opt.step(lr_factor)
+        if self.ema is not None:  # EMAHook.after_step: also after a step the loss scaler skipped
+            self.ema.update()
         return loss_dict

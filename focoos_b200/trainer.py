@@ -6,8 +6,11 @@
   WarmupMultiStepLR                 focoos/trainer/solver/lr_scheduler.py:73-110 -> `lr_factor`
   run_train / launch                focoos/trainer/trainer.py:283-420, utils/distributed/dist.py:40-137 -> `run_train_entry` (one process per GPU, NCCL)
   inference_on_dataset              focoos/trainer/evaluation/evaluator.py:115-238 -> `inference_on_dataset` (batched, instances stay on the device)
+  EMAHook / EMAUpdater              focoos/trainer/solver/ema.py:96-228    -> train_step.ModelEMA (TrainerArgs.ema_enabled: one device pass per step,
+                                                                              evaluation and model_final.pth from the averaged weights)
 
-Out of scope (reference control plane, SURVEY §2): hooks, checkpointer rotation, EMA, Hub sync, tensorboard, COCO-json evaluators (pycocotools);
+Out of scope (reference control plane, SURVEY §2): hooks, checkpointer rotation, resume / init_checkpoint (so no `ema_state` in checkpoints, and
+`ema_warmup` applies as given), Hub sync, tensorboard, COCO-json evaluators (pycocotools);
 `BoxAPEvaluator` below is a small self-contained AP@[.5:.95] / AP50 so that `model.eval` returns numbers without those dependencies.
 
 Dataset contract (reference `MapDataset` of `DatasetEntry`, ports.py): `len(ds)`, `ds[i]` -> entry with `.image` (uint8 / float tensor [3,H,W]),
@@ -17,6 +20,7 @@ COCO-shape data of BASELINE configs[4] is 640x640).
 """
 from __future__ import annotations
 
+import contextlib
 import json
 import os
 from dataclasses import asdict, dataclass
@@ -59,6 +63,9 @@ class TrainerArgs:
     freeze_bn: bool = False
     clip_gradients: float = 0.1
     sync_bn: bool = True  # torch.nn.SyncBatchNorm.convert_sync_batchnorm when world_size > 1 (trainer.py:334)
+    ema_enabled: bool = False  # model EMA (trainer.py:488-495): evaluation and model_final.pth from the averaged weights
+    ema_decay: float = 0.999
+    ema_warmup: int = 2000
     master_port: int = 29531
 
 
@@ -106,7 +113,7 @@ def lr_factor(it: int, max_iters: int, scheduler: str = "MULTISTEP", extra: Opti
 
 
 def _train_worker(rank: int, world: int, fm, args: TrainerArgs, data_train, data_val, out_dir: str):
-    from .train_step import FlatAdamW, GradBucketReducer, TrainStep, get_optimizer_params
+    from .train_step import FlatAdamW, GradBucketReducer, ModelEMA, TrainStep, get_optimizer_params
     if world > 1:
         os.environ.update(RANK=str(rank), LOCAL_RANK=str(rank), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(args.master_port))
         torch.cuda.set_device(rank)
@@ -130,7 +137,9 @@ def _train_worker(rank: int, world: int, fm, args: TrainerArgs, data_train, data
     opt.track_unused_parameters()
     red = GradBucketReducer(opt)
     red.attach_hooks()
-    step = TrainStep(model, opt, red)
+    # EMAHook.before_train: the EMA starts from the weights every rank trains from (after the reducer's broadcast); every rank keeps its own
+    ema = ModelEMA(model, opt, args.ema_decay, args.ema_warmup) if args.ema_enabled else None
+    step = TrainStep(model, opt, red, ema)
     g = torch.Generator().manual_seed(args.seed + rank)
     n = len(data_train)
     history = []
@@ -145,7 +154,9 @@ def _train_worker(rank: int, world: int, fm, args: TrainerArgs, data_train, data
                 print(f"[focoos_b200.train] iter {it}: total_loss {tot:.4f} lr_factor {lr_factor(it, args.max_iters, args.scheduler, args.scheduler_extra):.3g} scale {history[-1]['scale']:.0f}", flush=True)
         # EvalHook.after_step (trainer/hooks/hook.py:539-545): every eval_period iterations; the one after the last iteration is the final evaluation
         if data_val is not None and args.eval_period > 0 and (it + 1) % args.eval_period == 0 and it + 1 != args.max_iters:
-            history.append({"iter": it, "val_metrics": _evaluate_while_training(fm, data_val, args.batch_size, dev)})
+            history.append({"iter": it, "val_metrics": _evaluate_while_training(fm, data_val, args.batch_size, dev, ema)})
+    if ema is not None:  # _store_model (trainer.py:367-375): the final evaluation and model_final.pth see the averaged weights
+        ema.apply()
     metrics = None
     if data_val is not None:  # every rank evaluates its shard; rank 0 gets the metrics of all of data_val
         metrics = _evaluate_while_training(fm, data_val, args.batch_size, dev)
@@ -164,12 +175,14 @@ def _train_worker(rank: int, world: int, fm, args: TrainerArgs, data_train, data
         dist.destroy_process_group()
 
 
-def _evaluate_while_training(fm, data_val, batch_size: int, dev) -> dict:
+def _evaluate_while_training(fm, data_val, batch_size: int, dev, ema=None) -> dict:
     """inference_on_dataset between training iterations, leaving training as it was: no gradients flow (no_grad), the parameters, optimiser state and
     BatchNorm running statistics are only read (the eval forward packs its own copy of the weights), the global RNG state is restored, and the model
-    returns to train mode.  {} on ranks other than 0."""
+    returns to train mode.  With a ModelEMA the model holds the averaged weights during the evaluation and its training values again after it
+    (apply_model_ema_and_restore, trainer.py:447-452); the eval engine is packed afresh from them, as model.eval() drops the packed one.
+    {} on ranks other than 0."""
     model = fm.model
-    with torch.random.fork_rng(devices=[dev] if dev.type == "cuda" else []):
+    with torch.random.fork_rng(devices=[dev] if dev.type == "cuda" else []), (ema.applied() if ema is not None else contextlib.nullcontext()):
         model.eval()
         try:
             return inference_on_dataset(fm, data_val, batch_size=batch_size)

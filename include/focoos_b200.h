@@ -358,6 +358,14 @@ int fb200_optim_finalize(const void* workspace, float* ctrl, float max_norm, int
 int fb200_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const int64_t* chunk_start, const int* chunk_len,
                      const int* chunk_seg, int nchunks, const float* seg_lr, const float* seg_wd, const int* seg_active, float lr_factor,
                      float one_minus_beta1, float one_minus_beta2, float eps, const float* ctrl, void* stream);
+/* Model EMA update (focoos/trainer/solver/ema.py:112-140), one launch: ema[i] = fma(one_minus_decay, params[i], ema[i] * decay) over the
+ * n-element arena laid out like the flat parameter buffer (n a multiple of 4, both 16-byte aligned), the bit-exact result of
+ * torch._foreach_mul_ + torch._foreach_add_(alpha) on the device; plus `nchunks` rows of `chunks` (int64 [nchunks][4]: source address,
+ * EMA address, element count, kind) for the entries outside that buffer: kind 0 = fp32 as above, kind 1 = int64 as
+ * trunc(fp32(ema) * decay + fp32(src) * one_minus_decay) with fp32 products and sum.  decay and 1 - decay are formed in double by the caller
+ * and rounded to fp32.  The loss scaler's found-inf flag is not read: the EMA follows the weights on skipped steps too. */
+int fb200_ema_update(float* ema, const float* params, int64_t n, const int64_t* chunks, int nchunks, float decay, float one_minus_decay,
+                     void* stream);
 
 /* ---- backward / training-mode kernels (SURVEY 8 a21: what autograd executes under TrainerLoop.run_step, trainer/trainer.py:757) ----
  * fp32, NHWC, caller-owned workspaces.  Each replaces the aten backward of the torch call the reference makes at the cited site. */

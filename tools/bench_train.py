@@ -18,12 +18,13 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from focoos_b200 import DETRConfig, FAIDetr, ops  # noqa: E402
 from focoos_b200 import distributed as D  # noqa: E402
 from focoos_b200.criterion import DETRTargets  # noqa: E402
-from focoos_b200.train_step import FlatAdamW, GradBucketReducer, TrainStep, get_optimizer_params  # noqa: E402
+from focoos_b200.train_step import FlatAdamW, GradBucketReducer, ModelEMA, TrainStep, get_optimizer_params  # noqa: E402
 from focoos_b200.utils.seeded_weights import desaturate_classifiers, seeded_state_dict  # noqa: E402
 
 
-def run_leg(batch=16, size=640, steps=5, warmup=2, precision="fp32_tc", by_symbol=True, sync_bn=None):
-    """One fine-tune leg on the ALREADY-INITIALISED process group (every rank calls it); returns the result dict on every rank."""
+def run_leg(batch=16, size=640, steps=5, warmup=2, precision="fp32_tc", by_symbol=True, sync_bn=None, ema=False):
+    """One fine-tune leg on the ALREADY-INITIALISED process group (every rank calls it); returns the result dict on every rank.  ema: with the model EMA
+    (TrainerArgs.ema_enabled defaults: decay 0.999, warmup 2000) updated after every step."""
     rank, local, world = int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     dev = torch.device("cuda", local)
     cfg = DETRConfig(num_classes=80)
@@ -37,7 +38,7 @@ def run_leg(batch=16, size=640, steps=5, warmup=2, precision="fp32_tc", by_symbo
     opt.track_unused_parameters()
     red = GradBucketReducer(opt)
     red.attach_hooks()
-    step = TrainStep(m, opt, red)
+    step = TrainStep(m, opt, red, ModelEMA(m, opt) if ema else None)
     g = torch.Generator().manual_seed(4 + rank)  # SURVEY 8(d).5: seed 4 + rank
     x = torch.randint(0, 256, (batch, 3, size, size), generator=g).float().to(dev)
     targets = []
@@ -97,7 +98,7 @@ def run_leg(batch=16, size=640, steps=5, warmup=2, precision="fp32_tc", by_symbo
                                                                       "amp": "ONE f16 wgmma product (fp16-rounded operands, f32 accumulation) for conv/linear forward, data and weight gradients - the reference's torch.autocast(fp16) + GradScaler arithmetic (trainer/trainer.py:735)"}[precision],
            "precision": precision,
            "config": {"workload": f"fai-detr-l (80 classes) bs={batch}/GPU {size}x{size} synthetic COCO-shape targets (BASELINE configs[4])", "global_batch": batch * world,
-                      "sync_bn": bool(getattr(m, "sync_bn", False)) and world > 1},
+                      "sync_bn": bool(getattr(m, "sync_bn", False)) and world > 1, "ema": bool(ema)},
            "kernel_launches_per_step": launches, "phases_ms": phases, "peak_mem_GB": torch.cuda.max_memory_allocated() / 1e9, "loss_total": total, "optimizer": opt.stats(), "by_symbol": by_sym}
     red.detach_hooks() if hasattr(red, "detach_hooks") else None
     del step, red, opt, m, x, targets
@@ -113,11 +114,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--precision", default="fp32_tc", choices=["fp32", "fp32_tc", "amp"])
     ap.add_argument("--no-sync-bn", action="store_true")
+    ap.add_argument("--ema", action="store_true")
     args = ap.parse_args()
     rank, local, world = int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     torch.cuda.set_device(local)
     D.init_from_env("nccl", torch.device("cuda", local))
-    res = run_leg(args.batch, args.size, args.steps, args.warmup, args.precision, sync_bn=False if args.no_sync_bn else None)
+    res = run_leg(args.batch, args.size, args.steps, args.warmup, args.precision, sync_bn=False if args.no_sync_bn else None, ema=args.ema)
     if rank == 0:
         print(json.dumps(res))
     if world > 1:
