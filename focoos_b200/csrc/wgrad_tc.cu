@@ -10,7 +10,8 @@
 //   transposed (MN-major).  The X box is the dY box shifted by the tap offset; out-of-bounds rows/columns (conv zero padding, ragged
 //   pixel tiles) are zero-filled by the TMA unit for BOTH operands, so ragged tiles contribute exact zeros.
 // fp32 accuracy: operands are the [hi | lo] fp16 pairs of the fp32 tensors (fb200_split_f32_pair); each 64-pixel K chunk issues
-//   dY_hi*X_hi + dY_hi*X_lo + dY_lo*X_hi  into the same fp32 register accumulator (error ~2^-21 relative, like the forward mode).
+//   dY_hi*X_hi + dY_hi*X_lo + dY_lo*X_hi  into one fp32 register accumulator per chunk, and the chunks are added in fp32 (round to nearest)
+//   (error ~2^-21 relative, like the forward mode).
 // Parallelism: work item = (128 x BLOCK_N weight tile, tap, pixel split); persistent CTAs, warp-specialised (one TMA producer thread,
 //   two consumer warp-groups that each own 64 output channels of the tile), 3-stage smem ring;
 //   split partials are reduced in a fixed order by wgrad_reduce_kernel (reproducible, no atomics).
@@ -120,14 +121,16 @@ __global__ void __launch_bounds__(384, 1) wgrad_tc_kernel(const __grid_constant_
   const int g = ct >> 7;
   const int row = g * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2);  // accumulator rows row and row + 8
   const int cq = 2 * (lane & 3);
-  float acc[BLOCK_N / 2];
+  // The wgmma accumulator does not round its additions to nearest: summed in it over a whole split (up to ~10^4 chunks for the stem's 1.6 M-pixel
+  // weight gradients), products of one sign drift by many ulps.  So each 64-pixel chunk is summed in `acc` alone and added to `tot` with an fp32
+  // (round-to-nearest) add; the drift stays that of one chunk's 4 (single) or 12 (split) products per element.
+  float acc[BLOCK_N / 2], tot[BLOCK_N / 2];
   int stage = 0;
   uint32_t phase = 0;
   for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
     int mt, nt, tap, split;
     decode(item, mt, nt, tap, split);
     const int pt_begin = split * p.pt_per_split, pt_end = min(p.pt_total, pt_begin + p.pt_per_split);
-    int prev = -1;
     for (int pt = pt_begin; pt < pt_end; ++pt) {
       mbar_wait(&full_bar[stage], phase);
       const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + (uint32_t)(g * BOX_BYTES), sb = smem_u32(smem + stage * STAGE_BYTES) + A_BOXES * BOX_BYTES;
@@ -137,20 +140,22 @@ __global__ void __launch_bounds__(384, 1) wgrad_tc_kernel(const __grid_constant_
 #pragma unroll
       for (int k = 0; k < BLOCK_K / 16; ++k) {  // 16 pixels = two 8-pixel groups = 2048 B: +128 in 16-byte units
         const uint64_t adv = (uint64_t)(k * 128);
-        Wgmma<BLOCK_N, 1>::mma(acc, a_hi + adv, b_hi + adv, (pt > pt_begin || k > 0) ? 1u : 0u);
+        Wgmma<BLOCK_N, 1>::mma(acc, a_hi + adv, b_hi + adv, k > 0 ? 1u : 0u);
         if (!p.single) {
           Wgmma<BLOCK_N, 1>::mma(acc, a_hi + adv, b_lo + adv, 1u);
           Wgmma<BLOCK_N, 1>::mma(acc, a_lo + adv, b_hi + adv, 1u);
         }
       }
       wgmma_commit();
-      wgmma_wait<1>();  // the previous chunk's products are done: its stage may be refilled
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
+      wgmma_wait<0>();  // this chunk's products are done: its stage may be refilled (the producer keeps the next stages loaded meanwhile)
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) {
+        asm volatile("" : "+f"(acc[i])::"memory");  // read acc only after the wait above (it carries no register dependence on the async products)
+        tot[i] = pt > pt_begin ? tot[i] + acc[i] : acc[i];
+      }
     }
-    wgmma_wait<0>();
-    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
     // registers -> split partial in global memory (Cin % 8 == 0: a column pair never straddles the end of a row)
     const int n0 = nt * BLOCK_N;
 #pragma unroll
@@ -161,7 +166,7 @@ __global__ void __launch_bounds__(384, 1) wgrad_tc_kernel(const __grid_constant_
 #pragma unroll
       for (int j = 0; j < BLOCK_N / 8; ++j) {
         const int c = 8 * j + cq;
-        if (n0 + c < p.Cin) *reinterpret_cast<float2*>(dst + c) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        if (n0 + c < p.Cin) *reinterpret_cast<float2*>(dst + c) = make_float2(tot[4 * j + 2 * h], tot[4 * j + 2 * h + 1]);
       }
     }
   }

@@ -15,6 +15,33 @@ bits flipping on 1e-5 differences) does not reach the comparison, and the bars s
 
 Check 3 allows the tie: hi = fp16(v), lo = fp16(v - hi) can round lo up to exactly half an fp16 ulp of hi, and fp16(hi + lo) then rounds to even, away
 from hi, for about one element in 6000.  That is a correct split, so "hi == fp16(hi + lo)" alone would reject it.
+
+The backward operators of the fine-tune step are wrapped the same way: conv_wgrad, conv_wgrad_tc, conv_wgrad_tc_f16, dilate2, colsum and add_act.  Before
+each of these launches the output is filled with NaN, so an element the kernel never writes, or a kernel that adds onto `dw` although the call passes
+accumulate = 0, fails check 1.
+  * weight gradient  dW[co,kh,kw,ci] = sum over the K = B*Ho*Wo output pixels of dy * x, against fp64 of the operand values the launch received (the
+    fp32 tensors; hi + lo of both [hi | lo] pairs; the fp16 values of the amp operands).  A = the same sum over |x| * |dy|.  The split products omit
+    lo x dy_lo (LOLO); the fp16 products are exact in fp32, so only the accumulation term remains.  With K up to 1.6 M (the 32-channel convs of the
+    stem at bs=16, 640x640) the per-element bar is C_ACC * sqrt(K) * u32 ~ 3e-4 of A, far above a dropped hi x dy_lo product (each term 2^-11 of its
+    product).  The per-launch bar (C_AGG + LOLO) ~ 16 u32 of ||A|| is what sees it: the dropped terms carry the rounding residual of dy, whose sign is
+    unrelated to the product's, so they add up as a random walk to ~2^-12 * sqrt(K) * rms(dy x) per element - above 16 u32 * A ~ 16 u32 * K * mean|dy x|
+    while K stays below ~10^5 (every launch of a small step; at bs=16 the weight gradients of the deep stages, not the 1.6 M-pixel stem convs).
+  * dilate2          exact: dy at the even (h, w), zeros elsewhere.
+  * colsum           fp32 sum of K = R rows: A = the column sum of |x|.
+  * add_act          forward act(a + b), or the gradient dy * act'(a + b).  a + b is one fp32 rounding and exact in fp64, so the forward sum (no
+                     activation) and ReLU equal fp32(a + b) exactly, and the pass-through gradient and the ReLU gradient gate (the sign of the
+                     rounded sum is the sign of the exact one) equal dy exactly.  The smooth activations (u = u32, z = a + b):
+      forward        the rounding of z moves the result by at most LIP * u * |z|; GELU = z/2 * (1 + erf(z / sqrt 2)) adds erff's 2 ulp (<= 2u, the values
+                     are below 1) and the two roundings of its argument (slope of erf times 2u|t| <= 1u) to 1 + erf, i.e. <= 1.5 u |z| after the
+                     product with z/2, and two roundings of the result; SiLU = z / (1 + expf(-z)) has expf's 2 ulp, the sum and the quotient, all
+                     relative to the result (<= 6 u |y|, and |y| <= |z|):  bound = (LIP + C_OUT) * u * |z| + C_OUT * u * |y64|
+      GELU gradient  act' = Phi(z) + z phi(z): Phi through erff as above (<= 2u), z phi(z) <= 0.25 with expf's 2 ulp, the argument -z^2/2 (relative
+                     z^2 u, <= 0.5u absolute after the factor z phi(z)) and two products (<= 2u); the rounding of z (|z act''(z)| <= 0.4, 0.4u); the sum
+                     (1.13u): <= 6u in all, so  bound = 2 * C_OUT * u * |dy| + C_OUT * u * |g64|
+      SiLU gradient  act' = s (1 + z (1 - s)), s = 1 / (1 + expf(-z)) rounded to <= 2u absolute, which 1 - s carries unchanged and z multiplies:
+                     bound = 2 * C_OUT * u * (1 + |z|) * |dy| + C_OUT * u * |g64|
+    An element-wise launch has no accumulation to average over, so its per-launch bar is the norm of the per-element bar.
+"Exact" compares values: +0 and -0 are equal (a ReLU gradient dy * 0 is -0 for a negative dy).
 """
 from __future__ import annotations
 
@@ -25,6 +52,7 @@ import sys
 import torch
 import torch.nn.functional as F
 
+from focoos_b200 import ops
 from focoos_b200.ops import Pair
 
 # ---- the bounds, from unit roundoff ------------------------------------------------------------------------------------------------------------------
@@ -42,14 +70,28 @@ LOLO = {"fp32": 0.0, "fp16": 0.0, "split": 2.0 ** -22}
 # output format: (relative, absolute) rounding of the stored result.  fp16 rounds to 2^-11 |y|; a Pair keeps v - hi to 2^-11, i.e. 2^-22 |y|.  Both
 # lose up to half the smallest fp16 subnormal (2^-25) where the value (fp16) or v - hi (Pair) falls below 2^-14.
 FMT = {"fp32": (0.0, 0.0), "fp16": (2.0 ** -11, 2.0 ** -25), "pair": (2.0 ** -22, 2.0 ** -25)}
+# tensor-core products of fp16 operands (split and fp16 arithmetic) have an absolute floor: a product of two fp16 values is a multiple of 2^-48, and the
+# wgmma sums lose products near that scale.  Measured on the fine-tune step's linear data gradients (K = 256, outputs ~1e-8 where dy lies at the fp16
+# underflow): errors up to 2^-40.4 against fp64 of the same fp16 operands, in elements whose bar without this term was 2^-42.  Per element: K * 2^-48
+# (1e-12 at K = 256), nothing next to the bars of outputs of ordinary magnitude.
+TC_ABS = {"split": 2.0 ** -48, "fp16": 2.0 ** -48}
+
+
+_TORCH_DIR = os.path.dirname(torch.__file__) + os.sep
 
 
 def _site():
-    """file:function:line of the model code that made the launch: the first frame outside the operator layer, this module and the engines' generic
-    layer calls (_conv / _linear)"""
+    """file:function:line of the model code that made the launch: the first frame outside the operator layer, this module, the autograd functions
+    (autograd_ops.py), torch itself and the engines' generic layer calls (_conv / _linear).  A backward launch is made by the autograd engine, not by the
+    model, so it is named by the autograd function's backward line (autograd_ops.py:Conv2dFn.backward:137)."""
     f = sys._getframe(2)
-    skip = (os.sep + "ops.py", os.sep + "conv_launch_check.py")
-    while f is not None and (f.f_code.co_filename.endswith(skip) or f.f_code.co_name in ("_conv", "_linear")):
+    skip = (os.sep + "ops.py", os.sep + "conv_launch_check.py", os.sep + "autograd_ops.py")
+    while f is not None:
+        fn = f.f_code.co_filename
+        if fn.endswith(os.sep + "autograd_ops.py") and f.f_code.co_name == "backward":
+            return f"autograd_ops.py:{f.f_code.co_qualname}:{f.f_lineno}"
+        if not (fn.endswith(skip) or fn.startswith(_TORCH_DIR) or f.f_code.co_name in ("_conv", "_linear")):
+            break
         f = f.f_back
     if f is None:
         return "?"
@@ -137,12 +179,41 @@ def _magnitude(za, s, b, r):
     return a if r is None else a + r.abs()
 
 
-def _bounds(A, y64, K, arith, fmt):
+def _bounds(A, y64, K, arith, fmt, lip=LIP):
     rel, ab = FMT[fmt]
     tail = (C_OUT * U32 + rel) * y64.abs() + ab
-    elem = LIP * ((C_ACC * math.sqrt(K) + C_EPI) * U32 + LOLO[arith]) * A + tail
-    agg = LIP * ((C_AGG + C_EPI) * U32 + LOLO[arith]) * A + tail
+    elem = lip * ((C_ACC * math.sqrt(K) + C_EPI) * U32 + LOLO[arith]) * A + tail + K * TC_ABS.get(arith, 0.0)
+    agg = lip * ((C_AGG + C_EPI) * U32 + LOLO[arith]) * A + tail
     return elem, agg
+
+
+def _wgrad64(x64, dy64, KH, KW, stride, pad):
+    """fp64 weight gradient [Cout,KH,KW,Cin] of an NHWC conv: one GEMM dy^T @ x per filter tap, over the tap's shifted (and, for stride 2,
+    element-strided) view of the zero-padded input"""
+    B, Ho, Wo, Cout = dy64.shape
+    Cin = x64.shape[-1]
+    d = dy64.reshape(-1, Cout).t()
+    if KH == 1 and KW == 1 and stride == 1 and pad == 0:
+        return (d @ x64.reshape(-1, Cin)).reshape(Cout, 1, 1, Cin)
+    xp = F.pad(x64, (0, 0, pad, pad, pad, pad))
+    dw = torch.empty((Cout, KH, KW, Cin), dtype=torch.float64, device=x64.device)
+    for kh in range(KH):
+        for kw in range(KW):
+            xs = xp[:, kh:kh + stride * (Ho - 1) + 1:stride, kw:kw + stride * (Wo - 1) + 1:stride, :]
+            dw[:, kh, kw, :] = d @ xs.reshape(-1, Cin)
+    return dw
+
+
+def _pair64(t, C):
+    """fp64 values of a dense [hi | lo] fp16 pair tensor [..., 2C]"""
+    return t[..., :C].double() + t[..., C:2 * C].double()
+
+
+def _stem_wgrad(x_shape, Cout, KH, stride, pad):
+    """fb200_conv_wgrad runs the stem's weight gradient (3x3 stride 2, at most 4 input channels, 32 outputs) on its dedicated kernel.  This is the
+    dispatch condition of fb200_conv_wgrad (csrc/bwd_conv_norm.cu) and must change with it; its other clause, that the workspace holds one partial per
+    block, always holds: fb200_conv_wgrad_workspace_bytes sizes the workspace for 2 * kNumSMs partials."""
+    return KH == 3 and stride == 2 and pad == 1 and x_shape[-1] <= 4 and Cout == 32
 
 
 class LaunchCheckError(AssertionError):
@@ -152,13 +223,13 @@ class LaunchCheckError(AssertionError):
 class CheckingBackend:
     """ops backend wrapper: every conv / linear launch checked against fp64 of its own operands (see the module docstring)"""
 
-    def __init__(self, inner, label: str = ""):
+    def __init__(self, inner, label: str = "", mode: str = ""):
         self.inner = inner
-        self.begin(label)
+        self.begin(label, mode)
 
-    def begin(self, label: str):
-        """start a new run (a model, a size, a precision): launch indices count from 0 again"""
-        self.label, self.index, self.rows, self.failures = label, 0, [], []
+    def begin(self, label: str, mode: str = ""):
+        """start a new run (a model, a size, a precision): launch indices count from 0 again; `mode` (a training arithmetic) is copied into every row"""
+        self.label, self.mode, self.index, self.rows, self.failures = label, mode, 0, [], []
 
     def __getattr__(self, name):
         return getattr(self.inner, name)
@@ -211,7 +282,85 @@ class CheckingBackend:
         geom = dict(op="linear_rowmax_pair", M=x64.shape[0], Cin=K, Cout=w3.shape[0], K=K, fmt="fp32")
         self._launch(geom, "split", [xp, w3, bias], out, lambda: self.inner.linear_rowmax_pair(xp, w3, bias, out), lambda: self._rowmax_ref(x64, w64, bias, prev))
 
+    # ---- the backward operators of the fine-tune step ----------------------------------------------------------------------------------------------
+    def conv_wgrad(self, x, dy, KH, KW, stride, pad, dw):
+        x64, dy64 = x.double(), dy.double()
+        geom = self._wgrad_geom("conv_wgrad", x.shape, dy.shape, KH, stride, "stem" if _stem_wgrad(x.shape, dy.shape[-1], KH, stride, pad) else "simt")
+        self._launch(geom, "fp32", [x, dy], dw, self._filled(dw, lambda: self.inner.conv_wgrad(x, dy, KH, KW, stride, pad, dw)),
+                     lambda: self._wgrad_ref(x64, dy64, KH, KW, stride, pad, "fp32"))
+
+    def conv_wgrad_tc(self, x_pair, dy_pair, KH, KW, stride, pad, dw):
+        Cin, Cout = x_pair.shape[-1] // 2, dy_pair.shape[-1] // 2
+        x64, dy64 = _pair64(x_pair, Cin), _pair64(dy_pair, Cout)
+        geom = self._wgrad_geom("conv_wgrad_tc", x64.shape, dy64.shape, KH, stride, "split")
+        self._launch(geom, "split", [x_pair, dy_pair], dw, self._filled(dw, lambda: self.inner.conv_wgrad_tc(x_pair, dy_pair, KH, KW, stride, pad, dw)),
+                     lambda: self._wgrad_ref(x64, dy64, KH, KW, stride, pad, "split"))
+
+    def conv_wgrad_tc_f16(self, x16, dy16, KH, KW, stride, pad, dw):
+        x64, dy64 = x16.double(), dy16.double()
+        geom = self._wgrad_geom("conv_wgrad_tc_f16", x16.shape, dy16.shape, KH, stride, "f16")
+        self._launch(geom, "fp16", [x16, dy16], dw, self._filled(dw, lambda: self.inner.conv_wgrad_tc_f16(x16, dy16, KH, KW, stride, pad, dw)),
+                     lambda: self._wgrad_ref(x64, dy64, KH, KW, stride, pad, "fp16"))
+
+    def dilate2(self, dy, out):
+        dy64 = dy.double()
+        B, Ho, Wo, C = dy.shape
+        geom = dict(op="dilate2", fmt="fp32", B=B, H=Ho, W=Wo, Cin=C, Cout=C, Ho=out.shape[1], Wo=out.shape[2], K=1, odd_map=bool(out.shape[1] % 2 or out.shape[2] % 2))
+
+        def ref():
+            y = torch.zeros(out.shape, dtype=torch.float64, device=out.device)
+            y[:, 0:2 * Ho:2, 0:2 * Wo:2] = dy64
+            return y, torch.zeros_like(y), torch.zeros_like(y)
+        self._launch(geom, "exact", [dy], out, self._filled(out, lambda: self.inner.dilate2(dy, out)), ref)
+
+    def colsum(self, x2d, out):
+        x64 = x2d.double()
+        geom = dict(op="colsum", fmt="fp32", M=x2d.shape[0], Cout=x2d.shape[1], K=x2d.shape[0])
+
+        def ref():
+            y, A = x64.sum(0), x64.abs().sum(0)
+            return (y, *_bounds(A, y, x64.shape[0], "fp32", "fp32", lip=1.0), A)
+        self._launch(geom, "fp32", [x2d], out, self._filled(out, lambda: self.inner.colsum(x2d, out)), ref)
+
+    def add_act(self, a, b, dy, act, out):
+        z64 = a.double() if b is None else a.double() + b.double()
+        dy64 = None if dy is None else dy.double()
+        geom = dict(op="add_act", fmt="fp32", act=act, grad=dy is not None, M=a.numel(), Cout=a.shape[-1], K=1, sum=b is not None)
+        exact = act in (ops.ACT_NONE, ops.ACT_RELU)
+        self._launch(geom, "exact" if exact else "fp32", [a, b, dy], out, self._filled(out, lambda: self.inner.add_act(a, b, dy, act, out)),
+                     lambda: self._add_act_ref(z64, dy64, act))
+
     # ---- references ---------------------------------------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _wgrad_ref(x64, dy64, KH, KW, stride, pad, arith):
+        y = _wgrad64(x64, dy64, KH, KW, stride, pad)
+        A = _wgrad64(x64.abs(), dy64.abs(), KH, KW, stride, pad)
+        return (y, *_bounds(A, y, dy64.shape[0] * dy64.shape[1] * dy64.shape[2], arith, "fp32", lip=1.0), A)
+
+    @staticmethod
+    def _add_act_ref(z, dy, act):
+        """the result and its bounds (module docstring): exact for no activation and ReLU, unit-roundoff bounds for SiLU and GELU"""
+        if dy is None:
+            if act in (ops.ACT_NONE, ops.ACT_RELU):  # the correctly rounded fp32 sum (fp64 holds a + b exactly, so rounding it once more is that)
+                y = _act64(z.float().double(), act)
+                return y, torch.zeros_like(y), torch.zeros_like(y)
+            y = _act64(z, act)
+            elem = (LIP + C_OUT) * U32 * z.abs() + C_OUT * U32 * y.abs()
+            return y, elem, elem
+        if act == ops.ACT_NONE:
+            return dy.clone(), torch.zeros_like(dy), torch.zeros_like(dy)
+        if act == ops.ACT_RELU:
+            return dy * (z > 0).double(), torch.zeros_like(dy), torch.zeros_like(dy)
+        if act == ops.ACT_SILU:
+            s = torch.sigmoid(z)
+            g = dy * s * (1.0 + z * (1.0 - s))
+            elem = 2 * C_OUT * U32 * (1.0 + z.abs()) * dy.abs() + C_OUT * U32 * g.abs()
+        else:
+            assert act == ops.ACT_GELU, f"unknown activation {act}"
+            g = dy * (0.5 * (1.0 + torch.erf(z / math.sqrt(2.0))) + z * torch.exp(-0.5 * z * z) / math.sqrt(2.0 * math.pi))
+            elem = 2 * C_OUT * U32 * dy.abs() + C_OUT * U32 * g.abs()
+        return g, elem, elem
+
     @staticmethod
     def _conv_ref(x64, w64, scale, bias, stride, pad, act, r64, groups=1):
         s = None if scale is None else scale.double()
@@ -231,6 +380,21 @@ class CheckingBackend:
         return torch.maximum(prev, z.max(-1).values), za.max(-1).values
 
     # ---- the launch and its checks -------------------------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _filled(out, call):
+        """the launch, with its fp32 output filled with the NaN sentinel first (an element left unwritten, or added onto, stays NaN)"""
+        def run():
+            out.fill_(float("nan"))
+            call()
+        return run
+
+    @staticmethod
+    def _wgrad_geom(op, xshape, dyshape, k, stride, kernel):
+        B, H, W, Cin = xshape
+        _, Ho, Wo, Cout = dyshape
+        return dict(op=op, fmt="fp32", kernel=kernel, B=B, H=H, W=W, Cin=Cin, Cout=Cout, k=k, stride=stride, K=B * Ho * Wo, Ho=Ho, Wo=Wo,
+                    odd_map=bool(H % 2 or W % 2), linear=(k == 1 and B == 1 and H == 1))
+
     @staticmethod
     def _geom(op, xshape, w, stride, act, residual, out):
         B, H, W, Cin = xshape
@@ -263,18 +427,20 @@ class CheckingBackend:
         call()
         if flat.is_cuda:
             torch.cuda.synchronize()
-        y64, A = ref()
+        r = ref()  # (y64, A), or (y64, per-element bound, per-launch bound[, A]) for an operator with bounds of its own
+        y64, (elem, agg) = r[0], (r[1:3] if len(r) >= 3 else _bounds(r[1], r[0], geom["K"], arith, geom["fmt"]))
+        A = r[1] if len(r) == 2 else (r[3] if len(r) == 4 else None)
         y = _val64(out)
         fails = []
         # 1 / 2: per element and per launch
-        elem, agg = _bounds(A, y64, geom["K"], arith, geom["fmt"])
         err = (y - y64).abs()
         bad = ~(err <= elem)  # NaN counts as a failure
         ratio = torch.where(err == 0, torch.zeros_like(err), err / elem)
         ratio = torch.where(torch.isnan(ratio), torch.full_like(err, float("inf")), ratio)
         worst = int(ratio.reshape(-1).argmax()) if ratio.numel() else 0
         elem_ratio = float(ratio.reshape(-1)[worst]) if ratio.numel() else 0.0
-        en, an, bn = float(torch.linalg.vector_norm(err)), float(torch.linalg.vector_norm(A)), float(torch.linalg.vector_norm(agg))
+        en, bn = float(torch.linalg.vector_norm(err)), float(torch.linalg.vector_norm(agg))
+        an = float(torch.linalg.vector_norm(A)) if A is not None else 0.0
         agg_ratio = en / bn if bn > 0 else (0.0 if en == 0 else float("inf"))
         if math.isnan(agg_ratio):
             agg_ratio = float("inf")
@@ -283,7 +449,7 @@ class CheckingBackend:
             fails.append(f"element {at}: y={float(y.reshape(-1)[worst]):.9g} ref={float(y64.reshape(-1)[worst]):.9g} err={float(err.reshape(-1)[worst]):.3e} "
                          f"bound={float(elem.reshape(-1)[worst]):.3e} ({int(bad.sum())} of {bad.numel()} elements over)")
         if not agg_ratio <= 1.0:
-            fails.append(f"aggregate ||y - y64|| = {en:.3e} over ||agg bound|| = {bn:.3e} (||A|| = {an:.3e})")
+            fails.append(f"aggregate ||y - y64|| = {en:.3e} over ||agg bound|| = {bn:.3e}" + (f" (||A|| = {an:.3e})" if A is not None else ""))
         # 3: a Pair output encodes its value
         if isinstance(out, Pair):
             hi, lo = out.hi, out.lo
@@ -304,7 +470,7 @@ class CheckingBackend:
                 continue
             if not torch.equal(_bits(v), _bits(v0)):
                 fails.append(f"an input of shape {tuple(v.shape)} changed")
-        row = dict(geom, label=self.label, index=idx, elem_ratio=elem_ratio, agg_ratio=agg_ratio, agg_rel_u32=(en / an / U32) if an > 0 else 0.0, ok=not fails)
+        row = dict(geom, label=self.label, mode=self.mode, index=idx, elem_ratio=elem_ratio, agg_ratio=agg_ratio, agg_rel_u32=(en / an / U32) if an > 0 else 0.0, ok=not fails)
         self.rows.append(row)
         for f in fails:
             self.failures.append(f"{self.label} launch #{idx} {_describe(geom)}: {f}")
@@ -316,6 +482,15 @@ class CheckingBackend:
 
 
 def _describe(g):
+    if g["op"].startswith("conv_wgrad"):
+        return (f"{g['op']} [{g['arith']}, {g['kernel']}] x {g['B']}x{g['H']}x{g['W']}x{g['Cin']} dy {g['Ho']}x{g['Wo']}x{g['Cout']} k{g['k']} s{g['stride']} "
+                f"K={g['K']} at {g['site']}")
+    if g["op"] == "dilate2":
+        return f"dilate2 {g['B']}x{g['H']}x{g['W']}x{g['Cin']} -> {g['Ho']}x{g['Wo']} at {g['site']}"
+    if g["op"] == "colsum":
+        return f"colsum [{g['arith']}] R={g['M']} C={g['Cout']} at {g['site']}"
+    if g["op"] == "add_act":
+        return f"add_act act {g['act']}{' gradient' if g['grad'] else ''}{' of a + b' if g['sum'] else ''} n={g['M']} at {g['site']}"
     if g["op"].startswith("linear_rowmax"):
         return f"{g['op']} [{g['arith']}] M={g['M']} K={g['K']} N={g['Cout']} at {g['site']}"
     return (f"{g['op']} [{g['arith']} -> {g['fmt']}] {g['B']}x{g['H']}x{g['W']}x{g['Cin']} -> {g['Ho']}x{g['Wo']}x{g['Cout']} k{g['k']} s{g['stride']} "
@@ -353,3 +528,32 @@ def summarize(rows):
         if r["agg_ratio"] >= cur[2]:
             cur[2], cur[3] = r["agg_ratio"], f"{r['label']} #{r['index']} {_describe(r)}"
     return out
+
+
+TRAIN_MODEL = "fai-detr-l-coco"
+
+
+def train_model(mode: str, device: str = "cpu"):
+    """fai-detr-l-coco with its seeded weights, classifiers desaturated as in the training goldens, in train mode with the training arithmetic `mode`
+    ("fp32", "fp32_tc" or "amp": the fp32_tc model with TrainerArgs.amp_enabled)"""
+    from focoos_b200.utils.seeded_weights import desaturate_classifiers
+
+    m = seeded_model(TRAIN_MODEL, "fp32" if mode == "fp32" else "fp32_tc", device)
+    m.load_state_dict(desaturate_classifiers(m.state_dict()), strict=True)
+    if mode == "amp":
+        m.train_precision = "amp"
+    m.train()
+    assert m.train_graph().prec == mode
+    return m
+
+
+def train_step(m, B: int, H: int, W: int, device: str = "cpu"):
+    """one TrainStep (forward, criterion, loss-scaled backward, clipped AdamW) on synthetic images and targets; returns the losses"""
+    from focoos_b200.criterion import DETRTargets
+    from focoos_b200.train_step import FlatAdamW, TrainStep, get_optimizer_params
+    from oracle.gen_golden_train import synth_targets
+
+    opt = FlatAdamW(get_optimizer_params(m, base_lr=1e-4, weight_decay=1e-4, weight_decay_norm=0.0, backbone_multiplier=0.1), clip_gradients=0.1, amp=True)
+    x = synth_batch(5, B, H, W, device)
+    targets = [DETRTargets(labels=t[0].to(device), boxes=t[1].to(device)) for t in synth_targets(6, B, m.config.num_classes)]
+    return TrainStep(m, opt)(x, targets)

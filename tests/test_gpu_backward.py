@@ -313,3 +313,30 @@ def test_stem_weight_gradient_kernel():
     close(yg, yr, "stem fwd")
     close(wg.grad, wr.grad, "stem dw")
     close(xg.grad, xr.grad, "stem dx")
+
+
+@pytest.mark.parametrize("kernel", ["split", "f16"])
+@pytest.mark.parametrize("signs", ["random", "same"])
+@pytest.mark.parametrize("B,H,W,Cin,Cout,k", [(1, 1, 900, 256, 80, 1), (1, 1, 4800, 256, 1024, 1), (16, 320, 320, 32, 64, 3)])
+def test_weight_gradient_long_same_sign_sums(B, H, W, Cin, Cout, k, signs, kernel):
+    """the tensor-core weight gradients at the fine-tune step's longest sums (the decoder linears over 300 * B rows; conv1_3 over 16 x 320 x 320
+    pixels, ~30 pixel splits of 53k pixels each) against fp64 of the operands they received, at the bars of tests/conv_launch_check.py.  Operands of one
+    sign (|x|, |dy|) make every product of a sum the same sign, as the correlated activations and gradients of a training step do: an accumulator whose
+    additions do not round to nearest then drifts in proportion to the number of additions into it (5x the per-launch bar over the 900-row linears and
+    2.7x the per-element bar over conv1_3 before each 64-pixel chunk got an accumulator of its own)."""
+    from tests.conv_launch_check import CheckingBackend
+
+    g = torch.Generator(device=DEV).manual_seed(3)
+    x = torch.randn((B, H, W, Cin), generator=g, device=DEV)
+    dy = torch.randn((B, H, W, Cout), generator=g, device=DEV) * 0.05
+    if signs == "same":
+        x, dy = x.abs(), dy.abs()
+    pad = (k - 1) // 2
+    assert ops._be().conv_wgrad_tc_supported(tuple(x.shape), tuple(dy.shape), k, k, 1, pad)
+    chk = CheckingBackend(ops.CudaBackend(), f"wgrad {kernel} {signs}")
+    dw = torch.empty((Cout, k, k, Cin), dtype=torch.float32, device=DEV)
+    if kernel == "f16":
+        chk.conv_wgrad_tc_f16(x.half(), dy.half(), k, k, 1, pad, dw)
+    else:
+        chk.conv_wgrad_tc(ops.split_pair(x), ops.split_pair(dy), k, k, 1, pad, dw)
+    chk.raise_failures()
